@@ -1,4 +1,4 @@
-"""Dense conv2d over libb3d's tcgen05 implicit-GEMM kernel (NHWC fp32 activations, tf32 tensor cores).
+"""Dense conv2d over libb3d's wgmma implicit-GEMM kernel (NHWC fp32 activations, tf32 tensor cores).
 
 Reference call sites: nn.Conv2d layers of /root/reference/code/models/gan.py (:57-65, :163-177, :294-302,
 :359, :364) — 3x3 / 1x1 / 5x5 stride 1 and 4x4 stride 2, zero padding along y only (x padding is explicit:
@@ -58,10 +58,8 @@ def conv2d_nhwc(x, weight, bias=None, pad_y=0, stride=1, leaky=1.0, wt=None, cin
     optr = ctypes.c_void_p(out.data_ptr() + 4 * pad_out * Cout)          # pixel (n, y, pad_out) of the padded buffer
     if pad_out and Cout % 4:
         raise B3DError("conv2d: pad_out needs Cout % 4 == 0")
-    wide_head = Wout >= 128 and N * Hout * (Wout // 128) >= 8 * 148 and not os.environ.get("B3D_THIN_HEAD_CUDA_CORES")
-    if _thin(Cout, Cin, kh, kw, stride) and not cin_major and not wide_head:
+    if _thin(Cout, Cin, kh, kw, stride) and not cin_major:
         # 1-4 output channels: fp32 CUDA-core reduction kernel (csrc/thin_kernels.cu), not a 64-wide MMA tile
-        # (wide heads — conv_final at 256 x 128 — take the row-window tensor-core kernel with N = 16 tiles instead)
         check(_conv_call(lib.b3d_conv2d_thin_fwd, ptr(x), ptr(wt), ptr(dev(bias, "bias") if bias is not None else None), optr, N, H, W,
                                       Cin, Hout, Wout, Cout, kh, kw, pad_y, x_crop, OW, Cout, float(leaky), stream_ptr(x)))
         if pad_out:
@@ -70,21 +68,9 @@ def conv2d_nhwc(x, weight, bias=None, pad_y=0, stride=1, leaky=1.0, wt=None, cin
     dy = [r - pad_y for r in range(kh) for _ in range(kw)]
     dx = [s + x_crop for _ in range(kh) for s in range(kw)]
     b = dev(bias, "bias") if bias is not None else None
-    # the halo-staged kernel wins on wide-N layers with enough tiles to fill the GPU twice; elsewhere the per-tap kernel
-    # (2 CTAs / SM) is as fast or faster (profiles/r1_conv_layers.md)
-    use_flat = stride == 1 and not cin_major and Cout > 64 and N * Hout * W >= 2 * 148 * 384 and not x_crop
-    if os.environ.get("B3D_CONV_FLAT"):
-        use_flat = stride == 1 and not cin_major and os.environ["B3D_CONV_FLAT"] == "1"
-    if use_flat:
-        # halo-staged kernel (tc_conv2.cu); falls through to the per-tap kernel when the halo does not fit in smem
-        rc = _conv_call(lib.b3d_conv2d_flat_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw,
-                                      _ints(dy), _ints(dx), Hout, OW, Cout, float(leaky), stream_ptr(x))
-        if rc != 0 and b"does not fit" not in lib.b3d_last_error():
-            check(rc)
-    if not use_flat or rc != 0:
-        check(_conv_call(lib.b3d_conv2d_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw, _ints(dy),
-                                  _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), int(cin_major), None, 0, None, 0, 0,
-                                  None, stream_ptr(x)))
+    check(_conv_call(lib.b3d_conv2d_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw, _ints(dy),
+                              _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), int(cin_major), None, 0, None, 0, 0,
+                              None, stream_ptr(x)))
     if pad_out:
         check(lib.b3d_wrap_x_inplace(ptr(out), N * Hout, Wout, Cout, pad_out, pad_mode, stream_ptr(x)))
     return out
@@ -153,7 +139,7 @@ def conv2d_wgrad_nhwc(dy_, x, kh, kw, pad_y=0, stride=1, x_crop=0):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# autograd: y = conv(x, w) + b on NHWC tensors; fprop / dgrad / wgrad all on the tcgen05 kernels
+# autograd: y = conv(x, w) + b on NHWC tensors; fprop / dgrad / wgrad all on the wgmma kernels
 # ------------------------------------------------------------------------------------------------------------------
 def _pad_last(t, mult):
     c = t.shape[-1]
@@ -231,7 +217,7 @@ _FOLD = os.environ.get("B3D_FOLD", "kh")
 
 
 def conv2d(x_nchw, weight, bias=None, pad_y=0, stride=1, leaky=1.0, pad_out=0, pad_mode=1, x_crop=0):
-    """Drop-in for F.conv2d(x, w, b, stride, padding=(pad_y, 0)) on logically-NCHW tensors: runs on the tcgen05
+    """Drop-in for F.conv2d(x, w, b, stride, padding=(pad_y, 0)) on logically-NCHW tensors: runs on the wgmma
     kernels over the channels-last storage (a no-copy view when x is already channels_last) and returns a
     logically-NCHW, channels-last tensor."""
     x = x_nchw.permute(0, 2, 3, 1)
@@ -321,31 +307,17 @@ class _ConvBanked(torch.autograd.Function):
         optr = ctypes.c_void_p(out.data_ptr() + 4 * pad_out * Cout)
         st = stream_ptr(x)
         thin = _thin(Cout, Cin, kh, kw, stride)
-        # wide thin heads (conv_final: 64 -> 3 at 256 x 128) go to the row-window tensor-core kernel with N = 16 tiles
-        thin_fwd = thin and not (Wout >= 128 and N * Hout * (Wout // 128) >= 8 * 148 and not os.environ.get("B3D_THIN_HEAD_CUDA_CORES"))
-        if thin_fwd:
+        if thin:
             check(_conv_call(lib.b3d_conv2d_thin_fwd, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh, kw, pad_y,
                              x_crop, OW, Cout, float(leaky), st))
         else:
             dy = [r - pad_y for r in range(kh) for _ in range(kw)]
             dx = [s + x_crop for _ in range(kh) for s in range(kw)]
-            use_flat = stride == 1 and Cout > 64 and N * Hout * W >= 2 * 148 * 384 and not x_crop and not fold_raw
-            if os.environ.get("B3D_CONV_FLAT"):
-                use_flat = stride == 1 and os.environ["B3D_CONV_FLAT"] == "1" and not fold_raw
-            if stats is not None:                 # the statistics epilogue lives in the persistent / row-window kernels
-                use_flat = False
-                if bias is not None or leaky != 1.0 or stride != 1:
-                    raise B3DError("banked conv: output statistics are taken before bias / activation (plain stride-1 convs only)")
-            rc = -1
-            if use_flat:
-                rc = _conv_call(lib.b3d_conv2d_flat_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw,
-                                _ints(dy), _ints(dx), Hout, OW, Cout, float(leaky), st)
-                if rc != 0 and b"does not fit" not in lib.b3d_last_error():
-                    check(rc)
-            if rc != 0:
-                check(_conv_call(lib.b3d_conv2d_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw,
-                                 _ints(dy), _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), 0, None, 0, ptr(stats),
-                                 fold_raw, fold_pad, None, st))
+            if stats is not None and (bias is not None or leaky != 1.0 or stride != 1):
+                raise B3DError("banked conv: output statistics are taken before bias / activation (plain stride-1 convs only)")
+            check(_conv_call(lib.b3d_conv2d_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw,
+                             _ints(dy), _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), 0, None, 0, ptr(stats),
+                             fold_raw, fold_pad, None, st))
         if pad_out:
             check(lib.b3d_wrap_x_inplace(ptr(out), N * Hout, Wout, Cout, pad_out, pad_mode, st))
         ctx.save_for_backward(x, out if (leaky != 1.0 or pad_out) else None)
@@ -488,12 +460,10 @@ def conv2d_banked(x_nchw, lw, pad_y=0, stride=1, leaky=1.0, pad_out=0, pad_mode=
     if lw.fold:
         Wout = x.shape[2] - lw.kw + 1
         need_wgrad = torch.is_grad_enabled() and lw.wf.requires_grad
-        if (lw.Cin == 8 and stride == 1 and not x_crop and Wout % 128 == 0 and x.shape[0] * x.shape[1] * (Wout // 128) >= 2 * 148
+        if (lw.Cin == 8 and stride == 1 and not x_crop and Wout % 128 == 0 and x.shape[0] * x.shape[1] * (Wout // 128) >= 2 * torch.cuda.get_device_properties(x.device).multi_processor_count
                 and not need_wgrad and not os.environ.get("B3D_FOLD_MATERIALIZE")):
             # 8-channel stems of wide images when no weight gradient is taken (generator step: the discriminator is frozen):
             # the forward kernel folds the kh rows on the fly (TMA boxes of 4 rows x 8 channels), no folded tensor is written.
-            # Same-box A/B inside the step graph: 41.21 ms with it, 41.45 ms with the materialised fold (B3D_FOLD_MATERIALIZE=1)
-            # — although a cold-cache ncu launch of the 32-byte-swizzle kernel alone looks slower than fold + conv.
             fold_raw = lw.kh
         else:
             from .ew import fold_rows

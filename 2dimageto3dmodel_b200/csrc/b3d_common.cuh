@@ -1,4 +1,4 @@
-// Shared helpers of libb3d (sm_100a).  Error plumbing for the C ABI, launch accounting,
+// Shared helpers of libb3d (sm_90a).  Error plumbing for the C ABI, launch accounting,
 // NaN-propagating clamps (torch.clamp semantics) and warp/block reductions.
 #pragma once
 #include <cuda_runtime.h>

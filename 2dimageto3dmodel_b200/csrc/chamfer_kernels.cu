@@ -1,4 +1,4 @@
-// Chamfer / pairwise nearest-neighbour kernel for sm_100a (BASELINE.json north star; the reference's only
+// Chamfer / pairwise nearest-neighbour kernel for sm_90a (BASELINE.json north star; the reference's only
 // pairwise-NN site is the mirror-vertex argmin of rendering/mesh_template.py:33-39).
 //
 // Shared-memory blocking over the candidate set: a CTA stages TILE candidates as float4 in shared memory

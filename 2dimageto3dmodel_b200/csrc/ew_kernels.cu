@@ -258,7 +258,6 @@ fold_rows_fwd_kernel(const float* __restrict__ x, float4* __restrict__ out, int 
         constexpr int U = 4;                                 // independent pixels in flight per thread
         if ((C & 3) == 0) {
             // C % 4 == 0: the four channels of a quad come from one image row (same r) -> one 16-byte load per output quad
-            // (streaming / evict-first stores were measured here and in cbn_act_fwd_rows: no difference on B200)
             for (int xb = px0; xb < W; xb += U * PPB) {
                 float4 v[U];
 #pragma unroll
@@ -313,7 +312,7 @@ fold_rows_bwd_kernel(const float* __restrict__ go, float* __restrict__ gx, int N
 
 int grid_for(long long n) {
     long long b = (n + NT - 1) / NT;
-    const long long cap = 148LL * 16;
+    const long long cap = 132LL * 16;
     return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 }  // namespace
@@ -352,7 +351,7 @@ int b3d_fold_rows_fwd(const float* x, float* out, int N, int H, int W, int C, in
     const int Hout = H + 2 * pad_y - kh + 1;
     B3D_REQUIRE(Cp / 4 <= NT, B3D_EINVAL, "b3d_fold_rows_fwd: Cp=%d too wide (max %d)", Cp, 4 * NT);
     const int rows = N * Hout;
-    fold_rows_fwd_kernel<<<rows < 148 * 16 ? rows : 148 * 16, NT, 0, (cudaStream_t)stream>>>(x, (float4*)out, N, H, W, C, Hout, Cp / 4,
+    fold_rows_fwd_kernel<<<rows < 132 * 16 ? rows : 132 * 16, NT, 0, (cudaStream_t)stream>>>(x, (float4*)out, N, H, W, C, Hout, Cp / 4,
                                                                                        kh, pad_y);
     B3D_LAUNCH_OK();
     return B3D_OK;
@@ -424,7 +423,7 @@ int b3d_pad_leaky_bias_bwd(const float* gout_pad, const float* y_pad, float* gy,
     B3D_CHECK_ALIGNED(gout_pad);
     B3D_CHECK_ALIGNED(y_pad);
     B3D_CHECK_ALIGNED(gy);
-    long long blocks = rows < 148LL * 16 ? rows : 148LL * 16;
+    long long blocks = rows < 132LL * 16 ? rows : 132LL * 16;
     const long long per = (rows + blocks - 1) / blocks;          // rows per block
     blocks = (rows + per - 1) / per;
     pad_leaky_bias_bwd_kernel<<<(int)blocks, NT, 0, (cudaStream_t)stream>>>((const float4*)gout_pad, (const float4*)y_pad, (float4*)gy,
@@ -509,7 +508,7 @@ extern "C" int b3d_bn_stats(const float* y, long long rows, int C, float eps, fl
     B3D_CUDA_OK(cudaMemsetAsync(workspace, 0, sizeof(double) * 2 * (size_t)C, st));
     const int ppb = NT / (C / 4);
     long long blocks = (rows + ppb - 1) / ppb;
-    if (blocks > 148 * 2) blocks = 148 * 2;                 // few blocks: every block ends with 2C same-address fp64 atomics
+    if (blocks > 132 * 2) blocks = 132 * 2;                 // few blocks: every block ends with 2C same-address fp64 atomics
     bn_stats_partial_kernel<<<(int)blocks, NT, 0, st>>>((const float4*)y, rows, C / 4, workspace);
     B3D_LAUNCH_OK();
     bn_stats_finish_kernel<<<(C + 127) / 128, 128, 0, st>>>(workspace, rows, C, eps, mean, invstd);
@@ -864,7 +863,7 @@ int b3d_cbn_act_fwd(const float* y, const float* scale, const float* shift, cons
     const long long total = (long long)N * up * H * (up * W + 2 * pad) * (C / 4);
     if (g.C4 <= NT && NT % g.C4 == 0 && (up == 1 || up == 2)) {
         const int rows = N * up * H;
-        cbn_act_fwd_rows_kernel<<<rows < 148 * 16 ? rows : 148 * 16, NT, 0, (cudaStream_t)stream>>>(
+        cbn_act_fwd_rows_kernel<<<rows < 132 * 16 ? rows : 132 * 16, NT, 0, (cudaStream_t)stream>>>(
             (const float4*)y, (const float4*)scale, (const float4*)shift, (const float4*)skip, (float4*)out, g);
     } else {
         cbn_act_fwd_kernel<<<grid_for(total), NT, 0, (cudaStream_t)stream>>>((const float4*)y, (const float4*)scale, (const float4*)shift,
@@ -890,7 +889,7 @@ int b3d_cbn_act_bwd1(const float* gout, const float* y, const float* scale, cons
     B3D_CUDA_OK(cudaMemset2DAsync(S2, sizeof(float) * (size_t)s_pitch, 0, sizeof(float) * (size_t)C, (size_t)N, st));
     CbnGeom g{N, H, W, C / 4, up, pad, skip_pitch, skip_off, slope, post_leaky};
     // enough CTAs to fill the GPU a few times, each with >= 1 row
-    int rows = (int)(((long long)N * H + 148 * 8 - 1) / (148 * 8));
+    int rows = (int)(((long long)N * H + 132 * 8 - 1) / (132 * 8));
     rows = rows < 1 ? 1 : rows;
     dim3 grid(b3d::ceil_div(H, rows), N);
     cbn_act_bwd1_kernel<<<grid, NT, 0, st>>>((const float4*)gout, (const float4*)y, (const float4*)scale, (const float4*)shift,
@@ -924,7 +923,7 @@ int b3d_bn_sums(const float* y, long long rows, int C, double* sums, void* strea
     B3D_CUDA_OK(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * (size_t)C, st));
     const int ppb = NT / (C / 4);
     long long blocks = (rows + ppb - 1) / ppb;
-    if (blocks > 148 * 2) blocks = 148 * 2;
+    if (blocks > 132 * 2) blocks = 132 * 2;
     bn_stats_partial_kernel<<<(int)blocks, NT, 0, st>>>((const float4*)y, rows, C / 4, sums);
     B3D_LAUNCH_OK();
     return B3D_OK;

@@ -1,5 +1,5 @@
-// FID evaluation path (SURVEY.md §8f rank 4: evaluate_fid, main.py:188-412; utils/fid.py; utils/inception.py) for sm_100a.
-// The Inception convolutions run on the tcgen05 kernels of tc_conv.cu (BatchNorm folded, ReLU in the epilogue, branch
+// FID evaluation path (SURVEY.md §8f rank 4: evaluate_fid, main.py:188-412; utils/fid.py; utils/inception.py) for sm_90a.
+// The Inception convolutions run on the wgmma kernels of tc_conv.cu (BatchNorm folded, ReLU in the epilogue, branch
 // outputs written straight into their channel slice of the concatenated tensor); this file holds the rest of the network
 // and the statistics:
 //   inception_input_kernel   utils/inception.py:123-131: bilinear resize to 299 x 299 (align_corners=False), 2x - 1,
@@ -120,7 +120,7 @@ fid_accumulate_kernel(const float* __restrict__ f, int n, int D, double* __restr
 
 inline int grid_for(size_t total) {
     const size_t b = (total + NT - 1) / NT;
-    return (int)(b < 148 * 16 ? (b ? b : 1) : 148 * 16);
+    return (int)(b < 132 * 16 ? (b ? b : 1) : 132 * 16);
 }
 
 }  // namespace

@@ -1,4 +1,4 @@
-// Loss kernels of the mesh path (SURVEY.md §8 row a12) for sm_100a.
+// Loss kernels of the mesh path (SURVEY.md §8 row a12) for sm_90a.
 //   flat_loss_*      loss_flat (utils/losses.py:5-17): neighbour-face normal cosine regulariser
 //   rgba_mse_iou_*   nn.MSELoss on cat(image, alpha) vs the RGBA target (run_reconstruction.py:429-431)
 //                    fused with mean_iou's counts (run_reconstruction.py:225-231): one pass over the
@@ -207,7 +207,7 @@ int b3d_rgba_mse_iou_fwd(const float* image, const float* alpha, const float* ta
     B3D_CUDA_OK(cudaMemsetAsync(loss, 0, sizeof(float), st));
     if (counts) B3D_CUDA_OK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * 2 * B, st));
     const int HW = H * W;
-    const int gx = min(b3d::ceil_div(HW, NT), 148 * 4);
+    const int gx = min(b3d::ceil_div(HW, NT), 132 * 4);
     rgba_mse_iou_fwd_kernel<<<dim3(gx, B), NT, 0, st>>>(image, alpha, target, HW, 1.f / (4.f * (float)B * (float)HW),
                                                        loss, counts);
     B3D_LAUNCH_OK();
@@ -219,7 +219,7 @@ int b3d_rgba_mse_bwd(const float* image, const float* alpha, const float* target
     B3D_REQUIRE(B > 0 && H > 0 && W > 0 && image && alpha && target && gloss && d_image && d_alpha, B3D_EINVAL,
                 "b3d_rgba_mse_bwd: bad arguments");
     const int HW = H * W;
-    const int gx = min(b3d::ceil_div(HW, NT), 148 * 4);
+    const int gx = min(b3d::ceil_div(HW, NT), 132 * 4);
     rgba_mse_bwd_kernel<<<dim3(gx, B), NT, 0, (cudaStream_t)stream>>>(image, alpha, target, HW,
                                                                      1.f / (4.f * (float)B * (float)HW), gloss,
                                                                      d_image, d_alpha);

@@ -1,4 +1,4 @@
-// Textured-mesh render path (SURVEY.md §8 rows a7-a9, a12) for sm_100a: kaolin-free DIB-R.
+// Textured-mesh render path (SURVEY.md §8 rows a7-a9, a12) for sm_90a: kaolin-free DIB-R.
 //
 //   mesh_face_setup_kernel   ortho_projection (renderer.py:9-28): gathers by `faces`/`ft`, scales the 2-D
 //                            vertices by the rasteriser's multiplier, face normal (FMA pattern of torch.cross),

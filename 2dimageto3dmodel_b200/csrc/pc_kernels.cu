@@ -1,4 +1,4 @@
-// Point-cloud "effective loss" path (SURVEY.md §8 rows a1-a5) for sm_100a.
+// Point-cloud "effective loss" path (SURVEY.md §8 rows a1-a5) for sm_90a.
 //
 //   pc_project_kernel        a1+a2+a3(index part): quaternion rotate, perspective divide, grid coords,
 //                            in-bounds mask, floor index buffer.  Uses round-to-nearest intrinsics in the
@@ -1032,7 +1032,7 @@ int b3d_pc_splat_grid(const float* pg, int B, int N, int V, int mode, float* gri
         B3D_LAUNCH_OK();
     }
     const int blocks = (int)((cells + NTHREADS * 8 - 1) / (NTHREADS * 8));
-    clamp01_kernel<<<blocks < 148 * 8 ? blocks : 148 * 8, NTHREADS, 0, st>>>(grid, cells);
+    clamp01_kernel<<<blocks < 132 * 8 ? blocks : 132 * 8, NTHREADS, 0, st>>>(grid, cells);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }

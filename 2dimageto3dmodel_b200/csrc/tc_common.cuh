@@ -1,7 +1,8 @@
-// sm_100a tensor-core plumbing shared by the GEMM / implicit-GEMM conv kernels: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma kind::tf32 / commit / ld) wrappers in inline PTX, UMMA
-// shared-memory and instruction descriptors, and the host-side tensor-map encoder (driver entry point
-// resolved at run time through cudaGetDriverEntryPoint: the library does not link libcuda).
+// sm_90a tensor-core plumbing shared by the implicit-GEMM conv kernels: mbarrier, TMA (cp.async.bulk.tensor) and
+// warpgroup MMA (wgmma.mma_async kind tf32) wrappers in inline PTX, wgmma shared-memory descriptors, the operand
+// transpose used where an operand arrives M/N-major (wgmma reads tf32 operands K-major only), the fragment-layout
+// helpers of the epilogues and the host-side tensor-map encoder (driver entry point resolved at run time through
+// cudaGetDriverEntryPoint: the library does not link libcuda).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -18,6 +19,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// generic-proxy shared-memory writes (the operand transposes) made visible to the async proxy (wgmma, TMA)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -39,17 +41,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         "r"(parity)
         : "memory");
 }
+// named barrier over `count` threads (ids 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t count) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // ---------------------------------------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            smem_u32(smem)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
     asm volatile(
@@ -66,7 +65,6 @@ __device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* m, ui
         "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
         : "memory");
 }
-
 __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
                                             int c3, int c4) {
     asm volatile(
@@ -76,287 +74,125 @@ __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* m, ui
         : "memory");
 }
 
-// The same, issued only where `on` is non-zero: the producer warps run their loops convergently too (see "MMA issue from a
-// CONVERGENT warp" below: coordinates, shared-memory addresses and barrier addresses stay in uniform registers, no per-load
-// ELECT / R2UR waterfall) and one elected lane performs the arrive and the bulk-tensor copies.
-__device__ __forceinline__ void mbar_arrive_expect_tx_if(uint32_t on, uint64_t* bar, uint32_t bytes) {
-    asm volatile(
-        "{\n"
-        ".reg .pred q;\n"
-        "setp.ne.b32 q, %2, 0;\n"
-        "@q mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(bytes), "r"(on)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_if(uint32_t on, void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "{\n"
-        ".reg .pred q;\n"
-        "setp.ne.b32 q, %6, 0;\n"
-        "@q cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n"
-        "}\n" ::"r"(smem_u32(smem)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(on)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_if(uint32_t on, void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                               int c3) {
-    asm volatile(
-        "{\n"
-        ".reg .pred q;\n"
-        "setp.ne.b32 q, %7, 0;\n"
-        "@q cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];\n"
-        "}\n" ::"r"(smem_u32(smem)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(on)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_if(uint32_t on, void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                               int c3, int c4) {
-    asm volatile(
-        "{\n"
-        ".reg .pred q;\n"
-        "setp.ne.b32 q, %8, 0;\n"
-        "@q cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];\n"
-        "}\n" ::"r"(smem_u32(smem)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "r"(on)
-        : "memory");
-}
+// ---------------------------------------------------------------------------------------------- wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// ---------------------------------------------------------------------------------------------- tcgen05
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {     // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {        // the same warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// D[64 x N] (+)= A[64 x 8] * B[8 x N], tf32 operands (fp32 words in shared memory, K-major), fp32 accumulators in the
+// registers of the issuing warpgroup.  Fragment: thread t (warp w = t / 32, lane l) holds d[4j + e] = D[16w + l/4 + 8(e/2),
+// 8j + 2(l%4) + e%2].
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<64> {
+    __device__ __forceinline__ static void mma(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "setp.ne.b32 p, %34, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+            "%32, %33, p, 1, 1;\n"
+            "}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(da), "l"(db), "r"(accumulate));
+    }
+};
+template <>
+struct Wgmma<128> {
+    __device__ __forceinline__ static void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "setp.ne.b32 p, %66, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+            "%64, %65, p, 1, 1;\n"
+            "}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(da), "l"(db), "r"(accumulate));
+    }
+};
+template <>
+struct Wgmma<256> {
+    __device__ __forceinline__ static void mma(float (&d)[128], uint64_t da, uint64_t db, uint32_t accumulate) {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "setp.ne.b32 p, %130, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+            "%128, %129, p, 1, 1;\n"
+            "}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+            : "l"(da), "l"(db), "r"(accumulate));
+    }
+};
 
-// D[tmem] (+)= A[smem] * B[smem], tf32 inputs (fp32 words in shared memory), fp32 accumulate
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// ---- MMA issue from a CONVERGENT warp -------------------------------------------------------------------------------
-// ncu (profiles/r2_h_issue_loop.md): with the issue loop inside `if (lane == 0)` every loop variable lives in vector
-// registers, so ptxas wraps each tcgen05.mma in an ELECT / R2UR.BROADCAST "waterfall" loop to move the TMEM address into a
-// uniform register and rebuilds both descriptors with shift / mask / or chains: ~13 SASS instructions and a branch per MMA.
-// At N = 64 an MMA occupies the tensor pipe for ~53 cycles but the issuing thread needed ~95 — the 64-wide layers were bound
-// by instruction issue, not by tensor, L2 or shared-memory bandwidth.  Fix: all 32 lanes of the MMA warp walk the loop
-// (warp-uniform control flow: ptxas keeps the loop state, the descriptors and the TMEM addresses in UNIFORM registers), the
-// TMEM base goes through a warp reduction (REDUX writes a uniform register), descriptors are advanced with one integer add
-// on their low word, and only an elected lane executes the tcgen05 instructions: 3.4 instructions per MMA.
-__device__ __forceinline__ uint32_t elect_one() {          // 1 in exactly one lane of the (fully active) warp
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "elect.sync _|p, 0xffffffff;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(pred));
-    return pred;
-}
-__device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __reduce_or_sync(0xffffffffu, v); }   // same v in all lanes
-// Descriptor words: the high word (stride offset, version, layout type) does not depend on the address; the low word holds
-// the start address in 16-byte units in bits [0,14) (+ the leading byte offset in [16,30)), so the descriptor of
-// `addr + off` is `lo(addr) + (off >> 4)` — no carry out of the field for any shared-memory address.
-__device__ __forceinline__ uint32_t desc_lo(uint64_t d) { return (uint32_t)d; }
-__device__ __forceinline__ uint32_t desc_hi(uint64_t d) { return (uint32_t)(d >> 32); }
-__device__ __forceinline__ void umma_tf32_words_if(uint32_t on, uint32_t tmem_d, uint32_t lo_a, uint32_t hi_a, uint32_t lo_b,
-                                                   uint32_t hi_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p, q;\n"
-        ".reg .b64 da, db;\n"
-        "setp.ne.b32 p, %6, 0;\n"
-        "setp.ne.b32 q, %7, 0;\n"
-        "mov.b64 da, {%1, %2};\n"
-        "mov.b64 db, {%3, %4};\n"
-        "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "r"(lo_a), "r"(hi_a), "r"(lo_b), "r"(hi_b), "r"(idesc), "r"(accumulate), "r"(on)
-        : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void umma_commit_if(uint32_t on, uint64_t* bar) {
-    asm volatile(
-        "{\n"
-        ".reg .pred q;\n"
-        "setp.ne.b32 q, %1, 0;\n"
-        "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(on)
-        : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread t of the warp gets lane (lane_base + t), columns col .. col+31
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// UMMA shared-memory matrix descriptor, K-major operand, 128-byte swizzle: rows of 128 B (32 fp32), 8-row
-// swizzle atoms of 1024 B stacked along M/N (stride byte offset 1024), base 1024-B aligned.
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t smem_addr) {
+// wgmma shared-memory matrix descriptor, K-major operand.  128-byte swizzle: rows of 128 B (32 fp32), 8-row atoms of
+// 1024 B stacked along M/N (stride byte offset 1024), base 1024-B aligned; the k-th 8-wide K step of a 32-wide slice
+// starts 32 B further.  32-byte swizzle: rows of 32 B (one K step), 8-row atoms of 256 B.
+__device__ __forceinline__ uint64_t desc_k128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address,      bits [0,14)
     d |= (uint64_t)1 << 16;                             // leading byte offset (unused for swizzled K-major)
     d |= (uint64_t)(1024 >> 4) << 32;                   // stride byte offset, bits [32,46)
-    d |= (uint64_t)1 << 46;                             // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                             // layout type: SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                             // layout type: SWIZZLE_128B
     return d;
 }
-
-// K-major operand, 32-byte swizzle: rows of 32 B (8 fp32 = one UMMA_K step of tf32), 8-row atoms of 256 B stacked along
-// M/N.  What TMA writes for a box whose inner dimension is 8 floats under CU_TENSOR_MAP_SWIZZLE_32B (tools/probe/tma_probe.cu:
-// under the 128-byte modes such a box is padded to one 128-byte line per inner row instead).
-__device__ __forceinline__ uint64_t umma_desc_k32(uint32_t smem_addr) {
+__device__ __forceinline__ uint64_t desc_k32(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;                             // leading byte offset (unused: K extent = one atom)
+    d |= (uint64_t)1 << 16;
     d |= (uint64_t)(256 >> 4) << 32;                    // stride byte offset: 8 rows x 32 B
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)6 << 61;                             // layout type: SWIZZLE_32B
+    d |= (uint64_t)3 << 62;                             // layout type: SWIZZLE_32B
     return d;
 }
 
-// MN-major operand, 128-byte swizzle: the tile is stored as [mn block of 32][k rows][32 fp32 along M/N]; one
-// swizzle atom = 8 k-rows x 128 B.  Leading byte offset = distance between consecutive 32-wide M/N blocks,
-// stride byte offset = distance between consecutive groups of 8 k-rows.
-__device__ __forceinline__ uint64_t umma_desc_mn128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                     uint32_t layout_type = 1) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)layout_type << 61;                   // 1 = SWIZZLE_128B with 32-byte atoms (32-bit MN-major)
-    return d;
+// One 32-wide K slice of an operand that TMA delivered M/N-major (NHWC pixels along K: the weight gradient's dY and X)
+// as `rows` / 32 boxes [k][32 mn] (no swizzle; boxes blk_stride floats apart), K rows k0 .. k0 + 31 rewritten K-major
+// into `dst` in the 128-byte-swizzled layout that desc_k128 reads: row mn, 16-byte chunk c at byte
+// mn * 128 + ((c ^ (mn % 8)) << 4).  Executed by the 128 threads of the producer warpgroup; consecutive threads take
+// consecutive rows (conflict-free reads and stores).
+__device__ __forceinline__ void transpose_slice_k128(const float* raw, unsigned char* dst, int rows, int tid, int blk_stride = 1024,
+                                                     int k0 = 0) {
+    for (int i = tid; i < rows * 8; i += 128) {
+        const int mn = i % rows, kc = i / rows;
+        const float* src = raw + (mn >> 5) * blk_stride + (k0 + kc * 4) * 32 + (mn & 31);
+        const float4 v = make_float4(src[0], src[32], src[64], src[96]);
+        *reinterpret_cast<float4*>(dst + mn * 128 + ((kc ^ (mn & 7)) << 4)) = v;
+    }
 }
 
-// instruction descriptor for kind::tf32: D = fp32, A/B = tf32, M x N tile; *_mn = operand is M/N-major (transposed)
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N, bool a_mn = false, bool b_mn = false) {
-    return (1u << 4)                       // c_format = F32
-           | (2u << 7)                     // a_format = TF32
-           | (2u << 10)                    // b_format = TF32
-           | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16)
-           | ((uint32_t)(N >> 3) << 17)    // n_dim
-           | ((uint32_t)(M >> 4) << 24);   // m_dim
-}
-
-// ---------------------------------------------------------------------------------------------- epilogue: BN statistics
-// Per-channel sum / sum of squares of a conv OUTPUT accumulated by the epilogue that already holds the values in
-// registers (SURVEY §5 / §7 step 7 "BN statistics in the conv epilogue"; replaces a separate pass over the tensor).
-// v[32]: this lane's pixel, 32 consecutive channels (zeros for pixels outside the tensor).  A transposing butterfly
-// (31 shuffles per quantity) leaves lane l with the warp's sum for channel l; the four epilogue warps fold into a CTA
-// shared-memory pair sm_stats[2][BN] and the CTA flushes it with fp64 global atomics once per work item.
-__device__ __forceinline__ void warp_channel_sums(const float (&v)[32], float& s, float& q) {
-    float a[32], b[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) { a[i] = v[i]; b[i] = v[i] * v[i]; }
+// ---------------------------------------------------------------------------------------------- epilogue helpers
+// Column sums of one 8-wide block of a 64 x N accumulator fragment over the rows flagged valid: va[e] / vb[e] = this
+// thread's values of column 2 (l % 4) + e in row l/4 / l/4 + 8 of the warp's 16 (zero where the row is not valid), added
+// into sm_stats[0][c8 + ...] (and the sums of squares into sm_stats[BN_ + ...] unless sum_only).  A butterfly over the
+// eight lanes that share l % 4 leaves lanes 0-3 with the warp's sums of their two columns.
+__device__ __forceinline__ void stats_accumulate8(const float (&va)[2], const float (&vb)[2], float* sm_stats, int BN_, int c8,
+                                                  bool sum_only) {
     const int lane = threadIdx.x & 31;
 #pragma unroll
-    for (int ofs = 16; ofs >= 1; ofs >>= 1) {
-        const bool up = (lane & ofs) != 0;
+    for (int e = 0; e < 2; ++e) {
+        float s = va[e] + vb[e], q = va[e] * va[e] + vb[e] * vb[e];
 #pragma unroll
-        for (int i = 0; i < ofs; ++i) {
-            const float sa = up ? a[i] : a[i + ofs], ka = up ? a[i + ofs] : a[i];
-            const float sb = up ? b[i] : b[i + ofs], kb = up ? b[i + ofs] : b[i];
-            a[i] = ka + __shfl_xor_sync(0xffffffffu, sa, ofs);
-            b[i] = kb + __shfl_xor_sync(0xffffffffu, sb, ofs);
+        for (int o = 4; o < 32; o <<= 1) {
+            s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (!sum_only) q += __shfl_xor_sync(0xffffffffu, q, o);
+        }
+        if (lane < 4) {
+            const int c = c8 + 2 * lane + e;
+            atomicAdd(sm_stats + c, s);
+            if (!sum_only) atomicAdd(sm_stats + BN_ + c, q);
         }
     }
-    s = a[0];
-    q = b[0];
 }
-// epilogue warps: add this chunk's 32 channel sums into sm_stats[0][c..c+32) / sm_stats[1][...]  (BN = row length)
-__device__ __forceinline__ void stats_accumulate(const float (&v)[32], bool valid, float* sm_stats, int BN_, int c) {
-    float z[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) z[i] = valid ? v[i] : 0.f;
-    float s, q;
-    warp_channel_sums(z, s, q);
-    const int lane = threadIdx.x & 31;
-    atomicAdd(sm_stats + c + lane, s);
-    atomicAdd(sm_stats + BN_ + c + lane, q);
-}
-// sums only (bias gradient of a fused activation adjoint): half the shuffles
-__device__ __forceinline__ void stats_accumulate_sum(const float (&v)[32], bool valid, float* sm_stats, int c) {
-    float a[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) a[i] = valid ? v[i] : 0.f;
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int ofs = 16; ofs >= 1; ofs >>= 1) {
-        const bool up = (lane & ofs) != 0;
-#pragma unroll
-        for (int i = 0; i < ofs; ++i) {
-            const float sa = up ? a[i] : a[i + ofs], ka = up ? a[i + ofs] : a[i];
-            a[i] = ka + __shfl_xor_sync(0xffffffffu, sa, ofs);
-        }
-    }
-    atomicAdd(sm_stats + c + lane, a[0]);
-}
-// Activation adjoint fused into an input-gradient epilogue: v[i] *= (m[i] >= 0 ? 1 : slope), m = the 32 activated forward
-// values at this lane's output pixel (LeakyReLU keeps the sign, so the activated tensor is its own mask; the same rule as
-// pad_leaky_bias_bwd_kernel in ew_kernels.cu).  The epilogue warps fetch the signs of a whole work item as bit words
-// BEFORE they wait for the accumulator (the loads overlap the item's MMA main loop instead of sitting between tcgen05.ld
-// and the stores).  `vec`: all 32 channels exist and are 16-byte aligned; channels >= nch read as "pass".
-__device__ __forceinline__ uint32_t act_mask_bits32(const float* m, bool vec, int nch) {
-    uint32_t bits = 0;
-    if (vec) {
-        float4 t[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) t[i] = __ldg(reinterpret_cast<const float4*>(m) + i);
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-            bits |= ((t[i].x >= 0.f ? 1u : 0u) | (t[i].y >= 0.f ? 2u : 0u) | (t[i].z >= 0.f ? 4u : 0u) | (t[i].w >= 0.f ? 8u : 0u)) << (4 * i);
-    } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) bits |= ((i >= nch || __ldg(m + (i < nch ? i : 0)) >= 0.f) ? 1u : 0u) << i;
-    }
-    return bits;
-}
-template <int NW>
-__device__ __forceinline__ uint32_t pick_word(const uint32_t (&w)[NW], int idx) {      // register-resident dynamic index
-    uint32_t r = w[0];
-#pragma unroll
-    for (int k = 1; k < NW; ++k) r = (k == idx) ? w[k] : r;
-    return r;
-}
-__device__ __forceinline__ void apply_act_bits32(float (&v)[32], uint32_t bits, float slope) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = ((bits >> i) & 1u) ? v[i] : v[i] * slope;
-}
-// one epilogue warp after all four are done with the item (named barrier 1, 128 threads): flush + clear
-__device__ __forceinline__ void stats_flush(float* sm_stats, int BN_, double* gstats, int C, int c0, int ep_tid) {
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    for (int i = ep_tid; i < BN_; i += 128) {
+// the `nthreads` epilogue threads after all of them are done with the item (named barrier 1): flush + clear
+__device__ __forceinline__ void stats_flush(float* sm_stats, int BN_, double* gstats, int C, int c0, int ep_tid, int nthreads) {
+    named_sync(1, nthreads);
+    for (int i = ep_tid; i < BN_; i += nthreads) {
         if (c0 + i < C) {
             atomicAdd(gstats + c0 + i, (double)sm_stats[i]);
             atomicAdd(gstats + C + c0 + i, (double)sm_stats[BN_ + i]);
@@ -364,7 +200,7 @@ __device__ __forceinline__ void stats_flush(float* sm_stats, int BN_, double* gs
         sm_stats[i] = 0.f;
         sm_stats[BN_ + i] = 0.f;
     }
-    asm volatile("bar.sync 1, 128;" ::: "memory");
+    named_sync(1, nthreads);
 }
 
 // ---------------------------------------------------------------------------------------------- host: tensor maps
@@ -409,6 +245,14 @@ inline int make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint6
         return B3D_ECUDA;
     }
     return B3D_OK;
+}
+
+// streaming multiprocessors of the current device (persistent grids, K splits)
+inline int num_sms() {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1)
+        return 132;
+    return n;
 }
 
 }  // namespace tc

@@ -1,439 +1,246 @@
-// Implicit-GEMM 2-D convolution on the 5th-generation tensor cores (sm_100a): the dense convs of the
+// Implicit-GEMM 2-D convolution on the Hopper tensor cores (sm_90a, wgmma kind tf32): the dense convs of the
 // conv-GAN generator / discriminators (models/gan.py:57-65,163-177,294-302,359,364; SURVEY.md §8 a13/a14).
 //
 //   Y[n, y, x, co] = sum_t sum_ci  X[n, sy*y + dy[t], sx*x + dx[t], ci] * Wt[t, co, ci]      (NHWC, fp32)
 //
-// "Tap-shifted TMA" formulation: no im2col buffer.  A CTA owns 128 output pixels (a BW x BH x BI box of
-// the output) x BN output channels.  For every filter tap t and every 32-channel slice of Cin the TMA
-// producer issues ONE 4-D tiled load of the input box shifted by (dy[t], dx[t]) — out-of-bounds rows and
-// columns are zero-filled by the TMA unit, which IS the convolution's zero padding — and one 3-D load of
-// the weight slice; both land in 128-byte-swizzled K-major tiles that `tcgen05.mma.kind::tf32` consumes
-// directly (fp32 words, tf32 precision, fp32 accumulation in TMEM).  The same kernel computes
+// "Tap-shifted TMA" formulation: no im2col buffer.  A work item is 128 output pixels (a BW x BH x BI box of the
+// output) x BN output channels.  For every filter tap t and every 32-channel slice of Cin the TMA producer issues ONE
+// 4-D tiled load of the input box shifted by (dy[t], dx[t]) — out-of-bounds rows and columns are zero-filled by the
+// TMA unit, which IS the convolution's zero padding — and one 3-D load of the weight slice; both land in
+// 128-byte-swizzled K-major tiles that `wgmma.mma_async ... .tf32` consumes directly (fp32 words, tf32 precision,
+// fp32 accumulation in registers).  The same kernel computes
 //   * fprop   (dy = r - pad_y, dx = s, Wt[t] = W[:, :, r, s]),
 //   * dgrad   (dy = pad_y - r, dx = -s, Wt[t] = W[:, :, r, s]^T)  — the "full" correlation falls out of the
 //     TMA zero fill, and strided (4x4 / stride 2) dgrad runs as 4 parity classes with a strided epilogue,
 //   * strided fprop (element strides in the tensor map).
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = MMA issuer (one elected lane), warps 2-5 =
-// epilogue (TMEM -> registers -> bias / LeakyReLU -> global).  STAGES-deep mbarrier ring between producer
-// and MMA; tcgen05.commit frees a stage and finally signals the epilogue.
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread issues), warpgroups 1-2 = wgmma on pixel rows 0-63 /
+// 64-127 of the tile and the epilogue straight from the accumulator registers (bias / LeakyReLU / BN statistics /
+// fused activation adjoint -> global).  Persistent: a CTA per SM walks the work items; the STAGES-deep mbarrier ring
+// keeps the producer loading the next item while the consumers run the epilogue of the current one.
 #include "tc_common.cuh"
-#include "tc_rowwin.cuh"
 
 namespace {
 
-constexpr int BM = 128;         // output pixels per CTA  (UMMA M)
+constexpr int BM = 128;         // output pixels per work item (two m64 warpgroup tiles)
 constexpr int BK = 32;          // fp32 channels per K slice = 128 B = one swizzle row
-constexpr int UMMA_K = 8;       // tf32
+constexpr int MMA_K = 8;        // tf32
 constexpr int MAX_TAPS = 25;
-constexpr int NTHREADS = 224;   // warp 0: A-operand TMA, warp 1: MMA issue, warps 2-5: epilogue, warp 6: B-operand TMA
+constexpr int NTHREADS = 384;   // warpgroup 0: TMA producer, warpgroups 1-2: MMA + epilogue
 
 struct ConvParams {
     int N, Hout, Wout, Cout;          // logical output extent covered by tiles (before the epilogue transform)
-    int BW, BH, BI;                   // output box per CTA, BW*BH*BI == 128
-    int tiles_x, tiles_y;             // tiles along W and H (tiles along N = gridDim.x / (tiles_x*tiles_y))
+    int BW, BH, BI;                   // output box per work item, BW*BH*BI == 128
+    int tiles_x, tiles_y;             // tiles along W and H (tiles along N = tiles / (tiles_x*tiles_y))
     int xbase;                        // first output column of this launch (a strip launch covers the last few columns)
-    int ntaps, kslices;               // filter taps, Cin / 32
+    int ntaps, kslices;               // filter taps (per class), Cin / 32
     int sy, sx;                       // input coordinate = s * out + d[t]
     int dy[MAX_TAPS], dx[MAX_TAPS];
     int wtap[MAX_TAPS];               // weight tap (row of the tap-major weight array) read for loop tap t
-    // epilogue: out pixel (n, oy*y + ooy, ox*x + oox) of a tensor [N, OH, OW, OC], channel offset 0
-    int OH, OW, OC, osy, osx, ooy, oox;
+    // epilogue: out pixel (n, osy*y + cooy[class], osx*x + coox[class]) of a tensor [N, OH, OW, OC], channel offset 0
+    int OH, OW, OC, osy, osx;
     float leaky;                      // 1.0 = identity
-    int dbg_lbo, dbg_sbo, dbg_lt;     // MN-major descriptor offsets (bytes), layout type
     double* stats;                    // nullable: [2][Cout] fp64 sum / sum of squares of the (pre-bias) output, accumulated
     int fold;                         // > 0: the A operand is folded on the fly from a raw [N,H,W,8] tensor (thin stems): K slice ks
-    int fold_y0;                      //      = image rows y + fold_y0 + 4 ks .. + 3 of the 8 channels (tensor map dims c, row, x, n)
+    int fold_y0;                      //      = image rows y + fold_y0 + 4 ks .. + 3 of the 8 channels (tensor map dims c, x, row, n)
     const float* mask;                // nullable: tensor of the output's geometry; acc *= (mask >= 0 ? 1 : mslope) before statistics / bias
     float mslope;                     //           (LeakyReLU adjoint fused into the input-gradient epilogue)
     int stats_sum;                    // statistics: sums only (the bias gradient of the fused adjoint)
     int ncls;                         // >= 1 output classes in ONE launch (the stride-2 input gradient's parity classes): class c uses taps
     int cooy[4], coox[4];             //      [c * ntaps, (c + 1) * ntaps) of dy / dx / wtap and the output offset (cooy[c], coox[c])
+    int dx0, shift[5];                // row window (KW > 1): window starts at column x + dx0; tap t of a filter row reads it shift[t] rows in
 };
 
-template <int BN, int STAGES>
-struct Smem {
-    static constexpr int A_BYTES = BM * BK * 4;
-    static constexpr int B_BYTES = BN * BK * 4;
+// KW == 1: one stage = the 128-pixel A tile of one tap and its weight tile.  KW > 1 (row window): one stage = ONE window of
+// 128 + KW - 1 input pixels of a filter row and the KW weight tiles of that row; the consumers feed tap t as the window
+// shifted by whole 128-byte rows (the 128-byte swizzle is a function of the absolute shared-memory address, so TMA's write
+// pattern and the shifted descriptor agree), i.e. the A operand is loaded once per filter row instead of once per tap.
+template <int BN, int STAGES, int KW>
+struct CSmem {
+    static constexpr int WIN_BYTES = (BM + KW - 1) * BK * 4;                 // what the A box delivers
+    static constexpr int A_BYTES = (WIN_BYTES + 1023) / 1024 * 1024;         // B tiles start on a swizzle-atom boundary
+    static constexpr int B_BYTES = KW * BN * BK * 4;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int TX_BYTES = WIN_BYTES + B_BYTES;
+    static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * BN * 4 /*BN statistics*/;
 };
 
-template <int BN, int STAGES, bool WMN, int MINB>
-__global__ void __launch_bounds__(NTHREADS, MINB)
-conv_tf32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                 const ConvParams p, const float* __restrict__ bias, float* __restrict__ out) {
-    using S = Smem<BN, STAGES>;
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * S::STAGE_BYTES);
-    uint64_t* empty = full + STAGES;
-    uint64_t* acc_full = empty + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // tile coordinates
-    int t = blockIdx.x;
-    const int tx = t % p.tiles_x;
-    t /= p.tiles_x;
-    const int ty = t % p.tiles_y;
-    const int tn = t / p.tiles_y;
-    const int x0 = p.xbase + tx * p.BW, y0 = ty * p.BH, n0 = tn * p.BI;
-    const int c0 = blockIdx.y * BN;
-
-    if (warp == 0 && lane == 0) {
-        tc::tma_prefetch_desc(&tmap_x);
-        tc::tma_prefetch_desc(&tmap_w);
+// The K loop of one work item for one consumer warpgroup: rows [64 h, 64 h + 64) of the 128 x BN accumulator.  A stage
+// is handed back to the producer once the wgmma group that read it has retired (one arrival per warpgroup).
+template <int BN, int STAGES, int KW, bool FOLD>
+__device__ __forceinline__ void mainloop(float (&acc)[BN / 2], unsigned char* base, uint64_t* full, uint64_t* empty, int KI,
+                                         uint32_t& git, int h, bool leader, const int* shift) {
+    constexpr int A_BYTES = CSmem<BN, STAGES, KW>::A_BYTES, STAGE = CSmem<BN, STAGES, KW>::STAGE_BYTES;
+    for (int it = 0; it < KI; ++it, ++git) {
+        const int s = git % STAGES;
+        tc::mbar_wait(full + s, (git / STAGES) & 1);
+        const uint32_t a = tc::smem_u32(base + s * STAGE), b = a + A_BYTES;
+        tc::wgmma_fence();
+#pragma unroll
+        for (int t = 0; t < KW; ++t) {
+            const uint32_t at = a + h * (64 * 128) + (KW > 1 ? shift[t] * 128 : 0);
+#pragma unroll
+            for (int k = 0; k < BK / MMA_K; ++k) {
+                // on-the-fly fold: K step k = image row k of the 4-row box, a [128 px][32 B] tile of its own (32-byte swizzle)
+                const uint64_t da = FOLD ? tc::desc_k32(a + k * (BM * 32) + h * (64 * 32)) : tc::desc_k128(at + k * MMA_K * 4);
+                tc::Wgmma<BN>::mma(acc, da, tc::desc_k128(b + t * (BN * 128) + k * MMA_K * 4), (it | t | k) ? 1u : 0u);
+            }
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();
+        if (it > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES);
     }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < STAGES; ++s) {
-            tc::mbar_init(full + s, 1);
-            tc::mbar_init(empty + s, 1);
-        }
-        tc::mbar_init(acc_full, 1);
-        tc::fence_barrier_init();
-    }
-    if (warp == 2) tc::tmem_alloc<(BN < 32 ? 32 : BN)>(tmem_slot);
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_acc = *tmem_slot;
-    const int KI = p.ntaps * p.kslices;
-
-    // One elected lane spends ~200 cycles per TMA instruction (profiles/r1_conv_layers.md), about the tensor-core time of
-    // the K slice it feeds, so the two operands are issued by two different warps; both complete on the same barrier.
-    if (warp == 0) {
-        if (lane == 0) {
-            for (int it = 0; it < KI; ++it) {
-                const int s = it % STAGES, ph = (it / STAGES) & 1;
-                tc::mbar_wait(empty + s, ph ^ 1);
-                const int tap = it / p.kslices, ks = it % p.kslices;
-                unsigned char* a = base + s * S::STAGE_BYTES;
-                tc::mbar_arrive_expect_tx(full + s, S::STAGE_BYTES);
-                tc::tma_load_4d(a, &tmap_x, full + s, ks * BK, p.sx * x0 + p.dx[tap], p.sy * y0 + p.dy[tap], n0);
-            }
-        }
-    } else if (warp == 6) {
-        if (lane == 0) {
-            for (int it = 0; it < KI; ++it) {
-                const int s = it % STAGES, ph = (it / STAGES) & 1;
-                tc::mbar_wait(empty + s, ph ^ 1);
-                const int tap = it / p.kslices, ks = it % p.kslices;
-                unsigned char* b = base + s * S::STAGE_BYTES + S::A_BYTES;
-                if constexpr (WMN) {      // weights [tap][Cin][Cout]: 32 cin rows x 32 cout per box (N-major B operand)
-#pragma unroll
-                    for (int nb = 0; nb < BN / 32; ++nb) tc::tma_load_3d(b + nb * 4096, &tmap_w, full + s, c0 + nb * 32, ks * BK, p.wtap[tap]);
-                } else {
-                    tc::tma_load_3d(b, &tmap_w, full + s, ks * BK, c0, p.wtap[tap]);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = tc::umma_idesc_tf32(BM, BN, false, WMN);
-            for (int it = 0; it < KI; ++it) {
-                const int s = it % STAGES, ph = (it / STAGES) & 1;
-                tc::mbar_wait(full + s, ph);
-                tc::tc_fence_after();
-                const uint32_t a = tc::smem_u32(base + s * S::STAGE_BYTES);
-                const uint32_t b = a + S::A_BYTES;
-#pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k) {
-                    const uint64_t da = tc::umma_desc_k128(a + k * UMMA_K * 4);
-                    const uint64_t db = WMN ? tc::umma_desc_mn128(b + k * 1024, p.dbg_lbo, p.dbg_sbo, p.dbg_lt) : tc::umma_desc_k128(b + k * UMMA_K * 4);
-                    tc::umma_tf32(tmem_acc, da, db, idesc, (it | k) ? 1u : 0u);
-                }
-                tc::umma_commit(empty + s);          // frees the stage when these MMAs have read it
-            }
-            tc::umma_commit(acc_full);               // accumulator complete
-        }
-    } else {
-        // epilogue warps 2..5: TMEM lane quarter = warp % 4
-        const int q = warp & 3;
-        const int r = q * 32 + lane;                 // row of the tile = output pixel
-        const int bx = r % p.BW, by = (r / p.BW) % p.BH, bi = r / (p.BW * p.BH);
-        const int n = n0 + bi, y = y0 + by, x = x0 + bx;
-        const bool valid = n < p.N && y < p.Hout && x < p.Wout;
-        float* dst = out + (((size_t)n * p.OH + (size_t)(p.osy * y + p.ooy)) * p.OW + (size_t)(p.osx * x + p.oox)) * p.OC;
-        tc::mbar_wait(acc_full, 0);
-        tc::tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < BN; c += 32) {
-            float v[32];
-            tc::tmem_ld32(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
-            if (valid) {
-                const int cb = c0 + c;
-                if (cb + 32 <= p.Cout && (p.OC & 3) == 0) {       // full 32-channel run: 8 x 16-byte stores
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        float4 o;
-                        o.x = v[j] + (bias ? __ldg(bias + cb + j) : 0.f);
-                        o.y = v[j + 1] + (bias ? __ldg(bias + cb + j + 1) : 0.f);
-                        o.z = v[j + 2] + (bias ? __ldg(bias + cb + j + 2) : 0.f);
-                        o.w = v[j + 3] + (bias ? __ldg(bias + cb + j + 3) : 0.f);
-                        o.x = o.x >= 0.f ? o.x : o.x * p.leaky;
-                        o.y = o.y >= 0.f ? o.y : o.y * p.leaky;
-                        o.z = o.z >= 0.f ? o.z : o.z * p.leaky;
-                        o.w = o.w >= 0.f ? o.w : o.w * p.leaky;
-                        *reinterpret_cast<float4*>(dst + cb + j) = o;
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const int co = cb + j;
-                        if (co < p.Cout) {
-                            float o = v[j] + (bias ? __ldg(bias + co) : 0.f);
-                            dst[co] = o >= 0.f ? o : o * p.leaky;
-                        }
-                    }
-                }
-            }
-        }
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tc::tmem_dealloc<(BN < 32 ? 32 : BN)>(tmem_acc);
+    tc::wgmma_wait<0>();
+    if (KI > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES);
 }
 
-// ----------------------------------------------------------------------------------------------
-// Persistent variant: one CTA loops over (tile, channel block) work items with TWO accumulators in tensor memory, so the
-// epilogue of item j (TMEM -> registers -> global, then the store drain) overlaps the TMA / MMA main loop of item j+1
-// inside the same CTA, and barrier init / TMEM allocation / descriptor prefetch are paid once per CTA instead of once
-// per 128 output pixels.  ncu on the one-tile-per-CTA kernel (profiles/r1_c_conv_final_full.md): layers with short K
-// loops (folded stems: 10 K slices, stride-2 dgrad classes: 16) keep the tensor pipe 18-23 % busy with no memory
-// system above 60 % — the CTA lifetime is fill + epilogue + drain.
-// Barriers: full/empty ring shared by all items (global K-slice counter), acc_full[2] (MMA -> epilogue, tcgen05.commit),
-// acc_empty[2] (epilogue -> MMA, one arrival per epilogue warp).
-// ----------------------------------------------------------------------------------------------
-constexpr int PTHREADS = 192;   // warp 0: TMA, warp 1: MMA issue, warps 2-5: epilogue
-
-// R = pixel tiles stacked per work item: they share every weight tile that arrives (R accumulators of BN columns per
-// TMEM buffer), which cuts the weight bytes per FLOP through the L2 -> SM fabric by R.
-template <int BN, int STAGES, int R>
-struct PSmem {
-    static constexpr int A_TILE = BM * BK * 4;
-    static constexpr int A_BYTES = R * A_TILE;
-    static constexpr int B_BYTES = BN * BK * 4;
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 320 /*barriers*/ + 2 * BN * 4 /*BN statistics*/;
-    static constexpr int CTAS_PER_SM = (2 * TOTAL <= 227 * 1024 && 4 * R * BN <= 512) ? 2 : 1;
-};
-
-template <int BN, int STAGES, bool WMN, int R>
-__global__ void __launch_bounds__(PTHREADS, PSmem<BN, STAGES, R>::CTAS_PER_SM)
-conv_tf32_persistent_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                            const ConvParams p, const float* __restrict__ bias, float* __restrict__ out, int tiles,
-                            int groups, int work_items) {
-    using S = PSmem<BN, STAGES, R>;
+template <int BN, int STAGES, int KW>
+__global__ void __launch_bounds__(NTHREADS, 1)
+conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w, const ConvParams p,
+                  const float* __restrict__ bias, float* __restrict__ out, int tiles, int work_items) {
+    using S = CSmem<BN, STAGES, KW>;
     extern __shared__ unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * S::STAGE_BYTES);
     uint64_t* empty = full + STAGES;
-    uint64_t* acc_full = empty + STAGES;
-    uint64_t* acc_empty = acc_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-    float* sm_stats = reinterpret_cast<float*>(base + STAGES * S::STAGE_BYTES + 320);
-    constexpr uint32_t TCOLS = 2 * R * BN < 32 ? 32 : 2 * R * BN;
-    static_assert(TCOLS <= 512 && (TCOLS & (TCOLS - 1)) == 0, "TMEM: 2 buffers x R accumulators x BN columns");
+    float* sm_stats = reinterpret_cast<float*>(base + STAGES * S::STAGE_BYTES + 256);
     for (int i = threadIdx.x; i < 2 * BN; i += blockDim.x) sm_stats[i] = 0.f;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tc::tma_prefetch_desc(&tmap_x);
         tc::tma_prefetch_desc(&tmap_w);
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; ++s) {
             tc::mbar_init(full + s, 1);
-            tc::mbar_init(empty + s, 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            tc::mbar_init(acc_full + b, 1);
-            tc::mbar_init(acc_empty + b, 4);
+            tc::mbar_init(empty + s, 2);
         }
         tc::fence_barrier_init();
     }
-    if (warp == 2) tc::tmem_alloc<TCOLS>(tmem_slot);
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_acc = *tmem_slot;
-    const int KI = p.ntaps * p.kslices;
+    const int KI = p.ntaps / KW * p.kslices;           // K steps: (taps or filter rows) x channel slices
+    const int wg = threadIdx.x >> 7;
 
-    if (warp == 0) {
-        {
-            const uint32_t leader = tc::elect_one();          // convergent producer loop: one elected lane arrives / issues the copies
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
             uint32_t git = 0;
             for (int w = blockIdx.x; w < work_items; w += gridDim.x) {
                 // classes are the fastest index: the CTAs that work on the same pixel tiles at the same time share them in L2
                 const int cls = w % p.ncls, wq = w / p.ncls, tb = cls * p.ntaps;
-                const int g = wq % groups, c0 = (wq / groups) * BN;
-                int x0[R], y0[R], n0[R];
-#pragma unroll
-                for (int r = 0; r < R; ++r) {
-                    int t = g * R + r;
-                    t = t < tiles ? t : tiles - 1;           // a group past the end re-loads the last tile (its result is dropped)
-                    x0[r] = p.xbase + (t % p.tiles_x) * p.BW;
-                    t /= p.tiles_x;
-                    y0[r] = (t % p.tiles_y) * p.BH;
-                    n0[r] = (t / p.tiles_y) * p.BI;
-                }
-                for (int it = 0; it < KI; ++it, ++git) {
-                    const int s = git % STAGES, ph = (git / STAGES) & 1;
-                    tc::mbar_wait(empty + s, ph ^ 1);
-                    const int tap = it / p.kslices, ks = it % p.kslices;
-                    unsigned char* a = base + s * S::STAGE_BYTES;
-                    unsigned char* b = a + S::A_BYTES;
-                    tc::mbar_arrive_expect_tx_if(leader, full + s, S::STAGE_BYTES);
-#pragma unroll
-                    for (int r = 0; r < R; ++r) {
-                        if (p.fold)     // box {8 ch, BW px, 4 rows}: lands as [row][pixel][8 floats] = four 32-byte-swizzled K-step tiles
-                            tc::tma_load_4d_if(leader, a + r * S::A_TILE, &tmap_x, full + s, 0, x0[r] + p.dx[tb + tap], y0[r] + p.fold_y0 + 4 * ks, n0[r]);
-                        else
-                            tc::tma_load_4d_if(leader, a + r * S::A_TILE, &tmap_x, full + s, ks * BK, p.sx * x0[r] + p.dx[tb + tap], p.sy * y0[r] + p.dy[tb + tap], n0[r]);
-                    }
-                    if constexpr (WMN) {
-#pragma unroll
-                        for (int nb = 0; nb < BN / 32; ++nb) tc::tma_load_3d_if(leader, b + nb * 4096, &tmap_w, full + s, c0 + nb * 32, ks * BK, p.wtap[tb + tap]);
-                    } else {
-                        tc::tma_load_3d_if(leader, b, &tmap_w, full + s, ks * BK, c0, p.wtap[tb + tap]);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // convergent issue loop (tc_common.cuh "MMA issue from a CONVERGENT warp"): all lanes walk it, one elected lane issues
-        const uint32_t leader = tc::elect_one();
-        const uint32_t tmem_u = tc::warp_uniform(tmem_acc);
-        constexpr uint32_t idesc = tc::umma_idesc_tf32(BM, BN, false, WMN);
-        uint32_t git = 0, j = 0;
-        for (int w = blockIdx.x; w < work_items; w += gridDim.x, ++j) {
-            const uint32_t buf = j & 1;
-            tc::mbar_wait(acc_empty + buf, ((j >> 1) & 1) ^ 1);      // the epilogue has drained this buffer
-            tc::tc_fence_after();
-            const uint32_t acc = tmem_u + buf * (R * BN);
-            for (int it = 0; it < KI; ++it, ++git) {
-                const int s = git % STAGES, ph = (git / STAGES) & 1;
-                tc::mbar_wait(full + s, ph);
-                tc::tc_fence_after();
-                const uint32_t a = tc::smem_u32(base + s * S::STAGE_BYTES);
-                const uint32_t b = a + S::A_BYTES;
-                // on-the-fly fold: K step k = image row k of the 4-row box, a [128 px][32 B] tile of its own (32-byte swizzle)
-                const uint64_t da0 = p.fold ? tc::umma_desc_k32(a) : tc::umma_desc_k128(a);
-                const uint64_t db0 = WMN ? tc::umma_desc_mn128(b, p.dbg_lbo, p.dbg_sbo, p.dbg_lt) : tc::umma_desc_k128(b);
-                const uint32_t astep = p.fold ? (BM * 32) >> 4 : (UMMA_K * 4) >> 4, bstep = WMN ? 1024 >> 4 : (UMMA_K * 4) >> 4;
-#pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k) {
-#pragma unroll
-                    for (int r = 0; r < R; ++r)
-                        tc::umma_tf32_words_if(leader, acc + r * BN, tc::desc_lo(da0) + r * (S::A_TILE >> 4) + k * astep, tc::desc_hi(da0),
-                                               tc::desc_lo(db0) + k * bstep, tc::desc_hi(db0), idesc, (it | k) ? 1u : 0u);
-                }
-                tc::umma_commit_if(leader, empty + s);
-            }
-            tc::umma_commit_if(leader, acc_full + buf);
-        }
-    } else {
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const int bx = row % p.BW, by = (row / p.BW) % p.BH, bi = row / (p.BW * p.BH);
-        uint32_t j = 0;
-        for (int w = blockIdx.x; w < work_items; w += gridDim.x, ++j) {
-            const int cls = w % p.ncls, wq = w / p.ncls;
-            const int g = wq % groups, c0 = (wq / groups) * BN;
-            const int ooy = p.cooy[cls], oox = p.coox[cls];
-            const uint32_t buf = j & 1;
-            constexpr int NW = R * (BN / 32);
-            uint32_t mbits[NW];
-            if (p.mask) {                                     // signs of the item's activation mask, fetched under its main loop
-#pragma unroll
-                for (int r = 0; r < R; ++r) {
-                    int t = g * R + r;
-                    const bool tile_ok = t < tiles;
-                    const int tx = t % p.tiles_x;
-                    t /= p.tiles_x;
-                    const int n = (t / p.tiles_y) * p.BI + bi, y = (t % p.tiles_y) * p.BH + by, x = p.xbase + tx * p.BW + bx;
-                    const bool valid = tile_ok && n < p.N && y < p.Hout && x < p.Wout;
-                    const size_t off = (((size_t)n * p.OH + (size_t)(p.osy * y + ooy)) * p.OW + (size_t)(p.osx * x + oox)) * p.OC;
-#pragma unroll
-                    for (int cc = 0; cc < BN / 32; ++cc) {
-                        const int cb = c0 + 32 * cc;
-                        mbits[r * (BN / 32) + cc] = (valid && cb < p.Cout)
-                            ? tc::act_mask_bits32(p.mask + off + cb, cb + 32 <= p.Cout && (p.OC & 3) == 0, p.Cout - cb) : 0xffffffffu;
-                    }
-                }
-            }
-            tc::mbar_wait(acc_full + buf, (j >> 1) & 1);
-            tc::tc_fence_after();
-#pragma unroll 1
-            for (int r = 0; r < R; ++r) {
-                int t = g * R + r;
-                const bool tile_ok = t < tiles;
-                const int tx = t % p.tiles_x;
+                int t = wq % tiles;
+                const int c0 = (wq / tiles) * BN;
+                const int x0 = p.xbase + (t % p.tiles_x) * p.BW;
                 t /= p.tiles_x;
-                const int n = (t / p.tiles_y) * p.BI + bi, y = (t % p.tiles_y) * p.BH + by, x = p.xbase + tx * p.BW + bx;
-                const bool valid = tile_ok && n < p.N && y < p.Hout && x < p.Wout;
-                const size_t off = (((size_t)n * p.OH + (size_t)(p.osy * y + ooy)) * p.OW + (size_t)(p.osx * x + oox)) * p.OC;
-                float* dst = out + off;
-#pragma unroll 1
-                for (int c = 0; c < BN; c += 32) {
-                    float v[32];
-                    tc::tmem_ld32(tmem_acc + ((uint32_t)(q * 32) << 16) + buf * (R * BN) + r * BN + (uint32_t)c, v);
-                    if (r == R - 1 && c + 32 >= BN) {        // last read of this buffer: hand it back before the stores
-                        tc::tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) tc::mbar_arrive(acc_empty + buf);
-                    }
-                    if (p.mask) tc::apply_act_bits32(v, tc::pick_word<NW>(mbits, r * (BN / 32) + c / 32), p.mslope);
-                    if (p.stats) {
-                        if (p.stats_sum) tc::stats_accumulate_sum(v, valid, sm_stats, c);
-                        else tc::stats_accumulate(v, valid, sm_stats, BN, c);
-                    }
-                    if (valid) {
-                        const int cb = c0 + c;
-                        if (cb + 32 <= p.Cout && (p.OC & 3) == 0) {
+                const int y0 = (t % p.tiles_y) * p.BH, n0 = (t / p.tiles_y) * p.BI;
+                for (int it = 0; it < KI; ++it, ++git) {
+                    const int s = git % STAGES;
+                    tc::mbar_wait(empty + s, ((git / STAGES) & 1) ^ 1);
+                    const int tap = it / p.kslices * KW, ks = it % p.kslices;        // KW > 1: first tap of the filter row
+                    unsigned char* a = base + s * S::STAGE_BYTES;
+                    tc::mbar_arrive_expect_tx(full + s, S::TX_BYTES);
+                    if (KW > 1)     // window of 128 + KW - 1 pixels of the row; one box with the row's KW weight tiles
+                        tc::tma_load_4d(a, &tmap_x, full + s, ks * BK, x0 + p.dx0, y0 + p.dy[tb + tap], n0);
+                    else if (p.fold)     // box {8 ch, BW px, 4 rows}: lands as [row][pixel][8 floats] = four 32-byte-swizzled K-step tiles
+                        tc::tma_load_4d(a, &tmap_x, full + s, 0, x0 + p.dx[tb + tap], y0 + p.fold_y0 + 4 * ks, n0);
+                    else
+                        tc::tma_load_4d(a, &tmap_x, full + s, ks * BK, p.sx * x0 + p.dx[tb + tap], p.sy * y0 + p.dy[tb + tap], n0);
+                    tc::tma_load_3d(a + S::A_BYTES, &tmap_w, full + s, ks * BK, c0, p.wtap[tb + tap]);
+                }
+            }
+        }
+        return;
+    }
+
+    const int h = wg - 1, tid = threadIdx.x & 127, lane = tid & 31;
+    const int row_a = h * 64 + (tid >> 5) * 16 + (lane >> 2);          // this thread's two accumulator rows: row_a, row_a + 8
+    int bx[2], by[2], bi[2];
 #pragma unroll
-                            for (int jj = 0; jj < 32; jj += 4) {
-                                float4 o;
-                                o.x = v[jj] + (bias ? __ldg(bias + cb + jj) : 0.f);
-                                o.y = v[jj + 1] + (bias ? __ldg(bias + cb + jj + 1) : 0.f);
-                                o.z = v[jj + 2] + (bias ? __ldg(bias + cb + jj + 2) : 0.f);
-                                o.w = v[jj + 3] + (bias ? __ldg(bias + cb + jj + 3) : 0.f);
-                                o.x = o.x >= 0.f ? o.x : o.x * p.leaky;
-                                o.y = o.y >= 0.f ? o.y : o.y * p.leaky;
-                                o.z = o.z >= 0.f ? o.z : o.z * p.leaky;
-                                o.w = o.w >= 0.f ? o.w : o.w * p.leaky;
-                                *reinterpret_cast<float4*>(dst + cb + jj) = o;
-                            }
-                        } else {
+    for (int e = 0; e < 2; ++e) {
+        const int r = row_a + 8 * e;
+        bx[e] = r % p.BW;
+        by[e] = (r / p.BW) % p.BH;
+        bi[e] = r / (p.BW * p.BH);
+    }
+    float acc[BN / 2];
 #pragma unroll
-                            for (int jj = 0; jj < 32; ++jj) {
-                                const int co = cb + jj;
-                                if (co < p.Cout) {
-                                    float o = v[jj] + (bias ? __ldg(bias + co) : 0.f);
-                                    dst[co] = o >= 0.f ? o : o * p.leaky;
-                                }
-                            }
-                        }
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    uint32_t git = 0;
+    for (int w = blockIdx.x; w < work_items; w += gridDim.x) {
+        const int cls = w % p.ncls, wq = w / p.ncls;
+        const int tile = wq % tiles, c0 = (wq / tiles) * BN;
+        if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, full, empty, KI, git, h, tid == 0, p.shift);
+        else mainloop<BN, STAGES, KW, false>(acc, base, full, empty, KI, git, h, tid == 0, p.shift);
+
+        const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, tn = tile / (p.tiles_x * p.tiles_y);
+        bool valid[2];
+        size_t off[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int n = tn * p.BI + bi[e], y = ty * p.BH + by[e], x = p.xbase + tx * p.BW + bx[e];
+            valid[e] = n < p.N && y < p.Hout && x < p.Wout;
+            off[e] = valid[e] ? (((size_t)n * p.OH + (size_t)(p.osy * y + p.cooy[cls])) * p.OW + (size_t)(p.osx * x + p.coox[cls])) * p.OC : 0;
+        }
+        // one 8-wide column block at a time, without writing the accumulators (they stay wgmma-only registers)
+        const int cq = c0 + 2 * (lane & 3);                           // first channel of this thread's column pair in block j: cq + 8 j
+        const bool vec = (p.OC & 1) == 0;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            float v[2][2];                                            // [row a / b][column pair]
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int e = i >> 1, co = cq + 8 * j + (i & 1);
+                float t = acc[4 * j + i];
+                if (p.mask && valid[e] && co < p.Cout && !(__ldg(p.mask + off[e] + co) >= 0.f)) t *= p.mslope;   // as pad_leaky_bias_bwd_kernel
+                v[e][i & 1] = valid[e] ? t : 0.f;
+            }
+            if (p.stats) tc::stats_accumulate8(v[0], v[1], sm_stats, BN, 8 * j, p.stats_sum != 0);
+            const int co = cq + 8 * j;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                if (!valid[e]) continue;
+                float* dst = out + off[e];
+                float o0 = v[e][0], o1 = v[e][1];
+                if (vec && co + 1 < p.Cout) {
+                    if (bias) { o0 += __ldg(bias + co); o1 += __ldg(bias + co + 1); }
+                    o0 = o0 >= 0.f ? o0 : o0 * p.leaky;
+                    o1 = o1 >= 0.f ? o1 : o1 * p.leaky;
+                    *reinterpret_cast<float2*>(dst + co) = make_float2(o0, o1);
+                } else {
+                    if (co < p.Cout) {
+                        o0 += bias ? __ldg(bias + co) : 0.f;
+                        dst[co] = o0 >= 0.f ? o0 : o0 * p.leaky;
+                    }
+                    if (co + 1 < p.Cout) {
+                        o1 += bias ? __ldg(bias + co + 1) : 0.f;
+                        dst[co + 1] = o1 >= 0.f ? o1 : o1 * p.leaky;
                     }
                 }
             }
-            if (p.stats) tc::stats_flush(sm_stats, BN, p.stats, p.Cout, c0, threadIdx.x - 64);
         }
+        if (p.stats) tc::stats_flush(sm_stats, BN, p.stats, p.Cout, c0, threadIdx.x - 128, 256);
     }
-    tc::tc_fence_before();
+}
+
+// [taps][K][N] -> [taps][N][K]: the input gradient's weights arrive cin-major (N-major B operand), wgmma reads tf32 K-major
+__global__ void transpose_taps_kernel(const float* __restrict__ in, float* __restrict__ out, int K, int N) {
+    __shared__ float t[32][33];
+    const int tap = blockIdx.z, k0 = blockIdx.y * 32, n0 = blockIdx.x * 32;
+    const float* src = in + (size_t)tap * K * N;
+    float* dst = out + (size_t)tap * K * N;
+    for (int i = threadIdx.y; i < 32; i += blockDim.y)
+        if (k0 + i < K && n0 + (int)threadIdx.x < N) t[i][threadIdx.x] = src[(size_t)(k0 + i) * N + n0 + threadIdx.x];
     __syncthreads();
-    if (warp == 2) tc::tmem_dealloc<TCOLS>(tmem_acc);
+    for (int i = threadIdx.y; i < 32; i += blockDim.y)
+        if (n0 + i < N && k0 + (int)threadIdx.x < K) dst[(size_t)(n0 + i) * K + k0 + threadIdx.x] = t[threadIdx.x][i];
 }
 
 // ----------------------------------------------------------------------------------------------
 // wgrad:  dW[co, ci, r, s] += sum_{n,y,x} dY[n, y, x, co] * X[n, st*y + r - pad_y, st*x + s, ci]      (NHWC operands)
 // GEMM with M = Cout (128), N = Cin (BN), K = output pixels.  In NHWC the reduction index (pixel) is the SLOW index
-// of both operands, i.e. they are M/N-major: a K slice is a BWk x BHk box of 32 output pixels, loaded as 32-channel
-// wide TMA boxes ([32 pixels][32 channels], CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B) — four for dY, BN/32 for X, the X
-// boxes shifted by the tap on the OUTER dims (zero fill = padding, element strides for stride 2).  tcgen05.mma reads
-// them through MN-major shared-memory descriptors (layout SWIZZLE_128B_BASE32B — the 32-bit transpose layout: 4-row
-// atoms, SBO 512 B, LBO 4096 B; plain SWIZZLE_128B yields zeros for tf32, measured), so no NCHW copy is ever made.
-// One CTA per (co tile, ci tile, tap, K split); partial sums are reduced into dW with red.global.add.f32.
+// of both operands, i.e. they are M/N-major, and wgmma reads tf32 operands K-major only: a K slice is a BWk x BHk box of
+// 32 output pixels, loaded by TMA as [32 pixels][32 channels] boxes (four for dY, BN/32 for X, the X boxes shifted by the
+// tap on the OUTER dims: zero fill = padding, element strides for stride 2) into an NRAW-deep staging ring, and the
+// producer warpgroup rewrites each slice K-major into the swizzled stage the consumers read (tc::transpose_slice_k128).
+// No NCHW copy is ever made.  T > 1 (row of taps): a K slice is a 32-pixel row segment, the X box is a window of
+// 32 + T - 1 (rounded to 36) pixels, and the producer writes T K-major B tiles from it — tap t is the window shifted by t
+// pixels — which share the staged dY tile: T accumulators per consumer warpgroup, T taps per byte of dY.  One CTA per
+// (co tile, ci tile, tap group, K split); partial sums are reduced into dW with global atomics.
 // ----------------------------------------------------------------------------------------------
 struct WgradParams {
     int N, Hout, Wout, Cout, Cin;
@@ -441,191 +248,171 @@ struct WgradParams {
     int kx, ky;                    // K slices along x and y per image
     int kh, kw, pad_y, st;
     int xoff;                      // the convolution reads x from column xoff on (a caller-side crop of the padded input)
-    int splits;                    // K splits (gridDim.z / taps)
-    int fold;                      // > 0: X is the raw stem input [N,H,W,8]; 32-"channel" block b = image rows y - fold_pad + 4b .. + 3
+    int splits;                    // K splits (gridDim.z / tap groups)
     int tapmajor;                  // dW layout: 0 = [Cout][Cin][kh][kw], 1 = tap-major [kh*kw][Cout][Cin] (the F layout)
     int tstep;                     // taps of one CTA are s0, s0 + tstep, ... (1: adjacent taps of a stride-1 conv,
-                                   // 2: taps of equal parity of a stride-2 conv = adjacent rows of the strided window)
+                                   // 2: taps of equal parity of a stride-2 conv = adjacent pixels of the strided window)
 };
 
-template <int BN, int T>
-struct WgradSmem {
+template <int BN, int STAGES, int NRAW, int T>
+struct WSmem {
     static constexpr int A_BYTES = BM * BK * 4;
-    static constexpr int B_BYTES = (BN / 32) * (T == 1 ? 32 : 36) * 128;
-    static constexpr int STAGE_BYTES = ((A_BYTES + B_BYTES + 1023) / 1024) * 1024;
+    static constexpr int STAGE_BYTES = A_BYTES + T * BN * BK * 4;
+    static constexpr int WROWS = T == 1 ? 32 : 36;                      // X pixels per 32-channel block of a raw slice
+    static constexpr int RAW_X = (BN / 32) * WROWS * 128;
+    static constexpr int RAW_BYTES = (A_BYTES + RAW_X + 1023) / 1024 * 1024;
+    static constexpr int TOTAL = STAGES * STAGE_BYTES + NRAW * RAW_BYTES + 1024 + 256;
 };
 
-// T > 1: the CTA computes T horizontally adjacent taps (r, s0 .. s0+T-1) at once.  They share the dY tile, and their X
-// operands are views of ONE staged window of 32 + T - 1 (rounded to 36) pixels shifted by s rows — T accumulators of BN
-// columns in TMEM, ~T x fewer bytes per MAC through the L2 -> SM path that bounds this kernel (profiles/r1_conv_layers.md).
-template <int BN, int STAGES, int T>
-__global__ void __launch_bounds__(NTHREADS, (T * BN <= 256 && STAGES <= 4) ? 2 : 1)
-wgrad_tf32_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x,
-                  const WgradParams p, float* __restrict__ dw) {
-    constexpr int BLK = BK * 32 * 4;                      // dY: one [32 pixels][32 channels] box = 4 KB
-    constexpr int WROWS = T == 1 ? 32 : 36;               // X window rows (pixels) per 32-channel block
-    constexpr int XBLK = WROWS * 128;
-    using S = WgradSmem<BN, T>;
+template <int BN, int STAGES, int NRAW, int T>
+__global__ void __launch_bounds__(NTHREADS, 1)
+wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x,
+                   const WgradParams p, float* __restrict__ dw) {
+    using S = WSmem<BN, STAGES, NRAW, T>;
     extern __shared__ unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * S::STAGE_BYTES);
+    unsigned char* raw = base + STAGES * S::STAGE_BYTES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(raw + NRAW * S::RAW_BYTES);
     uint64_t* empty = full + STAGES;
-    uint64_t* acc_full = empty + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
+    uint64_t* rawfull = empty + STAGES;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int co0 = blockIdx.x * BM, ci0 = blockIdx.y * BN;
-    const int gpr = p.kw / T;                             // tap groups per kernel row
+    const int gpr = p.kw / T;                             // tap groups per filter row
     const int groups = p.kh * gpr;
     const int grp = blockIdx.z % groups, split = blockIdx.z / groups;
-    const int r = grp / gpr, s = grp % gpr;               // first tap of the group (tstep 1: gpr is 1 or kw; tstep 2: parity)
+    const int r = grp / gpr, s = grp % gpr;               // filter row and first tap of the group
     const int per_img = p.kx * p.ky;
     const long long ktotal = (long long)p.N * per_img;
     const long long k_lo = ktotal * split / p.splits, k_hi = ktotal * (split + 1) / p.splits;
     const int KI = (int)(k_hi - k_lo);
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tc::tma_prefetch_desc(&tmap_dy);
         tc::tma_prefetch_desc(&tmap_x);
-    }
-    if (warp == 1 && lane == 0) {
         for (int i = 0; i < STAGES; ++i) {
-            tc::mbar_init(full + i, 1);
-            tc::mbar_init(empty + i, 1);
+            tc::mbar_init(full + i, 128);
+            tc::mbar_init(empty + i, 2);
         }
-        tc::mbar_init(acc_full, 1);
+        for (int i = 0; i < NRAW; ++i) tc::mbar_init(rawfull + i, 1);
         tc::fence_barrier_init();
     }
-    constexpr uint32_t TCOLS = T * BN <= 64 ? 64 : T * BN <= 128 ? 128 : T * BN <= 256 ? 256 : 512;
-    if (warp == 2) tc::tmem_alloc<TCOLS>(tmem_slot);
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_acc = *tmem_slot;
+    const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
 
-    if (warp == 0 || warp == 6) {           // warp 0 streams dY, warp 6 streams X (two TMA issue lanes, one barrier)
-        {
-            const uint32_t leader = tc::elect_one();          // convergent producer loops: one elected lane arrives / issues the copies
-            for (int it = 0; it < KI; ++it) {
-                const int st = it % STAGES, ph = (it / STAGES) & 1;
-                tc::mbar_wait(empty + st, ph ^ 1);
-                const long long k = k_lo + it;
-                const int n = (int)(k / per_img), rem = (int)(k % per_img);
-                const int x0 = (rem % p.kx) * p.BWk, y0 = (rem / p.kx) * p.BHk;
-                unsigned char* a = base + st * S::STAGE_BYTES;
-                // channels are split as (32, C/32) in the tensor maps: ONE 5-D box lands all 32-channel blocks back to back
-                if (warp == 0) {
-                    tc::mbar_arrive_expect_tx_if(leader, full + st, S::STAGE_BYTES);
-                    tc::tma_load_5d_if(leader, a, &tmap_dy, full + st, 0, x0, y0, n, co0 / 32);
-                } else if (p.fold) {      // (c, row, x, n) boxes of 4 rows x 8 channels per pixel: one per 32-"channel" block
-#pragma unroll
-                    for (int blk = 0; blk < BN / 32; ++blk)
-                        tc::tma_load_4d_if(leader, a + S::A_BYTES + blk * XBLK, &tmap_x, full + st, 0, y0 - p.pad_y + 4 * (ci0 / 32 + blk), x0 + s + p.xoff, n);
-                } else {
-                    tc::tma_load_5d_if(leader, a + S::A_BYTES, &tmap_x, full + st, 0, p.st * x0 + s + p.xoff, p.st * y0 + r - p.pad_y, n, ci0 / 32);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // convergent issue loop (tc_common.cuh "MMA issue from a CONVERGENT warp"): all lanes walk it, one elected lane issues
-        const uint32_t leader = tc::elect_one();
-        const uint32_t tmem_u = tc::warp_uniform(tmem_acc);
-        constexpr uint32_t idesc = tc::umma_idesc_tf32(BM, BN, true, true);
+    if (wg == 0) {
+        auto issue = [&](int j) {
+            if (tid != 0) return;
+            const long long k = k_lo + j;
+            const int n = (int)(k / per_img), rem = (int)(k % per_img);
+            const int x0 = (rem % p.kx) * p.BWk, y0 = (rem / p.kx) * p.BHk;
+            const int rb = j % NRAW;
+            unsigned char* dst = raw + rb * S::RAW_BYTES;
+            // channels are split as (32, C/32) in the tensor maps: ONE 5-D box lands all 32-channel blocks back to back
+            tc::mbar_arrive_expect_tx(rawfull + rb, S::A_BYTES + S::RAW_X);
+            tc::tma_load_5d(dst, &tmap_dy, rawfull + rb, 0, x0, y0, n, co0 / 32);
+            tc::tma_load_5d(dst + S::A_BYTES, &tmap_x, rawfull + rb, 0, p.st * x0 + s + p.xoff, p.st * y0 + r - p.pad_y, n, ci0 / 32);
+        };
+        for (int j = 0; j < NRAW - 1 && j < KI; ++j) issue(j);
         for (int it = 0; it < KI; ++it) {
-            const int st = it % STAGES, ph = (it / STAGES) & 1;
-            tc::mbar_wait(full + st, ph);
-            tc::tc_fence_after();
-            const uint32_t a = tc::smem_u32(base + st * S::STAGE_BYTES);
-            const uint64_t da0 = tc::umma_desc_mn128(a, BLK, 512), db0 = tc::umma_desc_mn128(a + S::A_BYTES, XBLK, 512);
+            if (it + NRAW - 1 < KI) issue(it + NRAW - 1);     // its buffer was last read in iteration it - 1
+            const int rb = it % NRAW, st = it % STAGES;
+            tc::mbar_wait(rawfull + rb, (it / NRAW) & 1);
+            tc::mbar_wait(empty + st, ((it / STAGES) & 1) ^ 1);
+            const float* src = reinterpret_cast<const float*>(raw + rb * S::RAW_BYTES);
+            unsigned char* dst = base + st * S::STAGE_BYTES;
+            tc::transpose_slice_k128(src, dst, BM, tid);
 #pragma unroll
             for (int t = 0; t < T; ++t)
-#pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k)      // 8 pixel rows (two 4-row swizzle atoms, 1024 B) per MMA
-                    tc::umma_tf32_words_if(leader, tmem_u + t * BN, tc::desc_lo(da0) + k * (1024 >> 4), tc::desc_hi(da0),
-                                           tc::desc_lo(db0) + (((t + 8 * k) * 128) >> 4), tc::desc_hi(db0), idesc, (it | k) ? 1u : 0u);
-            tc::umma_commit_if(leader, empty + st);
+                tc::transpose_slice_k128(src + S::A_BYTES / 4, dst + S::A_BYTES + t * (BN * 128), BN, tid, S::WROWS * 32, t);
+            tc::fence_proxy_async();
+            tc::mbar_arrive(full + st);
+            tc::named_sync(2, 128);                               // the raw slice is consumed before it is loaded again
         }
-        tc::umma_commit_if(leader, acc_full);
-    } else if (KI > 0) {
-        const int q = warp & 3;
-        const int co = co0 + q * 32 + lane;
-        tc::mbar_wait(acc_full, 0);
-        tc::tc_fence_after();
-#pragma unroll 1
+        return;
+    }
+
+    const int h = wg - 1, lane = tid & 31;
+    float acc[T][BN / 2];
+#pragma unroll
+    for (int t = 0; t < T; ++t)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[t][i] = 0.f;
+    for (int it = 0; it < KI; ++it) {
+        const int st = it % STAGES;
+        tc::mbar_wait(full + st, (it / STAGES) & 1);
+        const uint32_t a = tc::smem_u32(base + st * S::STAGE_BYTES), b = a + S::A_BYTES;
+        tc::wgmma_fence();
+#pragma unroll
         for (int t = 0; t < T; ++t)
-#pragma unroll 1
-            for (int c = 0; c < BN; c += 32) {
-                float v[32];
-                tc::tmem_ld32(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)(t * BN + c), v);
-                if (co < p.Cout) {
-                    if (p.tapmajor) {       // 32 consecutive input channels of one (tap, co) row: 8 x 16-byte reductions
-                        float* row = dw + ((size_t)(r * p.kw + s + t * p.tstep) * p.Cout + co) * p.Cin + ci0 + c;
 #pragma unroll
-                        for (int j = 0; j < 32; j += 4)
-                            if (ci0 + c + j < p.Cin) atomicAdd(reinterpret_cast<float4*>(row + j), make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]));
-                    } else {
+            for (int k = 0; k < BK / MMA_K; ++k)
+                tc::Wgmma<BN>::mma(acc[t], tc::desc_k128(a + h * (64 * 128) + k * MMA_K * 4),
+                                   tc::desc_k128(b + t * (BN * 128) + k * MMA_K * 4), (it | k) ? 1u : 0u);
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();
+        if (it > 0 && tid == 0) tc::mbar_arrive(empty + (it - 1) % STAGES);
+    }
+    tc::wgmma_wait<0>();
+    if (KI == 0) return;
+    if (tid == 0) tc::mbar_arrive(empty + (KI - 1) % STAGES);
+    const int co_a = co0 + h * 64 + (tid >> 5) * 16 + (lane >> 2);
+    const int cq = ci0 + 2 * (lane & 3);
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int ci = ci0 + c + j;
-                            if (ci < p.Cin) atomicAdd(dw + (((size_t)co * p.Cin + ci) * p.kh + r) * p.kw + s + t * p.tstep, v[j]);
-                        }
-                    }
+    for (int t = 0; t < T; ++t) {
+        const int sc = s + t * p.tstep;                       // filter column of accumulator t
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int co = co_a + 8 * e;
+            if (co >= p.Cout) continue;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int ci = cq + 8 * j;
+                if (ci >= p.Cin) continue;                        // Cin % 32 == 0: ci + 1 < Cin as well
+                const float v0 = acc[t][4 * j + 2 * e], v1 = acc[t][4 * j + 2 * e + 1];
+                if (p.tapmajor) {
+                    atomicAdd(reinterpret_cast<float2*>(dw + ((size_t)(r * p.kw + sc) * p.Cout + co) * p.Cin + ci), make_float2(v0, v1));
+                } else {
+                    atomicAdd(dw + (((size_t)co * p.Cin + ci) * p.kh + r) * p.kw + sc, v0);
+                    atomicAdd(dw + (((size_t)co * p.Cin + ci + 1) * p.kh + r) * p.kw + sc, v1);
                 }
             }
+        }
     }
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tc::tmem_dealloc<TCOLS>(tmem_acc);
 }
 
-template <int BN, int STAGES, int T>
+template <int BN, int STAGES, int NRAW, int T>
 int launch_wgrad(const CUtensorMap& mdy, const CUtensorMap& mx, const WgradParams& p, float* dw, dim3 grid, cudaStream_t st) {
-    constexpr int WROWS = T == 1 ? 32 : 36;
-    constexpr int STAGE = ((BM * BK * 4 + (BN / 32) * WROWS * 128 + 1023) / 1024) * 1024;
-    constexpr int TOTAL = STAGES * STAGE + 1024 + 256;
-    static_assert(TOTAL <= 227 * 1024, "wgrad pipeline does not fit shared memory");
-    B3D_CUDA_OK(cudaFuncSetAttribute(wgrad_tf32_kernel<BN, STAGES, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, TOTAL));
-    wgrad_tf32_kernel<BN, STAGES, T><<<grid, NTHREADS, TOTAL, st>>>(mdy, mx, p, dw);
+    using S = WSmem<BN, STAGES, NRAW, T>;
+    static_assert(S::TOTAL <= 227 * 1024, "wgrad pipeline does not fit shared memory");
+    B3D_CUDA_OK(cudaFuncSetAttribute(wgrad_wgmma_kernel<BN, STAGES, NRAW, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+    wgrad_wgmma_kernel<BN, STAGES, NRAW, T><<<grid, NTHREADS, S::TOTAL, st>>>(mdy, mx, p, dw);
     B3D_LAUNCH_OK();
-    b3d::add_variant("wgrad_tf32<%d,%d,%d>", BN, STAGES, T);
+    b3d::add_variant("wgrad_wgmma<%d,%d,%d,%d>", BN, STAGES, NRAW, T);
     return B3D_OK;
 }
 
-template <int BN, int STAGES, bool WMN, int MINB>
-int launch(const CUtensorMap& mx, const CUtensorMap& mw, const ConvParams& p, const float* bias, float* out,
-           int tiles, cudaStream_t st) {
-    using S = Smem<BN, STAGES>;
-    B3D_CUDA_OK(cudaFuncSetAttribute(conv_tf32_kernel<BN, STAGES, WMN, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     S::TOTAL));
-    dim3 grid(tiles, b3d::ceil_div(p.Cout, BN));
-    conv_tf32_kernel<BN, STAGES, WMN, MINB><<<grid, NTHREADS, S::TOTAL, st>>>(mx, mw, p, bias, out);
+template <int BN, int STAGES, int KW = 1>
+int launch_conv(const CUtensorMap& mx, const CUtensorMap& mw, const ConvParams& p, const float* bias, float* out, int tiles,
+                cudaStream_t st) {
+    using S = CSmem<BN, STAGES, KW>;
+    static_assert(S::TOTAL <= 227 * 1024, "conv pipeline does not fit shared memory");
+    B3D_CUDA_OK(cudaFuncSetAttribute(conv_wgmma_kernel<BN, STAGES, KW>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+    const int work = tiles * b3d::ceil_div(p.Cout, BN) * p.ncls;
+    const int sms = tc::num_sms();
+    conv_wgmma_kernel<BN, STAGES, KW><<<work < sms ? work : sms, NTHREADS, S::TOTAL, st>>>(mx, mw, p, bias, out, tiles, work);
     B3D_LAUNCH_OK();
-    b3d::add_variant("conv_tf32<%d,%d,%d,%d>", BN, STAGES, (int)WMN, MINB);
+    if (KW > 1) b3d::add_variant("conv_wgmma_rowwin<%d,%d,%d>", BN, KW, STAGES);
+    else b3d::add_variant("conv_wgmma<%d,%d>", BN, STAGES);
     return B3D_OK;
 }
 
-template <int BN, int STAGES, bool WMN, int R>
-int launch_persistent(const CUtensorMap& mx, const CUtensorMap& mw, const ConvParams& p, const float* bias, float* out,
-                      int tiles, cudaStream_t st) {
-    using S = PSmem<BN, STAGES, R>;
-    static_assert(S::TOTAL <= 227 * 1024, "persistent conv pipeline does not fit shared memory");
-    B3D_CUDA_OK(cudaFuncSetAttribute(conv_tf32_persistent_kernel<BN, STAGES, WMN, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    const int groups = b3d::ceil_div(tiles, R);
-    const int work = groups * b3d::ceil_div(p.Cout, BN) * p.ncls;
-    const int slots = S::CTAS_PER_SM * 148;
-    const int grid = work < slots ? work : slots;
-    conv_tf32_persistent_kernel<BN, STAGES, WMN, R><<<grid, PTHREADS, S::TOTAL, st>>>(mx, mw, p, bias, out, tiles, groups, work);
-    B3D_LAUNCH_OK();
-    b3d::add_variant("conv_tf32_persistent<%d,%d,%d,%d>", BN, STAGES, (int)WMN, R);
-    return B3D_OK;
-}
-
-template <bool WMN>
-int dispatch_persistent(int BN, int stack, const CUtensorMap& mx, const CUtensorMap& mw, const ConvParams& p, const float* bias,
-                        float* out, int tiles, cudaStream_t st) {
-    if (BN == 256) return launch_persistent<256, 4, WMN, 1>(mx, mw, p, bias, out, tiles, st);
-    if (BN == 128) return stack ? launch_persistent<128, 4, WMN, 2>(mx, mw, p, bias, out, tiles, st) : launch_persistent<128, 3, WMN, 1>(mx, mw, p, bias, out, tiles, st);
-    return stack ? launch_persistent<64, 3, WMN, 4>(mx, mw, p, bias, out, tiles, st) : launch_persistent<64, 4, WMN, 1>(mx, mw, p, bias, out, tiles, st);
+// row-window launch of a filter grid of rows of kw horizontally consecutive taps (stages: as many as fit ~200 KB)
+template <int BN>
+int launch_rowwin(int kw, const CUtensorMap& mx, const CUtensorMap& mw, const ConvParams& p, const float* bias, float* out, int tiles,
+                  cudaStream_t st) {
+    if (kw == 2) return launch_conv<BN, BN == 64 ? 5 : 4, 2>(mx, mw, p, bias, out, tiles, st);
+    if (kw == 3) return launch_conv<BN, BN == 64 ? 4 : 3, 3>(mx, mw, p, bias, out, tiles, st);
+    return launch_conv<BN, BN == 64 ? 3 : 2, 5>(mx, mw, p, bias, out, tiles, st);
 }
 
 int pow2_floor(int v) {
@@ -639,7 +426,7 @@ int pow2_floor(int v) {
 extern "C" {
 
 // x   [N, H, W, Cin]  NHWC fp32, Cin % 32 == 0
-// wt  [ntaps, Cout, Cin] fp32 (tap-major, K-major rows)
+// wt  [ntaps, Cout, Cin] fp32 (tap-major, K-major rows); w_cin_major: [ntaps, Cin, Cout]
 // out [N, OH, OW, OC]; the tile grid covers (Hout, Wout) logical outputs, written to (osy*y+ooy, osx*x+oox)
 int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* out, int N, int H, int W, int Cin,
                     int Hout, int Wout, int Cout, int ntaps, const int* dy, const int* dx, int sy, int sx, int OH,
@@ -658,7 +445,6 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
     B3D_CHECK_ALIGNED(wt);
     b3d::clear_variant();
 
-    static const int persist_env = getenv("B3D_CONV_PERSIST") ? atoi(getenv("B3D_CONV_PERSIST")) : 1;
     const float* mask = opts ? opts->mask : nullptr;
     const float mslope = opts ? opts->mask_slope : 1.f;
     const int stats_sum = (opts && opts->stats_sum_only) ? 1 : 0;
@@ -671,8 +457,6 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
     int cooy[4] = {ooy, ooy, ooy, ooy}, coox[4] = {oox, oox, oox, oox};
     for (int c = 0; c < ncls && ncls > 1; ++c) { cooy[c] = opts->class_ooy[c]; coox[c] = opts->class_oox[c]; }
     B3D_REQUIRE(xpitch >= W && (fold_kh == 0 || xpitch == W), B3D_EINVAL, "b3d_conv2d_tf32: x_row_pitch=%d must be >= W=%d (and absent with the on-the-fly fold)", xpitch, W);
-    // statistics epilogue / on-the-fly fold / fused activation adjoint: persistent kernels
-    const int persist = persist_env || stats != nullptr || fold_kh > 0 || mask != nullptr || ncls > 1;
     if (fold_kh > 0) {
         // x is the RAW stem input [N, H, W, 8]; the convolution is kh x kw with the kh rows folded into the K dimension:
         // Cin = 32 * ceil(8 kh / 32) "channels", taps = the kw horizontal ones (dy ignored), zero rows = the y padding
@@ -680,69 +464,61 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
                     B3D_EINVAL, "b3d_conv2d_tf32: on-the-fly fold needs 8 input channels, stride 1 and Wout %% 128 == 0 (Wout=%d)", Wout);
     }
     B3D_REQUIRE(!stats || mask || (osy == 1 && osx == 1), B3D_EINVAL, "b3d_conv2d_tf32: statistics need a dense output");
-    static const int wide = getenv("B3D_CONV_BN256") ? atoi(getenv("B3D_CONV_BN256")) : 1;
-    // 256-wide output-channel tiles halve the input-tile bytes per FLOP through the L2 -> SM fabric (the bound of the
-    // per-tap formulation, profiles/r1_c_*.md) when there are >= 256 output channels and enough tiles to fill the GPU
-    const bool bn256 = persist && wide && Cout % 256 == 0 && (long long)N * Hout * Wout / BM * (Cout / 256) * ncls >= 148;
+    // 256-wide output-channel tiles halve the input-tile bytes per FLOP through the L2 -> SM path when there are >= 256
+    // output channels and enough work items to give every SM one
+    const bool bn256 = Cout % 256 == 0 && (long long)N * Hout * Wout / BM * (Cout / 256) * ncls >= tc::num_sms();
     const int BN = bn256 ? 256 : Cout > 64 ? 128 : 64;
     cudaStream_t st = (cudaStream_t)stream;
+    // wgmma reads tf32 operands K-major only: cin-major weights (the input gradient's, [ntaps, Cin, Cout]) are transposed
+    // once per call into a stream-ordered temporary
+    float* wk = nullptr;
+    if (w_cin_major) {
+        B3D_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&wk), (size_t)wtaps_total * Cin * Cout * sizeof(float), st));
+        transpose_taps_kernel<<<dim3(b3d::ceil_div(Cout, 32), b3d::ceil_div(Cin, 32), wtaps_total), dim3(32, 8), 0, st>>>(wt, wk, Cin, Cout);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) {
+            cudaFreeAsync(wk, st);
+            b3d::set_error("b3d_conv2d_tf32: weight transpose launch failed: %s", cudaGetErrorString(e));
+            return B3D_ECUDA;
+        }
+        b3d::count_launch();
+    }
+    const float* wkm = w_cin_major ? wk : wt;
     CUtensorMap mw;
-    if (w_cin_major) {        // wt [ntaps, Cin, Cout]: the B operand is N-major (no weight transpose for dgrad)
-        B3D_REQUIRE(Cout % 4 == 0, B3D_EINVAL, "b3d_conv2d_tf32: Cout=%d must be a multiple of 4 for cin-major weights", Cout);
-        const uint64_t dims[3] = {(uint64_t)Cout, (uint64_t)Cin, (uint64_t)wtaps_total};
-        const uint64_t strides[2] = {(uint64_t)Cout * 4, (uint64_t)Cout * Cin * 4};
-        const uint32_t box[3] = {32, (uint32_t)BK, 1};
-        if (int rc = tc::make_tmap_f32(&mw, wt, 3, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return rc;
-    } else {
+    {
         const uint64_t dims[3] = {(uint64_t)Cin, (uint64_t)Cout, (uint64_t)wtaps_total};
         const uint64_t strides[2] = {(uint64_t)Cin * 4, (uint64_t)Cout * Cin * 4};
         const uint32_t box[3] = {(uint32_t)BK, (uint32_t)BN, 1};
-        if (int rc = tc::make_tmap_f32(&mw, wt, 3, dims, strides, box)) return rc;
+        if (int rc = tc::make_tmap_f32(&mw, wkm, 3, dims, strides, box)) {
+            if (wk) cudaFreeAsync(wk, st);
+            return rc;
+        }
+    }
+
+    // Filter-grid detection for the row window (stride 1, no fold): every class has kh rows of kw in {2, 3, 5} horizontally
+    // consecutive taps (dx step +-1) whose weight taps form an arithmetic progression (step 1, or 2 for the stride-2
+    // input gradient's parity classes), the same column pattern in every class.
+    int g_kw = 0, g_step = 1, g_wstep = 1;
+    if (sy == 1 && sx == 1 && fold_kh == 0) {
+        int kw_ = 1;
+        while (kw_ < tpc && dy[kw_] == dy[0]) ++kw_;
+        const int step = kw_ > 1 ? dx[1] - dx[0] : 1;
+        const int wstep = (wtap && kw_ > 1) ? wtap[1] - wtap[0] : 1;
+        bool grid_ok = tpc % kw_ == 0 && (kw_ == 2 || kw_ == 3 || kw_ == 5) && (step == 1 || step == -1) && wstep >= 1 && wstep <= 2 &&
+                       (ncls == 1 || wtap != nullptr);
+        for (int t = 0; grid_ok && t < ntaps; ++t) {
+            const int tc_ = t % tpc, t0 = t - tc_;
+            grid_ok = dy[t] == dy[t0 + (tc_ / kw_) * kw_] && dx[t] == dx[0] + (tc_ % kw_) * step;
+            if (wtap) grid_ok = grid_ok && wtap[t] == wtap[t0 + (tc_ / kw_) * kw_] + (tc_ % kw_) * wstep;
+        }
+        if (grid_ok && BN <= 128) { g_kw = kw_; g_step = step; g_wstep = wstep; }
     }
 
     // One launch covers output columns [xlo, xhi).  A width of "power of two + a few columns" (dgrad of an x-padded
     // input: 130, 66, 34 ...; stride-2 parity classes: 129, 65 ...) would leave a second, almost empty 128-pixel tile in
     // every row, so the remainder columns get a narrow strip launch of their own.
-    // filter-grid detection for the row-window kernel (tc_conv3.cu): kh rows of kw horizontally consecutive taps; the weight
-    // taps of a row form an arithmetic progression (identity, or the stride-2 dgrad parity classes' tap lists)
-    int g_kw = 0, g_kh = 0, g_step = 0, g_wstep = 1;
-    if (sy == 1 && sx == 1 && !w_cin_major && fold_kh == 0) {
-        int kw_ = 1;
-        while (kw_ < tpc && dy[kw_] == dy[0]) ++kw_;
-        const int step = kw_ > 1 ? dx[1] - dx[0] : 1;
-        const int wstep = (wtap && kw_ > 1) ? wtap[1] - wtap[0] : 1;
-        bool grid_ok = tpc % kw_ == 0 && tpc / kw_ <= 5 && (kw_ == 2 || kw_ == 3 || kw_ == 5) && (step == 1 || step == -1) &&
-                       wstep >= 1 && wstep <= 2 && (osy == osx) && (osy == 1 || osy == 2) && (ncls == 1 || wtap != nullptr);
-        for (int t = 0; grid_ok && t < ntaps; ++t) {             // every class: the same column pattern, its own rows / weight taps
-            const int tc_ = t % tpc, t0 = t - tc_;
-            grid_ok = dy[t] == dy[t0 + (tc_ / kw_) * kw_] && dx[t] == dx[0] + (tc_ % kw_) * step;
-            if (wtap) grid_ok = grid_ok && wtap[t] == wtap[t0 + (tc_ / kw_) * kw_] + (tc_ % kw_) * wstep;
-        }
-        static const int rowwin_env = getenv("B3D_CONV_ROWWIN") ? atoi(getenv("B3D_CONV_ROWWIN")) : 1;
-        if (grid_ok && rowwin_env) { g_kw = kw_; g_kh = tpc / kw_; g_step = step; g_wstep = wstep; }
-    }
     auto run = [&](int xlo, int xhi) -> int {
         const int wspan = xhi - xlo;
-        if (g_kw && wspan >= BM) {
-            b3d::RowWinArgs a{};
-            a.x = x; a.wt = wt; a.bias = bias; a.out = out;
-            a.N = N; a.H = H; a.W = W; a.Cin = Cin; a.Hout = Hout; a.Cout = Cout; a.xlo = xlo; a.xhi = xhi;
-            a.kh = g_kh; a.kw = g_kw; a.ncls = ncls;
-            a.dx0 = g_step > 0 ? dx[0] : dx[g_kw - 1];
-            for (int t = 0; t < g_kw; ++t) a.shift[t] = dx[t] - a.dx0;
-            a.OH = OH; a.OW = OW; a.OC = OC; a.leaky = leaky; a.stats = stats;
-            a.osy = osy; a.osx = osx; a.wtaps_total = wtaps_total; a.wtap_step = g_wstep;
-            a.mask = mask; a.mslope = mslope; a.stats_sum = stats_sum; a.xpitch = xpitch;
-            for (int c = 0; c < ncls; ++c) {
-                a.ooy[c] = cooy[c]; a.oox[c] = coox[c];
-                for (int r = 0; r < g_kh; ++r) {
-                    a.dy[c][r] = dy[c * tpc + r * g_kw];
-                    a.wtap0[c][r] = wtap ? wtap[c * tpc + r * g_kw] : r * g_kw;
-                }
-            }
-            const int rc = b3d::conv_rowwin_launch(a, st);
-            if (rc <= 0) return rc;                           // launched (0) or a real error (< 0); 1 = not covered
-        }
         ConvParams p{};
         p.N = N; p.Hout = Hout; p.Wout = xhi; p.Cout = Cout; p.xbase = xlo;
         p.BW = pow2_floor(wspan < BM ? wspan : BM);
@@ -754,13 +530,29 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
         p.ntaps = tpc; p.kslices = Cin / BK; p.sy = sy; p.sx = sx; p.ncls = ncls;
         for (int t = 0; t < ntaps; ++t) { p.dy[t] = dy[t]; p.dx[t] = dx[t]; p.wtap[t] = wtap ? wtap[t] : t; }
         for (int c = 0; c < 4; ++c) { p.cooy[c] = cooy[c]; p.coox[c] = coox[c]; }
-        p.OH = OH; p.OW = OW; p.OC = OC; p.osy = osy; p.osx = osx; p.ooy = ooy; p.oox = oox;
+        p.OH = OH; p.OW = OW; p.OC = OC; p.osy = osy; p.osx = osx;
         p.leaky = leaky;
-        p.dbg_lbo = 4096; p.dbg_sbo = 512; p.dbg_lt = 1;     // 32-bit MN-major: SWIZZLE_128B_BASE32B, 4-row atoms
         p.stats = stats;
         p.mask = mask; p.mslope = mslope; p.stats_sum = stats_sum;
         p.fold = fold_kh; p.fold_y0 = -fold_pad;
         CUtensorMap mx;
+        if (g_kw && wspan >= BM) {
+            // row window: tiles are 128-pixel row segments (BW = 128, BH = BI = 1); one A box = 128 + kw - 1 pixels of a row,
+            // one weight box = the kw weight tiles of a filter row (element stride g_wstep along the tap dimension)
+            p.dx0 = g_step > 0 ? dx[0] : dx[g_kw - 1];
+            for (int t = 0; t < g_kw; ++t) p.shift[t] = dx[t] - p.dx0;
+            const uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
+            const uint64_t strides[3] = {(uint64_t)Cin * 4, (uint64_t)xpitch * Cin * 4, (uint64_t)H * xpitch * Cin * 4};
+            const uint32_t box[4] = {(uint32_t)BK, (uint32_t)(BM + g_kw - 1), 1, 1};
+            if (int rc = tc::make_tmap_f32(&mx, x, 4, dims, strides, box)) return rc;
+            CUtensorMap mwr;
+            const uint64_t wdims[3] = {(uint64_t)Cin, (uint64_t)Cout, (uint64_t)wtaps_total};
+            const uint64_t wstrides[2] = {(uint64_t)Cin * 4, (uint64_t)Cout * Cin * 4};
+            const uint32_t wbox[3] = {(uint32_t)BK, (uint32_t)BN, (uint32_t)((g_kw - 1) * g_wstep + 1)};
+            const uint32_t wes[3] = {1, 1, (uint32_t)g_wstep};
+            if (int rc = tc::make_tmap_f32(&mwr, wkm, 3, wdims, wstrides, wbox, wes)) return rc;
+            return BN == 128 ? launch_rowwin<128>(g_kw, mx, mwr, p, bias, out, tiles, st) : launch_rowwin<64>(g_kw, mx, mwr, p, bias, out, tiles, st);
+        }
         if (fold_kh > 0) {
             B3D_REQUIRE(p.BH == 1 && p.BI == 1, B3D_EINVAL, "b3d_conv2d_tf32: on-the-fly fold needs one-row tiles");
             const uint64_t dims[4] = {8, (uint64_t)W, (uint64_t)H, (uint64_t)N};                    // the raw NHWC tensor
@@ -768,44 +560,42 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
             const uint32_t box[4] = {8, (uint32_t)p.BW, 4, 1};                                     // 4 image rows per K slice
             if (int rc = tc::make_tmap_f32(&mx, x, 4, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_32B)) return rc;
         } else {
-        const uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-        const uint64_t strides[3] = {(uint64_t)Cin * 4, (uint64_t)xpitch * Cin * 4, (uint64_t)H * xpitch * Cin * 4};
-        const uint32_t box[4] = {(uint32_t)BK, (uint32_t)(sx * (p.BW - 1) + 1), (uint32_t)(sy * (p.BH - 1) + 1), (uint32_t)p.BI};
-        const uint32_t es[4] = {1, (uint32_t)sx, (uint32_t)sy, 1};
-        if (int rc = tc::make_tmap_f32(&mx, x, 4, dims, strides, box, es)) return rc;
+            const uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
+            const uint64_t strides[3] = {(uint64_t)Cin * 4, (uint64_t)xpitch * Cin * 4, (uint64_t)H * xpitch * Cin * 4};
+            const uint32_t box[4] = {(uint32_t)BK, (uint32_t)(sx * (p.BW - 1) + 1), (uint32_t)(sy * (p.BH - 1) + 1), (uint32_t)p.BI};
+            const uint32_t es[4] = {1, (uint32_t)sx, (uint32_t)sy, 1};
+            if (int rc = tc::make_tmap_f32(&mx, x, 4, dims, strides, box, es)) return rc;
         }
-        // CTAs per SM x ring depth: short K loops (few taps x few channel slices) are dominated by pipeline fill, epilogue
-        // and store drain, which only OTHER resident CTAs can hide -> more, shallower CTAs (profiles/r1_c_*.md)
-        if (persist) {
-            // stacked pixel tiles (1 CTA / SM, deeper stages) once there is work for ~2 waves of them
-            static const int stack_env = getenv("B3D_CONV_STACK") ? atoi(getenv("B3D_CONV_STACK")) : 1;
-            const int R = BN == 128 ? 2 : 4;
-            const bool stack = stack_env && BN < 256 && (long long)b3d::ceil_div(tiles, R) * b3d::ceil_div(Cout, BN) * ncls >= 2 * 148;
-            return w_cin_major ? dispatch_persistent<true>(BN, stack, mx, mw, p, bias, out, tiles, st)
-                               : dispatch_persistent<false>(BN, stack, mx, mw, p, bias, out, tiles, st);
-        }
-        static const int occ_env = getenv("B3D_CONV_OCC") ? atoi(getenv("B3D_CONV_OCC")) : 0;
-        const int occ = occ_env ? occ_env : 2;
-        if (w_cin_major) {
-            if (BN == 128) return occ >= 3 ? launch<128, 2, true, 3>(mx, mw, p, bias, out, tiles, st) : launch<128, 3, true, 2>(mx, mw, p, bias, out, tiles, st);
-            return occ >= 4 ? launch<64, 2, true, 4>(mx, mw, p, bias, out, tiles, st)
-                 : occ == 3 ? launch<64, 3, true, 3>(mx, mw, p, bias, out, tiles, st) : launch<64, 4, true, 2>(mx, mw, p, bias, out, tiles, st);
-        }
-        if (BN == 128) return occ >= 3 ? launch<128, 2, false, 3>(mx, mw, p, bias, out, tiles, st) : launch<128, 3, false, 2>(mx, mw, p, bias, out, tiles, st);
-        return occ >= 4 ? launch<64, 2, false, 4>(mx, mw, p, bias, out, tiles, st)
-             : occ == 3 ? launch<64, 3, false, 3>(mx, mw, p, bias, out, tiles, st) : launch<64, 4, false, 2>(mx, mw, p, bias, out, tiles, st);
+        // ring depth: as many stages as fit next to the statistics / barrier area (~192 KB of operands)
+        if (BN == 256) return launch_conv<256, 4>(mx, mw, p, bias, out, tiles, st);
+        if (BN == 128) return launch_conv<128, 6>(mx, mw, p, bias, out, tiles, st);
+        return launch_conv<64, 8>(mx, mw, p, bias, out, tiles, st);
     };
     const int bw_full = pow2_floor(Wout < BM ? Wout : BM);
     const int rem = Wout % bw_full;
+    int rc;
     if (rem != 0 && rem * 8 <= bw_full && Wout > bw_full) {
-        if (int rc = run(0, Wout - rem)) return rc;
-        return run(Wout - rem, Wout);
+        rc = run(0, Wout - rem);
+        if (rc == 0) rc = run(Wout - rem, Wout);
+    } else {
+        rc = run(0, Wout);
     }
-    return run(0, Wout);
+    if (wk) cudaFreeAsync(wk, st);
+    return rc;
 }
 
-// dy [N,Hout,Wout,Cout], x [N,H,W,Cin] NHWC (x already padded along x; Cin, Cout multiples of 4),
-// dw [Cout,Cin,kh,kw] (accumulated into)
+// Stride-1 convolution over an x-padded input of row pitch P (include/b3d.h): the same work as b3d_conv2d_tf32 with
+// unit strides and a dense output, which stages the row windows / tap tiles itself.
+int b3d_conv2d_flat_tf32(const float* x, const float* wt, const float* bias, float* out, int N, int H, int P, int Cin,
+                         int Hout, int Wout, int Cout, int ntaps, const int* dy, const int* dx, int OH, int OW, int OC,
+                         float leaky, void* stream) {
+    B3D_REQUIRE(Wout <= P, B3D_EINVAL, "b3d_conv2d_flat_tf32: Wout=%d exceeds the input pitch %d", Wout, P);
+    return b3d_conv2d_tf32(x, wt, bias, out, N, H, P, Cin, Hout, Wout, Cout, ntaps, dy, dx, 1, 1, OH, OW, OC, 1, 1, 0, 0, leaky, 0,
+                           nullptr, 0, nullptr, 0, 0, nullptr, stream);
+}
+
+// dy [N,Hout,Wout,Cout], x [N,H,W,Cin] NHWC (x already padded along x; Cin, Cout multiples of 32),
+// dw [Cout,Cin,kh,kw] or tap-major [kh*kw,Cout,Cin] (accumulated into)
 int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, int N, int H, int W, int Cin, int Hout, int Wout,
                           int Cout, int kh, int kw, int pad_y, int stride, int x_off, int tap_major, int fold_kh, int dy_row_pitch,
                           void* stream) {
@@ -818,6 +608,9 @@ int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, int N, int
     B3D_CHECK_ALIGNED(dy);
     B3D_CHECK_ALIGNED(x);
     b3d::clear_variant();
+    B3D_REQUIRE(fold_kh == 0, B3D_EINVAL,
+                "b3d_conv2d_wgrad_tf32: the on-the-fly fold is not available for the weight gradient: pass the materialised fold");
+    if (tap_major) B3D_CHECK_ALIGNED(dw);
     WgradParams p{};
     p.N = N; p.Hout = Hout; p.Wout = Wout; p.Cout = Cout; p.Cin = Cin;
     p.BWk = pow2_floor(Wout < BK ? Wout : BK);
@@ -825,23 +618,20 @@ int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, int N, int
     p.kx = b3d::ceil_div(Wout, p.BWk);
     p.ky = b3d::ceil_div(Hout, p.BHk);
     p.kh = kh; p.kw = kw; p.pad_y = pad_y; p.st = stride; p.xoff = x_off; p.tapmajor = tap_major ? 1 : 0;
-    p.fold = fold_kh;
-    B3D_REQUIRE(fold_kh == 0, B3D_EINVAL,
-                "b3d_conv2d_wgrad_tf32: the on-the-fly fold is not available for the weight gradient (TMA pads 32-byte inner boxes "
-                "to 128-byte lines under the 128B swizzles the MN-major tf32 operand needs): pass the materialised fold");
-    if (tap_major) B3D_CHECK_ALIGNED(dw);
-    // a row of kw taps per CTA when the K slice is a 32-pixel row segment (Wout >= 32) of a stride-1 conv
+    const int BN = Cin > 64 ? 128 : 64;
+    // a row of taps per CTA when the K slice is a 32-pixel row segment (Wout >= 32): the three taps of a 3x3 row at 64
+    // input channels, the taps {0,2} / {1,3} of a 4-wide stride-2 row (adjacent pixels of its strided window).  T
+    // accumulators of BN / 2 registers per thread must fit next to the rest (T * BN <= 256).
     int T = 1;
     p.tstep = 1;
-    if (Wout >= BK && !getenv("B3D_WGRAD_T1")) {
-        if (stride == 1 && (kw == 3 || kw == 5)) T = kw;
-        if (stride == 2 && kw == 4) { T = 2; p.tstep = 2; }      // taps {0,2} and {1,3}: rows t of one strided window
+    if (Wout >= BK) {
+        if (stride == 1 && kw == 3 && BN == 64) T = 3;
+        if (stride == 2 && kw == 4) { T = 2; p.tstep = 2; }
     }
-    const int BN = (Cin > 64 && T != 5) ? 128 : 64;          // T * BN <= 512 TMEM columns
     const int base_ctas = b3d::ceil_div(Cout, BM) * b3d::ceil_div(Cin, BN) * kh * (kw / T);
     const long long ktotal = (long long)N * p.kx * p.ky;
-    int splits = ((T == 2 ? 4 : 2) * 148 + base_ctas - 1) / base_ctas;   // ~2 waves of CTAs per resident CTA slot
-    if (splits > ktotal / 8) splits = (int)(ktotal / 8);         // at least 8 K slices per CTA
+    int splits = (2 * tc::num_sms() + base_ctas - 1) / base_ctas;    // ~2 waves of CTAs
+    if (splits > ktotal / 8) splits = (int)(ktotal / 8);           // at least 8 K slices per CTA
     if (splits < 1) splits = 1;
     p.splits = splits;
 
@@ -852,35 +642,22 @@ int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, int N, int
         B3D_REQUIRE(dpitch >= (uint64_t)Wout, B3D_EINVAL, "b3d_conv2d_wgrad_tf32: dy_row_pitch=%d must be >= Wout=%d", dy_row_pitch, Wout);
         const uint64_t strides[4] = {(uint64_t)Cout * 4, dpitch * Cout * 4, (uint64_t)Hout * dpitch * Cout * 4, 128};
         const uint32_t box[5] = {32, (uint32_t)p.BWk, (uint32_t)p.BHk, 1, (uint32_t)(BM / 32)};
-        if (int rc = tc::make_tmap_f32(&mdy, dy, 5, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return rc;
+        if (int rc = tc::make_tmap_f32(&mdy, dy, 5, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_NONE)) return rc;
     }
-    if (fold_kh > 0) {
-        const uint64_t dims[4] = {8, (uint64_t)H, (uint64_t)W, (uint64_t)N};                        // (c, row, x, n)
-        const uint64_t strides[3] = {(uint64_t)W * 32, 32, (uint64_t)H * W * 32};
-        const uint32_t box[4] = {8, 4, (uint32_t)(T == 1 ? p.BWk : 36), 1};
-        if (int rc = tc::make_tmap_f32(&mx, x, 4, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return rc;
-    } else {
+    {
         const uint64_t dims[5] = {32, (uint64_t)W, (uint64_t)H, (uint64_t)N, (uint64_t)Cin / 32};
         const uint64_t strides[4] = {(uint64_t)Cin * 4, (uint64_t)W * Cin * 4, (uint64_t)H * W * Cin * 4, 128};
-        const uint32_t box[5] = {32, (uint32_t)(T == 1 ? stride * (p.BWk - 1) + 1 : stride * 35 + 1), (uint32_t)(stride * (p.BHk - 1) + 1), 1,
-                                 (uint32_t)(BN / 32)};
+        const int wpx = T == 1 ? p.BWk : 36;                       // X pixels per slice: the K slice, or the window of T taps
+        const uint32_t box[5] = {32, (uint32_t)(stride * (wpx - 1) + 1), (uint32_t)(stride * (p.BHk - 1) + 1), 1, (uint32_t)(BN / 32)};
         const uint32_t es[5] = {1, (uint32_t)stride, (uint32_t)stride, 1, 1};
-        if (int rc = tc::make_tmap_f32(&mx, x, 5, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return rc;
+        if (int rc = tc::make_tmap_f32(&mx, x, 5, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_NONE)) return rc;
     }
     cudaStream_t st = (cudaStream_t)stream;
     dim3 grid(b3d::ceil_div(Cout, BM), b3d::ceil_div(Cin, BN), kh * (kw / T) * splits);
-    const bool two = !getenv("B3D_WGRAD_1CTA");           // two CTAs per SM (half-depth ring) where TMEM has room for both
-    if (T == 2 && BN == 128) return two ? launch_wgrad<128, 3, 2>(mdy, mx, p, dw, grid, st) : launch_wgrad<128, 6, 2>(mdy, mx, p, dw, grid, st);
-    if (T == 2) return two ? launch_wgrad<64, 4, 2>(mdy, mx, p, dw, grid, st) : launch_wgrad<64, 8, 2>(mdy, mx, p, dw, grid, st);
-    if (T == 3 && BN == 128) return launch_wgrad<128, 6, 3>(mdy, mx, p, dw, grid, st);
-    // Cout = Cin = 64 rows of three taps: nothing is saturated with one CTA per SM (ncu: tensor pipe 35 %, L2 14 %): two
-    // half-depth CTAs per SM overlap each other's TMA latency and epilogue (B3D_WGRAD_T3=1 restores the deep single ring)
-    static const int t3_one = getenv("B3D_WGRAD_T3") ? atoi(getenv("B3D_WGRAD_T3")) : 0;
-    if (T == 3) return t3_one ? launch_wgrad<64, 8, 3>(mdy, mx, p, dw, grid, st) : launch_wgrad<64, 4, 3>(mdy, mx, p, dw, grid, st);
-    if (T == 5) return launch_wgrad<64, 8, 5>(mdy, mx, p, dw, grid, st);
-    // single taps: the deep single-CTA ring measured faster (profiles/r1_conv_layers.md)
-    if (BN == 128) return launch_wgrad<128, 6, 1>(mdy, mx, p, dw, grid, st);
-    return launch_wgrad<64, 8, 1>(mdy, mx, p, dw, grid, st);
+    if (T == 3) return launch_wgrad<64, 3, 3, 3>(mdy, mx, p, dw, grid, st);
+    if (T == 2) return BN == 128 ? launch_wgrad<128, 2, 3, 2>(mdy, mx, p, dw, grid, st) : launch_wgrad<64, 3, 3, 2>(mdy, mx, p, dw, grid, st);
+    if (BN == 128) return launch_wgrad<128, 3, 3, 1>(mdy, mx, p, dw, grid, st);
+    return launch_wgrad<64, 4, 4, 1>(mdy, mx, p, dw, grid, st);
 }
 
 }  // extern "C"

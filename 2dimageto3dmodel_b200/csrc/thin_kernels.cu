@@ -1,7 +1,6 @@
 // Thin-head convolutions of the GAN: 5x5 layers with 1-4 OUTPUT channels (generator conv_final 64 -> 3, models/gan.py:359;
 // discriminator heads 512 -> 1 / 256 -> 1, models/gan.py:177, :302).  On the tensor-core path such a layer pads its
-// 1-3 output channels to a 64-wide MMA tile and re-fetches the input once per tap: 0.3 % of the network's FLOPs cost
-// 11 % of the step (profiles/r1_conv_layers.md).  They are reductions over (tap, ci) with almost no output, so they run
+// 1-3 output channels to a 64-wide MMA tile and re-fetches the input once per tap, for 0.3 % of the network's FLOPs.  They are reductions over (tap, ci) with almost no output, so they run
 // here on the fp32 CUDA cores with the channel dimension across the lanes of a warp (coalesced NHWC reads, the 25x
 // tap reuse served by L1):
 //   fwd    one warp = 4 adjacent output pixels of one row; per filter row the 4 + kw - 1 input pixels are loaded once
@@ -177,8 +176,7 @@ conv_thin_wgrad_kernel(const float* __restrict__ gy, const float* __restrict__ x
 // Sliding-window variant: along an output row the 5x5 input window moves by one column per pixel, so only its new
 // column (5 loads) is fetched per pixel instead of all 25 taps; the window lives in registers (slots rotate mod 5, the
 // row loop is unrolled by 5 so every slot index is static) and the new column is requested before the 4/5 of the FMAs
-// that do not need it.  ncu on the 25-loads version: 62 % of the samples are FFMAs waiting on the long scoreboard at
-// 12 % occupancy (profiles/r1_c_conv_final_full.md).
+// that do not need it (a 25-loads version leaves the FFMAs waiting on the loads at low occupancy).
 template <int COUT, int VEC>
 __global__ void __launch_bounds__(NT)
 conv_thin_wgrad_win_kernel(const float* __restrict__ gy, const float* __restrict__ x, float* __restrict__ dw, const ThinGeom g) {
@@ -273,7 +271,7 @@ template <int COUT, int VEC>
 int launch_fwd(const float* x, const float* wt, const float* bias, float* out, const ThinGeom& g, cudaStream_t st) {
     const long long items = (long long)g.N * g.Hout * ((g.Wout + OUTS - 1) / OUTS);
     long long blocks = (items + NT / 32 - 1) / (NT / 32);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     conv_thin_fwd_kernel<COUT, VEC><<<(int)blocks, NT, 0, st>>>(x, wt, bias, out, g);
     B3D_LAUNCH_OK();
     b3d::clear_variant();
@@ -284,7 +282,7 @@ int launch_fwd(const float* x, const float* wt, const float* bias, float* out, c
 template <int COUT, int VEC>
 int launch_wgrad(const float* gy, const float* x, float* dw, const ThinGeom& g, cudaStream_t st) {
     const int chunks = g.Cin / (32 * VEC);
-    int bpc = (148 * 2 + chunks - 1) / chunks;
+    int bpc = (132 * 2 + chunks - 1) / chunks;
     const int rows = g.N * g.Hout;
     if (bpc > (rows + NT / 32 - 1) / (NT / 32)) bpc = (rows + NT / 32 - 1) / (NT / 32);
     const size_t smem = (size_t)COUT * KS * KS * 32 * VEC * 4;

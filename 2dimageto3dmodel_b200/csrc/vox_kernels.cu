@@ -1,4 +1,4 @@
-// Dense voxel-grid kernels (sm_100a, HBM-bound, one pass each) for the parts of the point-cloud path that need a
+// Dense voxel-grid kernels (sm_90a, HBM-bound, one pass each) for the parts of the point-cloud path that need a
 // materialised [B,V,V,V] grid: the stand-alone VoxelsSmooth / termination_probs call surface and the paper-intended
 // semantics ("mode P": the Gaussian blur runs along x, y AND z, which couples the columns the fused mode-R kernel
 // keeps in shared memory).
@@ -189,7 +189,7 @@ int fill(Taps& t, const float* h, int n) {
 inline int blocks(long long n) { return (int)((n + NT - 1) / NT); }
 inline int capped(long long n) {
     const long long b = (n + NT - 1) / NT;
-    return (int)(b < 148 * 16 ? (b > 0 ? b : 1) : 148 * 16);
+    return (int)(b < 132 * 16 ? (b > 0 ? b : 1) : 132 * 16);
 }
 }  // namespace
 

@@ -1,5 +1,5 @@
 """Drop-in for /root/reference/code/models/gan.py: the conv-GAN texture/mesh generator and the multi-scale
-discriminators, with every nn.Conv2d running on libb3d's tcgen05 / TMA implicit-GEMM kernels
+discriminators, with every nn.Conv2d running on libb3d's wgmma / TMA implicit-GEMM kernels
 (csrc/tc_conv.cu: fprop, dgrad, wgrad; tf32 inputs, fp32 accumulate).
 
 Module tree, parameter and buffer names equal the reference's, so its checkpoints load with strict=True
@@ -32,7 +32,7 @@ class TCConv2d(nn.Conv2d):
         """`leaky` != 1 fuses LeakyReLU(leaky) into the convolution's epilogue (conv -> bias -> activation in one pass);
         `pad_out` > 0 also applies the next layer's x padding (the epilogue writes into the padded buffer)."""
         if not x.is_cuda:
-            raise B3DError("models.gan convolutions run on CUDA only (libb3d tcgen05 kernels); there is no CPU fallback")
+            raise B3DError("models.gan convolutions run on CUDA only (libb3d wgmma kernels); there is no CPU fallback")
         if self.stride[0] != self.stride[1] or self.dilation != (1, 1) or self.groups != 1 or self.padding_mode != 'zeros':
             raise B3DError("TCConv2d supports zero padding, square strides, no dilation / groups")
         if self.padding[1] != 0:          # the kernels zero-pad along y (TMA fill); zero padding along x is materialised

@@ -4,7 +4,7 @@ run_reconstruction.py trains through the renderer (SURVEY.md §8b, cfg4), and th
 Module tree, parameter and buffer names equal the reference's (`conv1e.weight`, `bn1e.running_mean`, `blk1.conv1.weight`,
 `blk4_mesh.shortcut.weight`, `conv_tex.bias`, `fc1_tex.weight`, ... — its checkpoints load with strict=True) and modules
 are created in the reference's order, so the same seed gives the same initial weights.  Every convolution is a
-models.gan.TCConv2d, i.e. runs on libb3d's tcgen05 / TMA implicit-GEMM kernels (fprop, dgrad and wgrad, tf32 inputs, fp32
+models.gan.TCConv2d, i.e. runs on libb3d's wgmma / TMA implicit-GEMM kernels (fprop, dgrad and wgrad, tf32 inputs, fp32
 accumulate; the 3-channel 5x5 heads on the thin-head kernels).  The encoder's zero padding along x is materialised, along
 y it is the TMA out-of-bounds fill; the decoder's replicate / circular x padding is explicit as in the reference.  Batch
 norms, the three linear layers, nearest upsampling and tanh are stock torch ops on channels-last tensors.  CUDA only:

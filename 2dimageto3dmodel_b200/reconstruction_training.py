@@ -8,7 +8,7 @@ it in a script with argparse, dataset loading and .cuda() at import time): `Reco
     loss = MSE(cat(image, alpha), X_real) + mesh_regularization * flat_warmup * loss_flat(normals(raw_vtx))
     two Adams: network (lr) and DatasetParams (lr_dataset)        :333-357
 
-with the flat-loss warm-up factor 10 -> 1 in steps of 0.1 (:356, :438-439).  CUDA path: tcgen05 convolutions
+with the flat-loss warm-up factor 10 -> 1 in steps of 0.1 (:356, :438-439).  CUDA path: wgmma convolutions
 (models.reconstruction), ONE fused vertex-pipeline launch (b3d.vertex), tiled DIB-R rasteriser + fused shader, fused
 RGBA-MSE / IoU and flat-loss kernels.  One process per GPU; under torch.distributed the batch is sharded per rank, the
 gradients are all-reduced (mean) and the network's BatchNorm layers synchronise their statistics (SyncBN — the

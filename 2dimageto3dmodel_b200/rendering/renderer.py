@@ -1,7 +1,7 @@
 """Drop-in for /root/reference/code/rendering/renderer.py — with the kaolin dependency replaced.
 
 `Renderer.forward` (reference :39-77) = ortho_projection (:9-28) -> kaolin DIB-R `linear_rasterizer`
-(:60-67) -> `fragmentshader` (:72).  Here those three stages are two sm_100a kernels of libb3d
+(:60-67) -> `fragmentshader` (:72).  Here those three stages are two sm_90a kernels of libb3d
 (csrc/mesh_kernels.cu: per-face setup, then a tile-binned rasteriser with the shader fused in).
 `linear_rasterizer` / `datanormalize` below stand in for the two kaolin functions the reference imports.
 """

@@ -1,5 +1,5 @@
 """Drop-in for /root/reference/code/utils/effective_loss_function.py (class EffectiveLossFunction,
-:10-81): points + quaternion (+ scale) -> soft silhouette [B,V,V], computed by the fused sm_100a
+:10-81): points + quaternion (+ scale) -> soft silhouette [B,V,V], computed by the fused sm_90a
 kernels of libb3d (csrc/pc_kernels.cu) instead of ~60 ATen launches and nine dense V^3 temporaries.
 
 `semantics="R"` (default) reproduces the reference as written once its execution defects are patched

@@ -1,7 +1,7 @@
 """Drop-in for /root/reference/code/utils/fid.py (init_inception :9-19, forward_inception_batch :21-25,
 calculate_stats :27-30, calculate_frechet_distance :33-82) — SURVEY §8f rank 4.
 
-* The Inception network is utils/inception.py here: its convolutions run on libb3d's tcgen05 kernels, pools and the
+* The Inception network is utils/inception.py here: its convolutions run on libb3d's wgmma kernels, pools and the
   input transform on csrc/fid_kernels.cu.  CUDA only, like everything behind libb3d.
 * `FIDStatistics` keeps the running sums of the pool features ON THE GPU (b3d_fid_accumulate: sum x and sum x x^T in
   fp64) so an evaluation over thousands of renders never copies activations to the host; `calculate_stats` keeps the

@@ -8,7 +8,7 @@ and `load_torchvision_state_dict` takes torchvision's own `inception_v3_google-*
 `Mixed_5b.branch1x1.bn.weight`, ...; the classifier and the auxiliary head are dropped, as the reference never runs them).
 
 Execution (inference only, like the reference: `requires_grad=False`, `.eval()`):
-* every BasicConv2d (conv, no bias -> BatchNorm eps 1e-3 -> ReLU) is ONE launch of libb3d's tcgen05 implicit-GEMM kernel
+* every BasicConv2d (conv, no bias -> BatchNorm eps 1e-3 -> ReLU) is ONE launch of libb3d's wgmma implicit-GEMM kernel
   (b3d_conv2d_tf32): the batch norm is folded into the weights (rounded to the nearest tf32) and a bias, ReLU is the
   epilogue's leaky slope 0, zero padding is the TMA out-of-bounds fill in both directions, and every branch writes
   straight into its channel slice of the block's concatenated NHWC output (no torch.cat);
@@ -38,7 +38,7 @@ def _pair(v):
 
 def round_tf32(w):
     """Round fp32 values to the nearest tf32 (10 mantissa bits), ties away from zero — cvt.rna.tf32.f32, what the weight
-    bank does for the GAN (tcgen05 kind::tf32 would otherwise truncate)."""
+    bank does for the GAN (the tf32 tensor-core inputs would otherwise be truncated)."""
     bits = w.contiguous().view(torch.int32)
     return ((bits + 0x1000) & ~0x1FFF).view(torch.float32)
 
@@ -125,7 +125,7 @@ class InceptionE(nn.Module):
 class _Folded:
     """One BasicConv2d ready for b3d_conv2d_tf32: tap-major weights [T][Cout'][Cin'] (batch norm folded, tf32-rounded),
     bias [Cout'], tap offsets.  Taps are listed column by column: the per-tap persistent kernel takes every geometry of
-    this network (odd widths, 1x7 / 7x1, stride 2), which the row-window variants are not written for."""
+    this network (odd widths, 1x7 / 7x1, stride 2), which the tap-shifted kernel covers with its generic tiles."""
     __slots__ = ("wt", "bias", "dy", "dx", "ntaps", "stride", "kh", "kw", "ph", "pw", "cin", "cinp", "cout", "coutp")
 
 

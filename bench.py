@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — render+loss(+GAN) images/sec on B200 (BASELINE.json metric), one JSON line on stdout.
+"""bench.py — render+loss(+GAN) images/sec on an H100 (BASELINE.json metric), one JSON line on stdout.
 
 Workloads (SURVEY.md §8d):
   cfg3 (default; BASELINE.json configs[2], the configuration the metric is quoted on): per step THREE training
@@ -32,6 +32,7 @@ for p in (PKG, ROOT):
     if p not in sys.path:
         sys.path.insert(0, p)
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 _T0 = time.time()
@@ -274,7 +275,7 @@ def chamfer_report(dev, B=32, N=8000):
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / reps
     fl = 8.0 * N * N * B * 2                      # both directions: (3 sub, 3 fma-equivalents, compare) ~ 8 flop per pair
-    fp32_peak = 148 * 128 * 2 * 1.965e9 / 1e12     # 148 SMs x 128 FMA lanes x 2 flop x 1.965 GHz
+    fp32_peak = 132 * 128 * 2 * 1.98e9 / 1e12      # H100 SXM data sheet: 132 SMs x 128 FMA lanes x 2 flop x 1.98 GHz
     return {"kernel": "chamfer_nn_kernel (both directions)", "sets": f"{B} x ({N} vs {N})", "ms_per_launch_pair": round(ms, 4),
             "achieved": round(fl / (ms * 1e-3) / 1e12, 2), "peak": round(fp32_peak, 1), "unit": "TFLOP/s (fp32 CUDA cores)",
             "frac": round(fl / (ms * 1e-3) / 1e12 / fp32_peak, 4), "bound": "fp32 issue (8NM flop over 20(N+M) bytes)"}
@@ -289,6 +290,30 @@ def algorithmic_bytes(B, F_=960):
     mesh_bwd = H * H * 32 + 12 * TEX * Tw + 60 * F_
     return {"b3d_pc_silhouette_fwd_hosttaps": B * pc_fwd, "b3d_pc_silhouette_bwd_hosttaps": B * (pc_all - pc_fwd),
             "b3d_mesh_render_fwd": B * mesh_fwd, "b3d_mesh_render_bwd": B * mesh_bwd}
+
+
+DUMP_PARAM_SAMPLE = 4 * 1024 * 1024          # parameter values kept by --dump-outputs (16 MB of float32)
+
+
+def dump_outputs(out_dir, loss, grads, wl):
+    """--dump-outputs: what the last timed step gave its caller, as .npy files in out_dir — the step's loss (float64), the
+    input gradients the render step returns (float32), and the trained networks' parameters after the step (float32, in
+    named_parameters order; a fixed, seeded sample of DUMP_PARAM_SAMPLE values when there are more).  The inputs are
+    seeded, so two builds run with the same arguments can be compared file by file."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().double().reshape(-1).cpu().numpy())
+    for name, g in zip(("points_grad", "quat_grad", "scale_grad", "mesh_map_grad", "tex_grad"), grads or ()):
+        if g is not None:
+            np.save(os.path.join(out_dir, name + ".npy"), g.detach().float().cpu().numpy())
+    trainer = wl.gan or wl.recon
+    if trainer is None:
+        return
+    mods = [(k, m) for k, m in sorted(vars(trainer).items()) if isinstance(m, torch.nn.Module)]
+    flat = torch.cat([p.detach().float().reshape(-1) for _, m in mods for _, p in m.named_parameters()])
+    if flat.numel() > DUMP_PARAM_SAMPLE:
+        idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_PARAM_SAMPLE].sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(out_dir, "params.npy"), flat.cpu().numpy())
 
 
 def run_cuda(args):
@@ -316,7 +341,7 @@ def run_cuda(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    hbm_peak, peak_src = (peaks["hbm_gbs"], "measured") if "hbm_gbs" in peaks else (6650.0, "fallback")
+    hbm_peak, peak_src = (peaks["hbm_gbs"], "measured") if "hbm_gbs" in peaks else (3350.0, "fallback")     # H100 SXM data sheet
 
     stage("process group ready" if world > 1 else "start")
     cfg = WORKLOADS[args.workload]
@@ -339,7 +364,7 @@ def run_cuda(args):
         host.append(hb)
     h2d = sum(t.numel() * t.element_size() for hb in host for t in hb.values())
     resident = [{k: v.to(dev) for k, v in hb.items()} for hb in host]
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)  # > the 50 MB L2
 
     def sync_all():
         if dist is not None:
@@ -371,6 +396,8 @@ def run_cuda(args):
 
     host_loss = torch.empty(1).pin_memory()
     graph = None
+    g_grads = None
+    last_step = {}
     # N > 1: the step contains NCCL collectives (gradient all-reduce, SyncBN statistics); they are captured into the
     # graph too (thread-local capture mode, NCCL async error handling off).  B3D_DDP_EAGER=1 launches eagerly instead.
     has_coll = cfg["gan"] or cfg["kind"] == "recon"
@@ -424,14 +451,15 @@ def run_cuda(args):
             consumed.record(main)
             prefetch()                                       # next step's H2D overlaps this step's kernels
             graph.replay()
-            loss = g_loss
+            loss, grads = g_loss, g_grads
         else:
             batches = [{k: v.clone() for k, v in sb.items()} for sb in staging]
             consumed.record(main)
             prefetch()
-            loss, _ = wl.step(batches)
+            loss, grads = wl.step(batches)
         host_loss.copy_(loss.reshape(1), non_blocking=True)
         main.synchronize()                                   # the user reads the loss every step
+        last_step["out"] = (loss, grads)
         return loss
 
     tf32 = measure_tf32_peak(dev) if (cfg["gan"] or cfg["kind"] == "recon") and rank == 0 else None
@@ -451,6 +479,8 @@ def run_cuda(args):
     stage("timing (end to end)")
     e2e_ms = timed(step_e2e, args.steps, args.warmup)
     clk = clocks.stop(lo, max(hi, lo + 1)) if clocks else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last_step["out"], wl)
 
     # per-entry-point device times (events on the launching stream), separate pass
     stage("per-entry-point profile pass")
@@ -530,13 +560,13 @@ def run_cuda(args):
         # dense-conv FLOPs of one G + two D iterations (SURVEY §8d / App. D at 256^2, nd=2: G 17.09, D 14.76 GF/img fwd),
         # counting only what is executed: G-step = fwd G+D, dgrad+wgrad G, dgrad D (the reference's discarded D wgrad is
         # skipped) = 3G + 2D; D-step = G fwd + D fwd/dgrad/wgrad on 2B images = G + 6D — over the time spent inside the
-        # tcgen05 conv entry points
+        # wgmma conv entry points
         # ... minus the input gradient of the discriminators' first layers in the D-step (their input needs no gradient, so
         # it is not executed): d1.conv1 1.678 + d2.conv1 0.036 GF per image of the 2B batch
         gf_img = (3 * 17.09 + 2 * 14.76) + 2 * (17.09 + 6 * 14.76 - 2 * (1.678 + 0.036))
         conv_ms = sum(v for k, v in prof_tot.items() if k.startswith("b3d_conv2d"))
         tpeak, tpeak_src = tf32["sustained"], tf32["how"]
-        tensor = {"kernel": "all conv entry points: conv_tf32_persistent + wgrad_tf32 (tcgen05 kind::tf32) + thin-head CUDA-core kernels", "bound": "tensor",
+        tensor = {"kernel": "all conv entry points: conv_wgmma + wgrad_wgmma (wgmma tf32) + thin-head CUDA-core kernels", "bound": "tensor",
                   "achieved": round(gf_img * B / (conv_ms * 1e-3) / 1e3, 1), "peak": round(tpeak, 1), "unit": "TFLOP/s",
                   "frac": round(gf_img * B / (conv_ms * 1e-3) / 1e3 / tpeak, 4), "traffic": None,
                   "peak_source": tpeak_src, "peak_burst": tf32["burst"],
@@ -740,10 +770,10 @@ def _run_reference(args):
         B = int(os.environ["B3D_REF_BATCH"])
     wl = OracleWorkload(cfg)
     d = cpu_inputs(cfg, B)
-    warm = 0 if cfg["gan"] else min(args.warmup, 1)
+    warm = args.warmup
     for _ in range(warm):
         wl.step(d)
-    steps = 1 if cfg["gan"] else max(1, min(args.steps, 3))
+    steps = args.steps
     t0 = time.perf_counter()
     for _ in range(steps):
         wl.step(d)
@@ -771,7 +801,12 @@ def main():
     ap.add_argument("--impl", default="b3d", choices=["b3d", "reference"])
     ap.add_argument("--workload", default="cfg3", choices=sorted(WORKLOADS))
     ap.add_argument("--no-graph", action="store_true", help="launch the step eagerly instead of replaying a CUDA graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last one computed to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the CUDA path's outputs; it is not available with --impl reference")
     if args.warmup < 3 and args.impl == "b3d":
         args.warmup = 3
     (run_reference if args.impl == "reference" else run_cuda)(args)

@@ -1,5 +1,5 @@
 /*
- * libb3d — C ABI of the B200-native hot path of NikolaZubic/2dimageto3dmodel.
+ * libb3d — C ABI of the H100-native (sm_90a) hot path of NikolaZubic/2dimageto3dmodel.
  *
  * The reference has no FFI of its own: its boundary is the Python call surface
  * (SURVEY.md §8b).  Every entry point below is what a reference-side binding for
@@ -10,7 +10,8 @@
  *   - plain pointers + sizes, no torch types; every pointer is DEVICE memory,
  *     contiguous, fp32 unless stated, base pointers 16-byte aligned;
  *   - the caller owns every buffer (inputs, outputs, workspaces); the library never
- *     allocates or frees persistent device memory;
+ *     allocates or frees persistent device memory (b3d_conv2d_tf32 with cin-major weights
+ *     takes a stream-ordered temporary for their transpose and frees it on the same stream);
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it, no
  *     internal synchronisation;
  *   - return 0 on success, a negative B3D_E* code otherwise; b3d_last_error()
@@ -45,7 +46,7 @@ extern "C" {
 B3D_API const char* b3d_last_error(void);
 B3D_API int b3d_version(void);
 /* ';'-joined names of the kernel template instances launched by the calling thread's most recent convolution
- * entry point (b3d_conv2d_tf32 / _flat_tf32 / _wgrad_tf32 / _thin_*), e.g. "conv_tf32_persistent<256,4,0,1>":
+ * entry point (b3d_conv2d_tf32 / _flat_tf32 / _wgrad_tf32 / _thin_*), e.g. "conv_wgmma<256,4>":
  * the parity tests assert WHICH variant they exercised, so dispatch drift cannot silently un-test a kernel. */
 B3D_API const char* b3d_last_variant(void);
 /* number of kernels this library has launched in the calling process (bench.py's gpu_launches) */
@@ -224,10 +225,10 @@ B3D_API int b3d_chamfer_bwd(const float* query, const float* cand, const int32_t
 
 /* ------------------------------------------------------------------------------------------
  * Dense 2-D convolution of the conv-GAN (nn.Conv2d call sites models/gan.py:57-65,163-177,294-302,359,364)
- * as a tcgen05 / TMA implicit GEMM (tf32 inputs, fp32 accumulate — cuDNN's default TF32 class, SURVEY §2.2).
+ * as a wgmma / TMA implicit GEMM (tf32 inputs, fp32 accumulate — cuDNN's default TF32 class, SURVEY §2.2).
  *   out[n, osy*y+ooy, osx*x+oox, co] = leaky( bias[co] + sum_t sum_ci x[n, sy*y+dy[t], sx*x+dx[t], ci] * wt[t, co, ci] )
  * x [N,H,W,Cin] NHWC fp32 (Cin % 32 == 0; reads outside [0,H)x[0,W) are zero = the conv's zero padding),
- * wt [ntaps,Cout,Cin] (w_cin_major = 0) or [ntaps,Cin,Cout] (w_cin_major = 1: N-major B operand, Cout % 4 == 0),
+ * wt [ntaps,Cout,Cin] (w_cin_major = 0) or [ntaps,Cin,Cout] (w_cin_major = 1: transposed to the K-major layout once per call, in a stream-ordered temporary),
  * bias [Cout] nullable, out [N,OH,OW,OC]; (y,x) run over [0,Hout)x[0,Wout).
  * fprop: dy = r - pad_y, dx = s.  dgrad: dy = pad_y - r, dx = -s with wt[t] = W[:,:,r,s]^T (strided dgrad = one
  * call per output parity class with osy = osx = 2).  leaky = negative slope of the fused LeakyReLU (1 = none).
@@ -271,18 +272,18 @@ B3D_API int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, 
  * outside the image = the zero padding fold_pad) — Cin is the folded channel count (32 * ceil(8 kh / 32)), the taps are the kw
  * horizontal ones, wt is the folded tap-major layout [kw][Cout][Cin] (b3d/bank.py `fold`).  Needs Wout % 128 == 0.            */
 
-/* Stride-1 variant with a halo-staged input and R stacked accumulators (csrc/tc_conv2.cu): x [N,H,P,Cin] with P the
- * padded width (row pitch), taps (dy, dx >= 0); same weights / bias / LeakyReLU semantics as b3d_conv2d_tf32, output
- * out[n,y,x,co] for y < Hout, x < Wout of a tensor [N,OH,OW,OC].  Returns B3D_EINVAL ("does not fit") when the halo
- * (max tap offset - min tap offset rows of 128 B) exceeds shared memory; callers then use b3d_conv2d_tf32.          */
+/* Stride-1 convolution of an x-padded input x [N,H,P,Cin] (P = padded width = row pitch), taps (dy, dx >= 0); same
+ * weights / bias / LeakyReLU semantics as b3d_conv2d_tf32, output out[n,y,x,co] for y < Hout, x < Wout of a tensor
+ * [N,OH,OW,OC].  Runs b3d_conv2d_tf32 with unit strides (its row-window kernel stages one window of 128 + kw - 1
+ * pixels per filter row and channel slice).                                                                         */
 B3D_API int b3d_conv2d_flat_tf32(const float* x, const float* wt, const float* bias, float* out, int N, int H, int P,
                                  int Cin, int Hout, int Wout, int Cout, int ntaps, const int* dy, const int* dx,
                                  int OH, int OW, int OC, float leaky, void* stream);
 
-/* Weight gradient of the same convolution (split-K tcgen05 GEMM over the output pixels, M/N-major operands
- * straight from the NHWC tensors):
+/* Weight gradient of the same convolution (split-K wgmma GEMM over the output pixels; the M/N-major operands are read
+ * straight from the NHWC tensors and transposed slice by slice in shared memory):
  *   dw[co, ci, r, s] += sum_{n,y,x} dy[n, y, x, co] * x[n, stride*y + r - pad_y, stride*x + s + x_off, ci]
- * dy [N,Hout,Wout,Cout], x [N,H,W,Cin] (x already padded along x; Cin, Cout multiples of 4),
+ * dy [N,Hout,Wout,Cout], x [N,H,W,Cin] (x already padded along x; Cin, Cout multiples of 32),
  * dw [Cout,Cin,kh,kw] is ACCUMULATED into (caller zeroes it).                                          */
 B3D_API int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, int N, int H, int W, int Cin,
                                   int Hout, int Wout, int Cout, int kh, int kw, int pad_y, int stride,

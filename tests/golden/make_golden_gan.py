@@ -59,33 +59,11 @@ def make(fname, res, nd, B, probe):
     print("wrote", path, os.path.getsize(path), "bytes; g_loss", out["g_loss"], "d losses", out["d_loss_fake"], out["d_loss_real"])
 
 
-def checkpoint_kat():
-    """Known-answer test from the SHIPPED checkpoint (SURVEY §8c(1)): the reference Generator, eval mode, running-average
-    weights of gan_weights/pretrained_weights_cub/checkpoint_latest.pth -> probes.  The 52 MB checkpoint is not
-    committed; __graft_entry__.build() stages a copy under tests/golden/_ckpt/ (git-ignored) when /root/reference exists."""
-    ck = "/root/reference/code/gan_weights/pretrained_weights_cub/checkpoint_latest.pth"
-    args = GC.make_args(512, 3)
-    G = ref_gan.Generator(args, 64, symmetric=True, mesh_head=True)
-    G.load_state_dict(torch.load(ck, map_location="cpu")["generator_running_avg"], strict=True)
-    G.eval()
-    torch.manual_seed(1234)
-    z, c = torch.randn(2, 64), torch.tensor([[3], [77]])
-    with torch.no_grad():
-        tex, mesh = G(z, c)
-    out = {"z": z.numpy(), "c": c.numpy(), "tex_probe": tex[:, :, ::16, ::16].numpy(), "tex_px": tex[0, :, 100, 200].numpy(),
-           "mesh": mesh.numpy(), "tex_sum": np.float64(tex.double().sum())}
-    path = os.path.join(HERE, "gan_checkpoint_kat.npz")
-    np.savez_compressed(path, **out)
-    print("wrote", path, os.path.getsize(path), "bytes; tex[0,:,100,200]", out["tex_px"], "sum", out["tex_sum"])
-
-
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["b2", "b32", "r512", "kat"]
+    which = sys.argv[1:] or ["b2", "b32", "r512"]
     if "b2" in which:
         make("gan_reference.npz", 256, 2, 2, 1)            # the small golden (full tensors)
     if "b32" in which:
         make("gan_reference_b32.npz", 256, 2, 32, 4)       # cfg3's batch: reaches the kernels bench.py dispatches
     if "r512" in which:
         make("gan_reference_r512.npz", 512, 3, 2, 1)       # cfg5's architecture (512^2, three discriminators)
-    if "kat" in which:
-        checkpoint_kat()

@@ -61,7 +61,7 @@ def _conv_args(x, wt, out, Hout, Wout, dy, dx, stats, opts):
 
 @pytest.mark.parametrize("N,H,W,Cin,Cout", [(2, 16, 130, 64, 64), (8, 80, 256, 64, 64), (1, 8, 40, 32, 128), (1, 16, 16, 256, 256)])
 def test_conv_epilogue_mask_and_row_pitch(N, H, W, Cin, Cout):
-    """3x3 stride-1 conv through b3d_conv2d_tf32 (row-window or persistent kernel, whichever the shape dispatches) with
+    """3x3 stride-1 conv through b3d_conv2d_tf32 (row-window or per-tap kernel, whichever the shape dispatches) with
     (a) the activation mask + sum statistics and (b) the input read as the interior of a wider buffer."""
     from b3d import check, lib, ptr
     from b3d.conv import _ConvOpts, taps_layout

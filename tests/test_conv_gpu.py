@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM conv (tf32) against torch's fp32 conv2d (TF32 disabled) on the same inputs.
+"""wgmma implicit-GEMM conv (tf32) against torch's fp32 conv2d (TF32 disabled) on the same inputs.
 Tolerance: tf32 keeps 10 mantissa bits (the tensor core truncates fp32 operands), so each product carries
 <= 2^-9 relative error; we require max |err| <= 4e-3 * max|ref| (cuDNN's TF32 path, the reference's default
 on Ampere+, is in the same class)."""

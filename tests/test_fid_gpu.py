@@ -1,5 +1,5 @@
 """FID evaluation path on the GPU (SURVEY §8f rank 4): the kernels of csrc/fid_kernels.cu against torch, the Inception
-convolution geometries on the tcgen05 kernel against an fp64 convolution, the whole CUDA Inception against the oracle's
+convolution geometries on the wgmma kernel against an fp64 convolution, the whole CUDA Inception against the oracle's
 restatement of the network (same state dict), a 299 x 299 render (the evaluation resolution, main.py:156) against the mesh
 oracle, and the evaluation loop end to end.
 

@@ -1,5 +1,5 @@
 """Host-side logic of the GAN drop-ins (CPU): state-dict layout, same-seed initial values and positional
-encoding equal the reference's when /root/reference is present (authoring container); GANLoss vs golden."""
+encoding equal the reference's (tests/golden/reference_pins.npz); GANLoss vs golden."""
 import importlib
 import os
 import sys
@@ -14,7 +14,6 @@ from conftest import GOLDEN, PKG
 sys.path.insert(0, GOLDEN)
 import gan_common as GC          # noqa: E402
 
-REF = "/root/reference/code"
 
 
 def test_ganloss_matches_reference_golden():
@@ -48,33 +47,20 @@ def test_state_dict_layout():
         G(torch.zeros(1, 64), torch.zeros(1, 1, dtype=torch.long))
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present (GPU box)")
 def test_equal_to_reference_modules():
-    # import the reference's models.gan next to ours under a private name
-    saved = {k: sys.modules.pop(k) for k in list(sys.modules) if k.split('.')[0] in ("models", "rendering", "utils", "sync_batchnorm")}
-    sys.path.remove(PKG)
-    sys.path.insert(0, REF)
-    try:
-        ref = importlib.import_module("models.gan")
-    finally:
-        sys.path.remove(REF)
-        for k in [k for k in sys.modules if k.split('.')[0] in ("models", "rendering", "utils", "sync_batchnorm")]:
-            sys.modules.pop(k)
-        sys.path.insert(0, PKG)
-        sys.modules.update(saved)
+    """Same-seed Generator / Discriminator state and positional encodings against the reference's, and the parameter
+    names / shapes a strict load of the shipped generator checkpoint requires (tests/golden/make_golden_reference_pins.py)."""
     from models import gan
-    args = GC.make_args(256, 2)
-    Gr, Dr = GC.build(ref, args)
-    Gm, Dm = GC.build(gan, args)
-    for a, b in ((Gr, Gm), (Dr, Dm)):
-        sa, sb = a.state_dict(), b.state_dict()
-        assert list(sa) == list(sb)
-        assert all(torch.equal(sa[k], sb[k]) for k in sa)
+    from test_recon_hostlogic import check_state_against_pins
+    pins = np.load(os.path.join(GOLDEN, "reference_pins.npz"))
+    Gm, Dm = GC.build(gan, GC.make_args(256, 2))
+    check_state_against_pins(Gm.state_dict(), pins, "gan_G")
+    check_state_against_pins(Dm.state_dict(), pins, "gan_D")
     for ny, nx in ((32, 32), (32, 16), (256, 128)):
-        assert np.abs(ref.positional_encoding(ny, nx) - gan.positional_encoding(ny, nx)).max() < 1e-12
-    ck = os.path.join(REF, "gan_weights/pretrained_weights_cub/checkpoint_latest.pth")
-    G5 = gan.Generator(GC.make_args(512, 3), 64)
-    G5.load_state_dict(torch.load(ck, map_location="cpu")["generator_running_avg"], strict=True)
+        assert np.abs(pins[f"pe_{ny}_{nx}"] - gan.positional_encoding(ny, nx)).max() < 1e-12
+    G5 = gan.Generator(GC.make_args(512, 3), 64).state_dict()
+    assert list(G5) == [str(n) for n in pins["ckpt_names"]]
+    assert [",".join(map(str, v.shape)) for v in G5.values()] == [str(s) for s in pins["ckpt_shapes"]]
 
 
 def test_model_wrapper_and_running_average_match_the_reference_step_logic():

@@ -1,4 +1,4 @@
-"""models.reconstruction.ReconstructionNetwork on the tcgen05 conv kernels against golden vectors produced by the
+"""models.reconstruction.ReconstructionNetwork on the wgmma conv kernels against golden vectors produced by the
 reference's own module on the CPU (tests/golden/make_golden_recon.py): same seed -> same weights, same inputs, one
 training-mode forward + backward (batch statistics, stride-2 3x3 / 5x5 encoder convs, ResBlocks, thin 3-channel heads).
 

@@ -1,5 +1,5 @@
 """Host-side logic of the models.reconstruction drop-in (CPU): state-dict layout and same-seed initial values equal the
-reference's when /root/reference is present (authoring container); DatasetParams against the reference golden."""
+reference's (tests/golden/reference_pins.npz); DatasetParams against the reference golden."""
 import os
 import sys
 
@@ -12,7 +12,6 @@ from conftest import GOLDEN
 sys.path.insert(0, GOLDEN)
 import recon_common as RC          # noqa: E402
 
-REF = "/root/reference/code"
 
 
 def test_dataset_params_match_reference_golden():
@@ -50,28 +49,20 @@ def test_state_dict_layout():
         ReconstructionNetwork(texture_res=100)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present (GPU box)")
+def check_state_against_pins(sd, pins, tag):
+    """A same-seed state dict against the reference's (make_golden_reference_pins.py): names in order, shapes, fp64 sums
+    and the first 16 values of every tensor."""
+    assert list(sd.keys()) == [str(n) for n in pins[tag + "_names"]]
+    for (k, v), shape, total, head in zip(sd.items(), pins[tag + "_shapes"], pins[tag + "_sums"], pins[tag + "_heads"]):
+        assert ",".join(map(str, v.shape)) == str(shape), k
+        h = v.detach().double().flatten()[:16].numpy()
+        assert np.array_equal(h, head[:h.size]), k
+        assert abs(float(v.double().sum()) - total) <= 1e-9 * max(1.0, abs(total)) + 1e-9 * v.numel(), k
+
+
 def test_same_seed_state_equals_reference():
-    import importlib
-    from conftest import PKG
     from models import reconstruction as mine
-    saved = {k: sys.modules.pop(k) for k in list(sys.modules) if k.split('.')[0] in ("models", "rendering", "utils")}
-    sys.path.remove(PKG)
-    sys.path.insert(0, REF)
-    try:
-        ref = importlib.import_module("models.reconstruction")
-        assert ref.__file__.startswith(REF)
-        r = RC.build(ref).state_dict()
-    finally:
-        sys.path.remove(REF)
-        for k in [k for k in sys.modules if k.split('.')[0] in ("models", "rendering", "utils")]:
-            sys.modules.pop(k)
-        sys.path.insert(0, PKG)
-        sys.modules.update(saved)
-    m = RC.build(mine).state_dict()
-    assert list(m.keys()) == list(r.keys())
-    for k in m:
-        assert m[k].shape == r[k].shape and torch.equal(m[k], r[k]), k
+    check_state_against_pins(RC.build(mine).state_dict(), np.load(os.path.join(GOLDEN, "reference_pins.npz")), "recon")
 
 
 def test_forward_wiring_matches_reference_golden_on_cpu(monkeypatch):

@@ -1,5 +1,5 @@
 """MeshTemplate (SURVEY §8 row a10) against the REFERENCE's own class: tests/golden/template_reference.npz was produced by
-running /root/reference/code/rendering/mesh_template.py:MeshTemplate unmodified on the CPU (make_golden_template.py: a
+running the reference's rendering/mesh_template.py:MeshTemplate unmodified on the CPU (make_golden_template.py: a
 stand-in supplies the one kaolin call, OBJ loading, and `.cuda()`).  Checked here, on the procedural UV spheres that travel
 with the repo (16 and 31 rings, symmetric and not): the oracle's restatement (oracle/mesh.py TemplateData, get_vertex_positions,
 adjust_uv_and_texture, compute_normals) — which thereby becomes PINNED — and the drop-in rendering/mesh_template.py on its
@@ -74,10 +74,12 @@ def test_drop_in_template_equals_the_reference_class(rings, sym):
 
 
 @pytest.mark.parametrize("rings", [16, 31])
-def test_shipped_templates_through_probes(rings):
-    path = f"/root/reference/code/mesh_templates/uvsphere_{rings}rings.obj"
-    if not os.path.exists(path):
-        pytest.skip("the reference tree (shipped OBJ templates) is only present in the authoring container")
+def test_shipped_templates_through_probes(rings, tmp_path):
+    import gzip
+    import shutil
+    path = str(tmp_path / f"uvsphere_{rings}rings.obj")             # the reference's shipped templates, stored gzip-compressed
+    with gzip.open(os.path.join(GOLDEN, f"uvsphere_{rings}rings.obj.gz"), "rb") as src, open(path, "wb") as dst:
+        shutil.copyfileobj(src, dst)
     from rendering.mesh_template import MeshTemplate
     tag = f"ship{rings}_sym"
     g = torch.Generator().manual_seed(int(G[tag + "_dmap_seed"][0]))

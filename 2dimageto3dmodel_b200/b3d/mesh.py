@@ -171,21 +171,26 @@ def flat_loss(norms, ff):
     return _FlatLoss.apply(norms, ff)
 
 
-class _RgbaMse(torch.autograd.Function):
+# criterion -> (forward + IoU counts, backward) entry points of csrc/loss_kernels.cu
+_RGBA_LOSS = {"mse": ("b3d_rgba_mse_iou_fwd", "b3d_rgba_mse_bwd"), "l1": ("b3d_rgba_l1_iou_fwd", "b3d_rgba_l1_bwd")}
+
+
+class _RgbaLoss(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, image, alpha, target):
+    def forward(ctx, image, alpha, target, criterion):
+        fwd, bwd = _RGBA_LOSS[criterion]
         im = dev(image.detach(), "image_pred")
         al = dev(alpha.detach(), "alpha_pred")
         tg = dev(target.detach(), "X_real")
         B, H, W, _ = im.shape
         if tg.shape != (B, 4, H, W) or al.numel() != B * H * W:
-            raise B3DError(f"rgba_mse_iou: shapes image {tuple(im.shape)} alpha {tuple(al.shape)} "
+            raise B3DError(f"rgba_{criterion}_iou: shapes image {tuple(im.shape)} alpha {tuple(al.shape)} "
                            f"target {tuple(tg.shape)}")
         loss = torch.empty(1, device=im.device, dtype=torch.float32)
         counts = torch.empty(B, 2, device=im.device, dtype=torch.int32)
-        check(lib.b3d_rgba_mse_iou_fwd(ptr(im), ptr(al), ptr(tg), B, H, W, ptr(loss), ptr(counts), stream_ptr(im)))
+        check(getattr(lib, fwd)(ptr(im), ptr(al), ptr(tg), B, H, W, ptr(loss), ptr(counts), stream_ptr(im)))
         ctx.save_for_backward(im, al, tg)
-        ctx.ashape = alpha.shape
+        ctx.ashape, ctx.bwd = alpha.shape, bwd
         ctx.mark_non_differentiable(counts)
         return loss.view(()), counts
 
@@ -195,14 +200,24 @@ class _RgbaMse(torch.autograd.Function):
         B, H, W, _ = im.shape
         g = dev(g.reshape(1), "grad")
         di, da = torch.empty_like(im), torch.empty_like(al)
-        check(lib.b3d_rgba_mse_bwd(ptr(im), ptr(al), ptr(tg), B, H, W, ptr(g), ptr(di), ptr(da), stream_ptr(im)))
-        return di, da.view(ctx.ashape), None
+        check(getattr(lib, ctx.bwd)(ptr(im), ptr(al), ptr(tg), B, H, W, ptr(g), ptr(di), ptr(da), stream_ptr(im)))
+        return di, da.view(ctx.ashape), None, None
+
+
+def _rgba_loss_iou(image_pred, alpha_pred, X_real, criterion):
+    loss, counts = _RgbaLoss.apply(image_pred, alpha_pred, X_real, criterion)
+    c = counts.to(torch.float32)
+    return loss, (c[:, 0] / c[:, 1]).mean()
 
 
 def rgba_mse_iou(image_pred, alpha_pred, X_real):
     """Fused form of run_reconstruction.py:429-436:
         X_fake = cat(image_pred, alpha_pred, 3).permute(0,3,1,2); nn.MSELoss()(X_fake, X_real); mean_iou(...)
     -> (recon_loss, miou); miou carries no gradient, like the reference's torch.no_grad() block."""
-    loss, counts = _RgbaMse.apply(image_pred, alpha_pred, X_real)
-    c = counts.to(torch.float32)
-    return loss, (c[:, 0] / c[:, 1]).mean()
+    return _rgba_loss_iou(image_pred, alpha_pred, X_real, "mse")
+
+
+def rgba_l1_iou(image_pred, alpha_pred, X_real):
+    """rgba_mse_iou with the reference's --loss l1 criterion nn.L1Loss() (run_reconstruction.py:347-352): the mean of
+    |X_fake - X_real|; its gradient is torch's sign(d) / n, 0 where prediction and target are equal."""
+    return _rgba_loss_iou(image_pred, alpha_pred, X_real, "l1")

@@ -1,8 +1,8 @@
 // Loss kernels of the mesh path (SURVEY.md §8 row a12) for sm_90a.
 //   flat_loss_*      loss_flat (utils/losses.py:5-17): neighbour-face normal cosine regulariser
-//   rgba_mse_iou_*   nn.MSELoss on cat(image, alpha) vs the RGBA target (run_reconstruction.py:429-431)
-//                    fused with mean_iou's counts (run_reconstruction.py:225-231): one pass over the
-//                    rendered image instead of cat + permute + sub + square + mean + 4 threshold passes.
+//   rgba_loss_iou_*  nn.MSELoss / nn.L1Loss on cat(image, alpha) vs the RGBA target (run_reconstruction.py:347-352,
+//                    429-431) fused with mean_iou's counts (run_reconstruction.py:225-231): one pass over the
+//                    rendered image instead of cat + permute + sub + square|abs + mean + 4 threshold passes.
 #include "b3d_common.cuh"
 
 namespace {
@@ -109,11 +109,27 @@ face_normals_bwd_kernel(const float* __restrict__ verts, const int32_t* __restri
     atomicAdd(db + 3 * ia, -(dux + dvx)); atomicAdd(db + 3 * ia + 1, -(duy + dvy)); atomicAdd(db + 3 * ia + 2, -(duz + dvz));
 }
 
-// image [B,H,W,3], alpha [B,H,W], target [B,4,H,W]; sse += sum of squared error; counts[b] = {inter, union}
+// The criterion of --loss (mse|l1): per-element term of the sum, and its derivative with respect to the prediction.
+enum class Crit { MSE, L1 };
+
+template <Crit C>
+__device__ __forceinline__ float loss_term(float d, float acc) {
+    return C == Crit::MSE ? fmaf(d, d, acc) : acc + fabsf(d);
+}
+
+// k = d loss / d (sum term) scale; L1 uses torch's sign (0 for a tie and for NaN, so background pixels where prediction
+// and target are both exactly 0 get no gradient)
+template <Crit C>
+__device__ __forceinline__ float loss_grad(float k, float d) {
+    return C == Crit::MSE ? k * d : k * (float)((d > 0.f) - (d < 0.f));
+}
+
+// image [B,H,W,3], alpha [B,H,W], target [B,4,H,W]; loss += inv_n * sum of per-element terms; counts[b] = {inter, union}
+template <Crit C>
 __global__ void __launch_bounds__(NT)
-rgba_mse_iou_fwd_kernel(const float* __restrict__ image, const float* __restrict__ alpha,
-                        const float* __restrict__ target, int HW, float inv_n, float* __restrict__ loss,
-                        int32_t* __restrict__ counts) {
+rgba_loss_iou_fwd_kernel(const float* __restrict__ image, const float* __restrict__ alpha,
+                         const float* __restrict__ target, int HW, float inv_n, float* __restrict__ loss,
+                         int32_t* __restrict__ counts) {
     __shared__ float red[32];
     const int b = blockIdx.y;
     const float* tb = target + (size_t)b * 4 * HW;
@@ -123,11 +139,11 @@ rgba_mse_iou_fwd_kernel(const float* __restrict__ image, const float* __restrict
         const size_t pix = (size_t)b * HW + p;
         const float a = alpha[pix], ta = tb[3 * (size_t)HW + p];
         float d = a - ta;
-        acc = fmaf(d, d, acc);
+        acc = loss_term<C>(d, acc);
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
             d = image[3 * pix + c] - tb[(size_t)c * HW + p];
-            acc = fmaf(d, d, acc);
+            acc = loss_term<C>(d, acc);
         }
         const bool pa = a > 0.5f, pt = ta > 0.5f;
         inter += (pa && pt) ? 1 : 0;
@@ -145,19 +161,45 @@ rgba_mse_iou_fwd_kernel(const float* __restrict__ image, const float* __restrict
     }
 }
 
+template <Crit C>
 __global__ void __launch_bounds__(NT)
-rgba_mse_bwd_kernel(const float* __restrict__ image, const float* __restrict__ alpha, const float* __restrict__ target,
-                    int HW, float inv_n, const float* __restrict__ gloss, float* __restrict__ d_image,
-                    float* __restrict__ d_alpha) {
+rgba_loss_bwd_kernel(const float* __restrict__ image, const float* __restrict__ alpha, const float* __restrict__ target,
+                     int HW, float inv_n, const float* __restrict__ gloss, float* __restrict__ d_image,
+                     float* __restrict__ d_alpha) {
     const int b = blockIdx.y;
-    const float k = 2.f * inv_n * gloss[0];
+    const float k = (C == Crit::MSE ? 2.f * inv_n : inv_n) * gloss[0];
     const float* tb = target + (size_t)b * 4 * HW;
     for (int p = blockIdx.x * NT + threadIdx.x; p < HW; p += gridDim.x * NT) {
         const size_t pix = (size_t)b * HW + p;
-        d_alpha[pix] = k * (alpha[pix] - tb[3 * (size_t)HW + p]);
+        d_alpha[pix] = loss_grad<C>(k, alpha[pix] - tb[3 * (size_t)HW + p]);
 #pragma unroll
-        for (int c = 0; c < 3; ++c) d_image[3 * pix + c] = k * (image[3 * pix + c] - tb[(size_t)c * HW + p]);
+        for (int c = 0; c < 3; ++c) d_image[3 * pix + c] = loss_grad<C>(k, image[3 * pix + c] - tb[(size_t)c * HW + p]);
     }
+}
+
+// launchers shared by the per-criterion exports, which check their arguments first
+template <Crit C>
+int rgba_loss_iou_fwd(const float* image, const float* alpha, const float* target, int B, int H, int W, float* loss,
+                      int32_t* counts, cudaStream_t st) {
+    B3D_CUDA_OK(cudaMemsetAsync(loss, 0, sizeof(float), st));
+    if (counts) B3D_CUDA_OK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * 2 * B, st));
+    const int HW = H * W;
+    const int gx = min(b3d::ceil_div(HW, NT), 132 * 4);
+    rgba_loss_iou_fwd_kernel<C><<<dim3(gx, B), NT, 0, st>>>(image, alpha, target, HW,
+                                                            1.f / (4.f * (float)B * (float)HW), loss, counts);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+template <Crit C>
+int rgba_loss_bwd(const float* image, const float* alpha, const float* target, int B, int H, int W, const float* gloss,
+                  float* d_image, float* d_alpha, cudaStream_t st) {
+    const int HW = H * W;
+    const int gx = min(b3d::ceil_div(HW, NT), 132 * 4);
+    rgba_loss_bwd_kernel<C><<<dim3(gx, B), NT, 0, st>>>(image, alpha, target, HW, 1.f / (4.f * (float)B * (float)HW),
+                                                        gloss, d_image, d_alpha);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
 }
 }  // namespace
 
@@ -203,27 +245,27 @@ int b3d_rgba_mse_iou_fwd(const float* image, const float* alpha, const float* ta
                          int32_t* counts, void* stream) {
     B3D_REQUIRE(B > 0 && H > 0 && W > 0 && image && alpha && target && loss, B3D_EINVAL,
                 "b3d_rgba_mse_iou_fwd: bad arguments");
-    cudaStream_t st = (cudaStream_t)stream;
-    B3D_CUDA_OK(cudaMemsetAsync(loss, 0, sizeof(float), st));
-    if (counts) B3D_CUDA_OK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * 2 * B, st));
-    const int HW = H * W;
-    const int gx = min(b3d::ceil_div(HW, NT), 132 * 4);
-    rgba_mse_iou_fwd_kernel<<<dim3(gx, B), NT, 0, st>>>(image, alpha, target, HW, 1.f / (4.f * (float)B * (float)HW),
-                                                       loss, counts);
-    B3D_LAUNCH_OK();
-    return B3D_OK;
+    return rgba_loss_iou_fwd<Crit::MSE>(image, alpha, target, B, H, W, loss, counts, (cudaStream_t)stream);
 }
 
 int b3d_rgba_mse_bwd(const float* image, const float* alpha, const float* target, int B, int H, int W,
                      const float* gloss, float* d_image, float* d_alpha, void* stream) {
     B3D_REQUIRE(B > 0 && H > 0 && W > 0 && image && alpha && target && gloss && d_image && d_alpha, B3D_EINVAL,
                 "b3d_rgba_mse_bwd: bad arguments");
-    const int HW = H * W;
-    const int gx = min(b3d::ceil_div(HW, NT), 132 * 4);
-    rgba_mse_bwd_kernel<<<dim3(gx, B), NT, 0, (cudaStream_t)stream>>>(image, alpha, target, HW,
-                                                                     1.f / (4.f * (float)B * (float)HW), gloss,
-                                                                     d_image, d_alpha);
-    B3D_LAUNCH_OK();
-    return B3D_OK;
+    return rgba_loss_bwd<Crit::MSE>(image, alpha, target, B, H, W, gloss, d_image, d_alpha, (cudaStream_t)stream);
+}
+
+int b3d_rgba_l1_iou_fwd(const float* image, const float* alpha, const float* target, int B, int H, int W, float* loss,
+                        int32_t* counts, void* stream) {
+    B3D_REQUIRE(B > 0 && H > 0 && W > 0 && image && alpha && target && loss, B3D_EINVAL,
+                "b3d_rgba_l1_iou_fwd: bad arguments");
+    return rgba_loss_iou_fwd<Crit::L1>(image, alpha, target, B, H, W, loss, counts, (cudaStream_t)stream);
+}
+
+int b3d_rgba_l1_bwd(const float* image, const float* alpha, const float* target, int B, int H, int W,
+                    const float* gloss, float* d_image, float* d_alpha, void* stream) {
+    B3D_REQUIRE(B > 0 && H > 0 && W > 0 && image && alpha && target && gloss && d_image && d_alpha, B3D_EINVAL,
+                "b3d_rgba_l1_bwd: bad arguments");
+    return rgba_loss_bwd<Crit::L1>(image, alpha, target, B, H, W, gloss, d_image, d_alpha, (cudaStream_t)stream);
 }
 }  // extern "C"

@@ -8,20 +8,23 @@ it in a script with argparse, dataset loading and .cuda() at import time): `Reco
     loss = MSE(cat(image, alpha), X_real) + mesh_regularization * flat_warmup * loss_flat(normals(raw_vtx))
     two Adams: network (lr) and DatasetParams (lr_dataset)        :333-357
 
-with the flat-loss warm-up factor 10 -> 1 in steps of 0.1 (:356, :438-439).  CUDA path: wgmma convolutions
-(models.reconstruction), ONE fused vertex-pipeline launch (b3d.vertex), tiled DIB-R rasteriser + fused shader, fused
-RGBA-MSE / IoU and flat-loss kernels.  One process per GPU; under torch.distributed the batch is sharded per rank, the
-gradients are all-reduced (mean) and the network's BatchNorm layers synchronise their statistics (SyncBN — the
+with the flat-loss warm-up factor 10 -> 1 in steps of 0.1 (:356, :438-439) and the criterion of --loss (mse|l1)
+(:347-352).  `ReconTrainer.evaluate` is the validation pass evaluate_all (:255-319) and `ReconTrainer.render_multiview`
+its turntable render (:188-221).  CUDA path: wgmma convolutions (models.reconstruction), ONE fused vertex-pipeline launch
+(b3d.vertex), tiled DIB-R rasteriser + fused shader, fused RGBA-MSE|L1 / IoU and flat-loss kernels.  One process per
+GPU; under torch.distributed the batch is sharded per rank, the gradients are all-reduced (mean) and the network's BatchNorm layers synchronise their statistics (SyncBN — the
 reference never ran this script multi-GPU; SURVEY §8e states the deviation that keeps N-GPU == 1-GPU on the same
 global batch)."""
 import types
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
-from b3d.mesh import rgba_mse_iou
+from b3d.mesh import rgba_l1_iou, rgba_mse_iou
 from models.reconstruction import DatasetParams, ReconstructionNetwork
 from rendering.renderer import Renderer
+from rendering.utils import qmul, qrot
 from utils.losses import loss_flat
 
 
@@ -35,6 +38,8 @@ def default_args(**kw):
 
 class ReconTrainer:
     def __init__(self, args, mesh_template, dataset_size, device='cuda', capturable=False):
+        if args.loss not in ('mse', 'l1'):
+            raise ValueError(f"ReconTrainer: loss={args.loss!r}; the reference's criteria are 'mse' and 'l1'")
         self.args, self.tpl = args, mesh_template
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         net = ReconstructionNetwork(symmetric=args.symmetric, texture_res=args.texture_resolution,
@@ -51,10 +56,13 @@ class ReconTrainer:
             self.dataset_params = DatasetParams(args, dataset_size).to(device)
             self.optimizer_dataset = torch.optim.Adam(self.dataset_params.parameters(), lr=args.lr_dataset,
                                                       capturable=capturable, fused=fused)
-        if args.loss != 'mse':
-            raise ValueError("ReconTrainer: only the reference's default criterion (mse) is built on the fused loss kernel")
         # flat-loss warm-up (:356, :438-439) as a device scalar so that a captured step keeps counting
         self.flat_warmup = torch.full((), 10.0, device=device)
+
+    def criterion(self, image_pred, alpha_pred, X_real):
+        """criterion(X_fake, X_real) over [B,4,H,W] + mean IoU on alpha, in one fused kernel (:347-352, :429-436)."""
+        fn = rgba_l1_iou if self.args.loss == 'l1' else rgba_mse_iou
+        return fn(image_pred, alpha_pred, X_real)
 
     def forward_loss(self, X_real, gt_scale, gt_translation, gt_rot, gt_idx=None):
         """-> (loss, recon_loss, flat_loss, miou); differentiable."""
@@ -68,7 +76,7 @@ class ReconTrainer:
             z0 = dp(gt_idx, 'z0')
         raw_vtx, vtx = self.tpl.vertices_and_pose(mesh_map, scale, trans, gt_rot, z0)
         image_pred, alpha_pred = self.tpl.forward_renderer(self.renderer, vtx, pred_tex)
-        recon_loss, miou = rgba_mse_iou(image_pred, alpha_pred, X_real)       # MSE over [B,4,H,W] + mean IoU on alpha
+        recon_loss, miou = self.criterion(image_pred, alpha_pred, X_real)
         flat_loss = loss_flat(self.tpl.mesh, self.tpl.compute_normals(raw_vtx))
         loss = recon_loss + (a.mesh_regularization * self.flat_warmup) * flat_loss
         return loss, recon_loss, flat_loss, miou
@@ -91,3 +99,59 @@ class ReconTrainer:
         if self.optimizer_dataset is not None:
             self.optimizer_dataset.step()
         return loss.detach(), recon_loss.detach(), flat_loss.detach(), miou
+
+    @torch.no_grad()
+    def evaluate(self, batches, distributed=False):
+        """The validation pass evaluate_all (:255-319) without its TensorBoard images: every batch (X_real, gt_scale,
+        gt_translation, gt_rot[, idx]) is posed with the DATASET-MEAN DatasetParams (transform_vertices(..., None), :274)
+        and scored with the configured criterion, loss_flat and mean IoU.  -> dict(recon_loss, flat_loss, miou, N): the
+        per-sample means over the N images, which the reference logs as
+        '[TEST] recon_loss {:.5f}, flat_loss {:.5f}, mIoU {:.5f}, N {}'.  A batch whose predicted and target alpha are
+        both empty has a NaN IoU, as in the reference.  The sums stay on the device in fp64 (one host sync at the end).
+        distributed: every rank passes its shard; the sums are all-reduced before the division, so every rank returns the
+        values of the whole set (eval-mode batch norm couples no samples)."""
+        a, dp = self.args, self.dataset_params
+        self.generator.eval()
+        sums = torch.zeros(4, dtype=torch.float64, device=next(self.generator.parameters()).device)
+        for X_real, gt_scale, gt_translation, gt_rot, *_ in batches:
+            B = X_real.shape[0]
+            pred_tex, mesh_map = self.generator(X_real)
+            scale, trans, z0 = gt_scale, gt_translation, None
+            if a.optimize_deltas:                   # means [1,3] / [1,1] broadcast over the batch
+                translation_delta, scale_delta = dp(None, 'deltas')
+                scale, trans = gt_scale + scale_delta, gt_translation + translation_delta
+            if a.optimize_z0:
+                z0 = dp(None, 'z0').expand(B, 1)
+            raw_vtx, vtx = self.tpl.vertices_and_pose(mesh_map, scale, trans, gt_rot, z0)
+            image_pred, alpha_pred = self.tpl.forward_renderer(self.renderer, vtx, pred_tex)
+            recon_loss, miou = self.criterion(image_pred, alpha_pred, X_real)
+            flat_loss = loss_flat(self.tpl.mesh, self.tpl.compute_normals(raw_vtx))
+            sums += torch.stack((recon_loss.double(), flat_loss.double(), miou.double(), sums.new_ones(()))) * B
+        if distributed:
+            dist.all_reduce(sums, op=dist.ReduceOp.SUM)
+        recon, flat, miou, n = sums.tolist()
+        return dict(recon_loss=recon / n, flat_loss=flat / n, miou=miou / n, N=int(n))
+
+    @torch.no_grad()
+    def render_multiview(self, raw_vtx, pred_tex, idx=0):
+        """Sample `idx` (object-space vertices raw_vtx [B,V,3], texture pred_tex [B,3,T,T]) rendered from the reference's
+        eight turntable views (:188-221) in one batch-8 render -> numpy [2R, 4R, 3] tile (rows of four views) in [0, 1]."""
+        d = raw_vtx.device
+        rad = -90 / 180 * np.pi
+        q0 = torch.tensor([np.cos(-rad / 2), 0, 0, np.sin(-rad / 2)], dtype=torch.float32, device=d)
+        rad = 110 / 180 * np.pi
+        q1 = torch.tensor([np.cos(-rad / 2), 0, np.sin(-rad / 2), 0], dtype=torch.float32, device=d)
+        q0 = qmul(q0, q1)
+        rot = []
+        for angle in (0, 45, 90, 135, 180, 225, 270, 315):
+            rad = angle / 180 * np.pi * 0.8
+            rot.append(qmul(q0, torch.tensor([np.cos(-rad / 2), 0, 0, np.sin(-rad / 2)], dtype=torch.float32, device=d)))
+        rot = torch.stack(rot, dim=0)
+        raw = raw_vtx[idx:idx + 1].expand(len(rot), -1, -1).contiguous()
+        tex = pred_tex[idx:idx + 1].expand(len(rot), -1, -1, -1).contiguous()
+        vtx = qrot(rot, raw) * 0.9
+        vtx[:, :, 1:] *= -1
+        view, _ = self.tpl.forward_renderer(self.renderer, vtx, tex)
+        R = view.shape[1]
+        tile = view.view(2, 4, R, view.shape[2], 3).permute(0, 2, 1, 3, 4).reshape(2 * R, 4 * view.shape[2], 3)
+        return (tile.cpu().numpy() + 1) / 2

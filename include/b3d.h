@@ -212,6 +212,15 @@ B3D_API int b3d_rgba_mse_iou_fwd(const float* image, const float* alpha, const f
 B3D_API int b3d_rgba_mse_bwd(const float* image, const float* alpha, const float* target, int B, int H,
                              int W, const float* gloss, float* d_image, float* d_alpha, void* stream);
 
+/* nn.L1Loss()(cat(image, alpha).permute(0,3,1,2), X_real) + the same counts (--loss l1)
+ *                                               run_reconstruction.py:225-231,347-352,429-431
+ * Arguments as b3d_rgba_mse_iou_fwd / b3d_rgba_mse_bwd.  bwd writes d_image, d_alpha
+ * (= sign(x - t) gloss / n, torch's sign: 0 where x == t or x - t is NaN).                          */
+B3D_API int b3d_rgba_l1_iou_fwd(const float* image, const float* alpha, const float* target, int B, int H,
+                                int W, float* loss, int32_t* counts, void* stream);
+B3D_API int b3d_rgba_l1_bwd(const float* image, const float* alpha, const float* target, int B, int H,
+                            int W, const float* gloss, float* d_image, float* d_alpha, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Chamfer / pairwise nearest neighbour (north-star kernel; no reference implementation exists —
  * the reference's only pairwise-NN site is rendering/mesh_template.py:33-39).

@@ -79,14 +79,39 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ uint32_t lds_u32(uint32_t smem_addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(smem_addr) : "memory");
+    return v;
+}
+// per-thread register budget of the executing warpgroup (warp-specialized kernels move registers from producer to consumers)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // D[64 x N] (+)= A[64 x 8] * B[8 x N], tf32 operands (fp32 words in shared memory, K-major), fp32 accumulators in the
 // registers of the issuing warpgroup.  Fragment: thread t (warp w = t / 32, lane l) holds d[4j + e] = D[16w + l/4 + 8(e/2),
 // 8j + 2(l%4) + e%2].
+// mma_rs takes A from registers instead (B stays in shared memory, K-major).  A fragment: thread t holds
+// a[e] = A[16w + l/4 + 8(e%2), l%4 + 4(e/2)], the raw fp32 words: the tensor core drops the low mantissa bits as it does
+// for operands read from shared memory, so both forms compute the same products.
 template <int N>
 struct Wgmma;
 template <>
 struct Wgmma<64> {
+    __device__ __forceinline__ static void mma_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "setp.ne.b32 p, %37, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+            "{%32, %33, %34, %35}, %36, p, 1, 1;\n"
+            "}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+    }
     __device__ __forceinline__ static void mma(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
         asm volatile(
             "{\n"
@@ -102,6 +127,18 @@ struct Wgmma<64> {
 };
 template <>
 struct Wgmma<128> {
+    __device__ __forceinline__ static void mma_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "setp.ne.b32 p, %69, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+            "{%64, %65, %66, %67}, %68, p, 1, 1;\n"
+            "}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+    }
     __device__ __forceinline__ static void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
         asm volatile(
             "{\n"
@@ -151,7 +188,7 @@ __device__ __forceinline__ uint64_t desc_k32(uint32_t smem_addr) {
     return d;
 }
 
-// One 32-wide K slice of an operand that TMA delivered M/N-major (NHWC pixels along K: the weight gradient's dY and X)
+// One 32-wide K slice of an operand that TMA delivered M/N-major (NHWC pixels along K: the weight gradient's X)
 // as `rows` / 32 boxes [k][32 mn] (no swizzle; boxes blk_stride floats apart), K rows k0 .. k0 + 31 rewritten K-major
 // into `dst` in the 128-byte-swizzled layout that desc_k128 reads: row mn, 16-byte chunk c at byte
 // mn * 128 + ((c ^ (mn % 8)) << 4).  Executed by the 128 threads of the producer warpgroup; consecutive threads take

@@ -233,14 +233,16 @@ __global__ void transpose_taps_kernel(const float* __restrict__ in, float* __res
 // ----------------------------------------------------------------------------------------------
 // wgrad:  dW[co, ci, r, s] += sum_{n,y,x} dY[n, y, x, co] * X[n, st*y + r - pad_y, st*x + s, ci]      (NHWC operands)
 // GEMM with M = Cout (128), N = Cin (BN), K = output pixels.  In NHWC the reduction index (pixel) is the SLOW index
-// of both operands, i.e. they are M/N-major, and wgmma reads tf32 operands K-major only: a K slice is a BWk x BHk box of
-// 32 output pixels, loaded by TMA as [32 pixels][32 channels] boxes (four for dY, BN/32 for X, the X boxes shifted by the
-// tap on the OUTER dims: zero fill = padding, element strides for stride 2) into an NRAW-deep staging ring, and the
-// producer warpgroup rewrites each slice K-major into the swizzled stage the consumers read (tc::transpose_slice_k128).
-// No NCHW copy is ever made.  T > 1 (row of taps): a K slice is a 32-pixel row segment, the X box is a window of
-// 32 + T - 1 (rounded to 36) pixels, and the producer writes T K-major B tiles from it — tap t is the window shifted by t
-// pixels — which share the staged dY tile: T accumulators per consumer warpgroup, T taps per byte of dY.  One CTA per
-// (co tile, ci tile, tap group, K split); partial sums are reduced into dW with global atomics.
+// of both operands, i.e. they are M/N-major: a K slice is a BWk x BHk box of 32 output pixels, loaded by TMA as
+// [32 pixels][32 channels] boxes (four for dY, BN/32 for X, the X boxes shifted by the tap on the OUTER dims: zero fill =
+// padding, element strides for stride 2) into an NRAW-deep staging ring.  wgmma reads tf32 operands from shared memory
+// K-major only, so the producer warpgroup rewrites each X slice K-major into the swizzled stage the consumers read
+// (tc::transpose_slice_k128).  dY is the A operand, which wgmma also takes from registers: the consumers load their
+// fragments straight from the staged dY tile (128-byte swizzled by TMA, conflict-free: dy_tile_offset) and hand the raw
+// slot back as soon as the loads are done.  No NCHW copy is ever made.  T > 1 (row of taps): a K slice is a 32-pixel row
+// segment, the X box is a window of 32 + T - 1 (rounded to 36) pixels, and the producer writes T K-major B tiles from it
+// — tap t is the window shifted by t pixels — which share the dY fragments: T accumulators per consumer warpgroup, T taps
+// per byte of dY.  One CTA per (co tile, ci tile, tap group, K split); partial sums are reduced into dW with global atomics.
 // ----------------------------------------------------------------------------------------------
 struct WgradParams {
     int N, Hout, Wout, Cout, Cin;
@@ -254,15 +256,31 @@ struct WgradParams {
                                    // 2: taps of equal parity of a stride-2 conv = adjacent pixels of the strided window)
 };
 
+// Stage: the T K-major X tiles.  Raw slot: the dY tile (offset 0, 1024-byte aligned: its 128-byte swizzle is the one
+// dy_tile_offset describes) and the X boxes behind it.
 template <int BN, int STAGES, int NRAW, int T>
 struct WSmem {
-    static constexpr int A_BYTES = BM * BK * 4;
-    static constexpr int STAGE_BYTES = A_BYTES + T * BN * BK * 4;
+    static constexpr int DY_BYTES = BM * BK * 4;
+    static constexpr int STAGE_BYTES = T * BN * BK * 4;
     static constexpr int WROWS = T == 1 ? 32 : 36;                      // X pixels per 32-channel block of a raw slice
     static constexpr int RAW_X = (BN / 32) * WROWS * 128;
-    static constexpr int RAW_BYTES = (A_BYTES + RAW_X + 1023) / 1024 * 1024;
+    static constexpr int RAW_BYTES = (DY_BYTES + RAW_X + 1023) / 1024 * 1024;
     static constexpr int TOTAL = STAGES * STAGE_BYTES + NRAW * RAW_BYTES + 1024 + 256;
 };
+
+// Row m (0..63) of a consumer warpgroup's m64 tile is output channel wgrad_row_co(m) of the warpgroup's 64: bits 2, 3, 4
+// of m rotated to 3, 4, 2.  Within a warp's fragment load the eight lanes that share l % 4 then see channels c, c + 1,
+// c + 2, c + 3, c + 16 ... c + 19, i.e. two 16-byte chunks of a 128-byte row that differ in chunk bit 2, while the four
+// values of l % 4 (consecutive pixels) XOR the chunk index with four different values in bits 0-1.
+__host__ __device__ constexpr int wgrad_row_co(int m) { return (m & 35) | ((m & 8) >> 1) | ((m & 16) >> 1) | ((m & 4) << 2); }
+
+// Byte offset of dY[co][px] (co < 128 of the CTA's tile, px < 32 of the K slice) in the staged dY tile: TMA lands four
+// [32 px][32 ch] boxes of 4 KB with the 128-byte swizzle (16-byte chunk index XOR row % 8).  With the rows of
+// wgrad_row_co, each of a thread's fragment loads (A[m][k] of the layout in tc_common.cuh, k = px % 8 of K step px / 8)
+// touches 32 different banks across the warp; K step k is 1024 bytes further.
+__host__ __device__ constexpr int dy_tile_offset(int co, int px) {
+    return (co >> 5) * 4096 + px * 128 + ((((co >> 2) & 7) ^ (px & 7)) << 4) + (co & 3) * 4;
+}
 
 template <int BN, int STAGES, int NRAW, int T>
 __global__ void __launch_bounds__(NTHREADS, 1)
@@ -275,6 +293,7 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_con
     uint64_t* full = reinterpret_cast<uint64_t*>(raw + NRAW * S::RAW_BYTES);
     uint64_t* empty = full + STAGES;
     uint64_t* rawfull = empty + STAGES;
+    uint64_t* rawempty = rawfull + NRAW;                  // dY fragments loaded: one arrival per consumer warp
 
     const int co0 = blockIdx.x * BM, ci0 = blockIdx.y * BN;
     const int gpr = p.kw / T;                             // tap groups per filter row
@@ -293,13 +312,19 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_con
             tc::mbar_init(full + i, 128);
             tc::mbar_init(empty + i, 2);
         }
-        for (int i = 0; i < NRAW; ++i) tc::mbar_init(rawfull + i, 1);
+        for (int i = 0; i < NRAW; ++i) {
+            tc::mbar_init(rawfull + i, 1);
+            tc::mbar_init(rawempty + i, 8);
+        }
         tc::fence_barrier_init();
     }
     __syncthreads();
     const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
 
+    // registers move from the producer (transpose loops) to the consumers (T accumulators and the dY fragments);
+    // 128 * (168 - 56) == 256 * (224 - 168)
     if (wg == 0) {
+        tc::setmaxnreg_dec<56>();
         auto issue = [&](int j) {
             if (tid != 0) return;
             const long long k = k_lo + j;
@@ -307,10 +332,11 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_con
             const int x0 = (rem % p.kx) * p.BWk, y0 = (rem / p.kx) * p.BHk;
             const int rb = j % NRAW;
             unsigned char* dst = raw + rb * S::RAW_BYTES;
+            tc::mbar_wait(rawempty + rb, ((j / NRAW) & 1) ^ 1);   // the consumers have loaded the dY fragments of slice j - NRAW
             // channels are split as (32, C/32) in the tensor maps: ONE 5-D box lands all 32-channel blocks back to back
-            tc::mbar_arrive_expect_tx(rawfull + rb, S::A_BYTES + S::RAW_X);
+            tc::mbar_arrive_expect_tx(rawfull + rb, S::DY_BYTES + S::RAW_X);
             tc::tma_load_5d(dst, &tmap_dy, rawfull + rb, 0, x0, y0, n, co0 / 32);
-            tc::tma_load_5d(dst + S::A_BYTES, &tmap_x, rawfull + rb, 0, p.st * x0 + s + p.xoff, p.st * y0 + r - p.pad_y, n, ci0 / 32);
+            tc::tma_load_5d(dst + S::DY_BYTES, &tmap_x, rawfull + rb, 0, p.st * x0 + s + p.xoff, p.st * y0 + r - p.pad_y, n, ci0 / 32);
         };
         for (int j = 0; j < NRAW - 1 && j < KI; ++j) issue(j);
         for (int it = 0; it < KI; ++it) {
@@ -318,51 +344,66 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_con
             const int rb = it % NRAW, st = it % STAGES;
             tc::mbar_wait(rawfull + rb, (it / NRAW) & 1);
             tc::mbar_wait(empty + st, ((it / STAGES) & 1) ^ 1);
-            const float* src = reinterpret_cast<const float*>(raw + rb * S::RAW_BYTES);
+            const float* src = reinterpret_cast<const float*>(raw + rb * S::RAW_BYTES + S::DY_BYTES);
             unsigned char* dst = base + st * S::STAGE_BYTES;
-            tc::transpose_slice_k128(src, dst, BM, tid);
 #pragma unroll
             for (int t = 0; t < T; ++t)
-                tc::transpose_slice_k128(src + S::A_BYTES / 4, dst + S::A_BYTES + t * (BN * 128), BN, tid, S::WROWS * 32, t);
+                tc::transpose_slice_k128(src, dst + t * (BN * 128), BN, tid, S::WROWS * 32, t);
             tc::fence_proxy_async();
             tc::mbar_arrive(full + st);
-            tc::named_sync(2, 128);                               // the raw slice is consumed before it is loaded again
+            tc::named_sync(2, 128);                               // the raw X boxes are consumed before they are loaded again
         }
         return;
     }
+    tc::setmaxnreg_inc<224>();
 
     const int h = wg - 1, lane = tid & 31;
+    // this thread's fragment registers a[0..3] of K step 0 in the staged dY tile (K step k: + 1024 k)
+    int aoff[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+        aoff[e] = dy_tile_offset(h * 64 + wgrad_row_co((tid >> 5) * 16 + (lane >> 2) + 8 * (e & 1)), (lane & 3) + 4 * (e >> 1));
     float acc[T][BN / 2];
 #pragma unroll
     for (int t = 0; t < T; ++t)
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[t][i] = 0.f;
+    // A wgmma reads its register operands after it issues, and register allocation does not see that: fragments
+    // double-buffered across slices may be given the same registers, and the compiler then waits for every wgmma before
+    // the next one issues.  So one set of fragments, reloaded once the slice's wgmma group has retired; the other consumer
+    // warpgroup's group keeps the tensor cores busy meanwhile.
+    const uint32_t raw_s = tc::smem_u32(raw);
     for (int it = 0; it < KI; ++it) {
-        const int st = it % STAGES;
+        const int st = it % STAGES, rb = it % NRAW;
+        tc::mbar_wait(rawfull + rb, (it / NRAW) & 1);
+        uint32_t frag[BK / MMA_K][4];
+#pragma unroll
+        for (int k = 0; k < BK / MMA_K; ++k)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) frag[k][e] = tc::lds_u32(raw_s + rb * S::RAW_BYTES + aoff[e] + k * 1024);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(rawempty + rb);      // the loads are complete: TMA may refill the slot
         tc::mbar_wait(full + st, (it / STAGES) & 1);
-        const uint32_t a = tc::smem_u32(base + st * S::STAGE_BYTES), b = a + S::A_BYTES;
+        const uint32_t b = tc::smem_u32(base + st * S::STAGE_BYTES);
         tc::wgmma_fence();
 #pragma unroll
         for (int t = 0; t < T; ++t)
 #pragma unroll
             for (int k = 0; k < BK / MMA_K; ++k)
-                tc::Wgmma<BN>::mma(acc[t], tc::desc_k128(a + h * (64 * 128) + k * MMA_K * 4),
-                                   tc::desc_k128(b + t * (BN * 128) + k * MMA_K * 4), (it | k) ? 1u : 0u);
+                tc::Wgmma<BN>::mma_rs(acc[t], frag[k], tc::desc_k128(b + t * (BN * 128) + k * MMA_K * 4), (it | k) ? 1u : 0u);
         tc::wgmma_commit();
-        tc::wgmma_wait<1>();
-        if (it > 0 && tid == 0) tc::mbar_arrive(empty + (it - 1) % STAGES);
+        tc::wgmma_wait<0>();
+        if (tid == 0) tc::mbar_arrive(empty + st);
     }
-    tc::wgmma_wait<0>();
     if (KI == 0) return;
-    if (tid == 0) tc::mbar_arrive(empty + (KI - 1) % STAGES);
-    const int co_a = co0 + h * 64 + (tid >> 5) * 16 + (lane >> 2);
+    const int m_a = (tid >> 5) * 16 + (lane >> 2);                // this thread's accumulator rows m_a, m_a + 8
     const int cq = ci0 + 2 * (lane & 3);
 #pragma unroll
     for (int t = 0; t < T; ++t) {
         const int sc = s + t * p.tstep;                       // filter column of accumulator t
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-            const int co = co_a + 8 * e;
+            const int co = co0 + h * 64 + wgrad_row_co(m_a + 8 * e);
             if (co >= p.Cout) continue;
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
@@ -642,7 +683,7 @@ int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, int N, int
         B3D_REQUIRE(dpitch >= (uint64_t)Wout, B3D_EINVAL, "b3d_conv2d_wgrad_tf32: dy_row_pitch=%d must be >= Wout=%d", dy_row_pitch, Wout);
         const uint64_t strides[4] = {(uint64_t)Cout * 4, dpitch * Cout * 4, (uint64_t)Hout * dpitch * Cout * 4, 128};
         const uint32_t box[5] = {32, (uint32_t)p.BWk, (uint32_t)p.BHk, 1, (uint32_t)(BM / 32)};
-        if (int rc = tc::make_tmap_f32(&mdy, dy, 5, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_NONE)) return rc;
+        if (int rc = tc::make_tmap_f32(&mdy, dy, 5, dims, strides, box)) return rc;    // 128-byte swizzle: dy_tile_offset
     }
     {
         const uint64_t dims[5] = {32, (uint64_t)W, (uint64_t)H, (uint64_t)N, (uint64_t)Cin / 32};

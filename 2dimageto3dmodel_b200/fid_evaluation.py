@@ -11,7 +11,13 @@ What runs where: generator, vertex pipeline (ONE fused launch for get_vertex_pos
 `MeshTemplate.vertices_and_pose`), rasteriser + shader, Inception and the feature statistics are libb3d kernels; the
 activations stay on the GPU (`utils.fid.FIDStatistics`) — the reference copies every batch's features to the host and
 concatenates them.  Only the D x D eigen-decompositions of the final distance are host numpy, as in the reference.
+
+`select_best_checkpoint` is main.py's `--evaluate --which_epoch best` search (:787-834).
 """
+import glob
+import os
+import re
+
 import numpy as np
 import torch
 
@@ -147,3 +153,33 @@ class FIDEvaluator:
             out["features"] = {k: torch.cat(v, dim=0) for k, v in feats.items() if v}
         out["num_generated"] = st["combined"].n
         return out
+
+
+def select_best_checkpoint(trainer, evaluator, checkpoint_dir, eval_batches, seed=None, distributed=False):
+    """main.py:787-834: every checkpoint_<epoch>.pth in checkpoint_dir (a name that matches the glob
+    checkpoint_[0-9]*.pth but not checkpoint_([0-9]+).pth raises ValueError) is loaded in 'evaluate' mode into trainer
+    (a GANTrainer) and scored by evaluator.evaluate(fast=True), newest epoch first; a later-visited checkpoint replaces
+    the best one only on a strictly smaller FID.  The best checkpoint is then loaded and evaluated in full.  evaluator
+    must score trainer's running-average generator (FIDEvaluator(trainer.trainer.generator_running_avg, ...)): the
+    loads copy into it in place.  seed and distributed are passed to every evaluate call (the reference seeds every
+    evaluation with 1234 in this mode).  -> dict(fast_fid={epoch: fid} in visit order, best_path, scores)."""
+    checkpoints = {}
+    for path in sorted(glob.glob(os.path.join(checkpoint_dir, 'checkpoint_[0-9]*.pth'))):
+        m = re.search('checkpoint_([0-9]+).pth', path)
+        if not m:
+            raise ValueError(f'Invalid path detected: {path}')
+        checkpoints[int(m.group(1))] = path
+    if not checkpoints:
+        raise ValueError(f'no checkpoint_<epoch>.pth in {checkpoint_dir}')
+    fast_fid, best_fid, best_path = {}, float('inf'), None
+    for epoch, path in sorted(checkpoints.items())[::-1]:
+        trainer.load_checkpoint(path, 'evaluate')
+        fid = evaluator.evaluate(eval_batches, fast=True, seed=seed, distributed=distributed)['fid']
+        fast_fid[epoch] = fid
+        if fid < best_fid:
+            best_fid, best_path = fid, path
+    if best_path is None:
+        raise ValueError(f'no finite fast FID among {sorted(checkpoints)}')
+    trainer.load_checkpoint(best_path, 'evaluate')
+    scores = evaluator.evaluate(eval_batches, seed=seed, distributed=distributed)
+    return dict(fast_fid=fast_fid, best_path=best_path, scores=scores)

@@ -1,7 +1,8 @@
 """The GAN step logic of /root/reference/code/main.py as an importable module (the reference keeps it in a
 script with argparse at import time): `ModelWrapper` (main.py:449-526: 'g' / 'd' / 'inference' modes, fake‖real
 batching, per-discriminator weights) and `GANTrainer` (main.py:588-589 optimisers, :691-723 G/D alternation with
-d_steps_per_g, mesh smoothness term, :431-447 running-average generator).  One process per GPU; under
+d_steps_per_g, mesh smoothness term, :431-447 running-average generator), its epoch loop (`train_epoch`: :738-747 linear
+learning-rate decay) and checkpoints (:599-633 loading, :749-770 save_checkpoint).  One process per GPU; under
 torch.distributed the gradients are all-reduced (mean) in flat buckets after backward and the generator's
 batch-norm statistics synchronise inside sync_batchnorm."""
 import math
@@ -10,6 +11,8 @@ import torch
 import torch.distributed as dist
 import torch.nn as nn
 
+import checkpoint_io
+from checkpoint_io import load_optimizer_state_dict, optimizer_state_dict
 from models.gan import Generator, MultiScaleDiscriminator
 from utils.losses import GANLoss, loss_flat
 
@@ -123,6 +126,9 @@ class GANTrainer:
         self.optimizer_d = torch.optim.Adam(d.parameters(), lr=args.lr_d, betas=(0.0, 0.9), capturable=capturable, fused=fused)
         self.total_it = 0
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+        self.epoch = 0
+        # main.py:591-594: the loss curves start with [0]; train_epoch appends one value per G / D iteration
+        self.g_curve, self.d_fake_curve, self.d_real_curve, self.flat_curve = [0], [0], [0], [0]
 
     def update_generator_running_avg(self, epoch=1000):
         a = self.args.g_running_average_alpha
@@ -154,11 +160,13 @@ class GANTrainer:
         finally:
             self._freeze_discriminator(False)
         loss_gan = loss.mean()
-        total = loss_gan
+        total, flat = loss_gan, None
         if pred_mesh is not None and self.mesh_template is not None:
             vtx = self.mesh_template.get_vertex_positions(pred_mesh)
-            total = total + self.args.mesh_regularization * loss_flat(self.mesh_template.mesh,
-                                                                       self.mesh_template.compute_normals(vtx))
+            flat = loss_flat(self.mesh_template.mesh, self.mesh_template.compute_normals(vtx))
+            total = total + self.args.mesh_regularization * flat
+        # the step's loss terms, still on the device, for the curves train_epoch keeps (read once per epoch)
+        self.last_terms = (loss_gan.detach(), flat.detach() if flat is not None else None)
         total.backward()
         if self.world > 1:
             allreduce_network_grads(self.trainer.generator, self.world)
@@ -169,7 +177,9 @@ class GANTrainer:
     def d_step(self, X_tex, X_alpha, X_mesh, C, noise=None):
         self.optimizer_d.zero_grad(set_to_none=True)
         loss_fake, loss_real, _, _ = self.trainer('d', X_tex, X_alpha, X_mesh, C, None, noise)
-        loss = loss_fake.mean() + loss_real.mean()
+        loss_fake, loss_real = loss_fake.mean(), loss_real.mean()
+        loss = loss_fake + loss_real
+        self.last_terms = (loss_fake.detach(), loss_real.detach())
         loss.backward()
         if self.world > 1:
             allreduce_network_grads(self.trainer.discriminator, self.world)
@@ -183,3 +193,82 @@ class GANTrainer:
         out = self.g_step(X_alpha, C, noise, epoch) if is_g else self.d_step(X_tex, X_alpha, X_mesh, C, noise)
         self.total_it += 1
         return out
+
+    # ------------------------------------------------------------------------------------------------ the epoch layer
+    def train_epoch(self, batches):
+        """One epoch of main.py's training loop (:672-747): `step` on every batch (a dict of step's arguments X_tex,
+        X_alpha, X_mesh, C and optionally noise) at this trainer's `epoch`, then epoch += 1 and the linear learning-rate
+        decay of both optimisers once epoch >= args.lr_decay_after (default 1000) while epoch < args.epochs (default 600).
+        The loss curves get this epoch's values with one host synchronisation.  -> the per-iteration step outputs.
+        A CUDA graph captured from `step` keeps the learning rate it was captured with: capture it again after this
+        changes the rate, and after load_checkpoint."""
+        outs, g, flat, d_fake, d_real = [], [], [], [], []
+        for b in batches:
+            is_g = self.total_it % (1 + self.args.d_steps_per_g) == 0
+            outs.append(self.step(**b, epoch=self.epoch))
+            if is_g:
+                g.append(self.last_terms[0])
+                if self.last_terms[1] is not None:
+                    flat.append(self.last_terms[1])
+            else:
+                d_fake.append(self.last_terms[0])
+                d_real.append(self.last_terms[1])
+        vals = torch.stack(g + flat + d_fake + d_real).tolist() if outs else []
+        for curve, n in ((self.g_curve, len(g)), (self.flat_curve, len(flat)), (self.d_fake_curve, len(d_fake)),
+                         (self.d_real_curve, len(d_real))):
+            curve.extend(vals[:n])
+            vals = vals[n:]
+        self.epoch += 1
+        a = self.args
+        after, epochs = getattr(a, 'lr_decay_after', 1000), getattr(a, 'epochs', 600)
+        if after <= self.epoch < epochs:
+            factor = 1 - min(max((self.epoch - after) / (epochs - after), 0), 1)
+            for group in self.optimizer_g.param_groups:
+                group['lr'] = a.lr_g * factor
+            for group in self.optimizer_d.param_groups:
+                group['lr'] = a.lr_d * factor
+        return outs
+
+    def checkpoint(self):
+        """The dict main.py's save_checkpoint writes (:749-770): same keys, nesting and value types."""
+        t = self.trainer
+        return {
+            'optimizer_g': optimizer_state_dict(self.optimizer_g),
+            'optimizer_d': optimizer_state_dict(self.optimizer_d),
+            'generator': t.generator.state_dict(),
+            'generator_running_avg': t.generator_running_avg.state_dict(),
+            'discriminator': t.discriminator.state_dict(),
+            'epoch': self.epoch,
+            'iteration': self.total_it,
+            'g_curve': list(self.g_curve),
+            'd_fake_curve': list(self.d_fake_curve),
+            'd_real_curve': list(self.d_real_curve),
+            'flat_curve': list(self.flat_curve),
+            'args': dict(vars(self.args)),
+        }
+
+    def save_checkpoint(self, path):
+        """Write checkpoint() to path (rank 0 under torch.distributed, then a barrier)."""
+        checkpoint_io.save(self.checkpoint(), path)
+
+    def load_checkpoint(self, path, mode='resume'):
+        """main.py:599-633, loaded onto this trainer's device.  mode 'resume' (--continue_train): the networks, the
+        running average, both optimisers, epoch, iteration (so the G / D alternation continues in phase) and the curves.
+        mode 'evaluate' (--evaluate): generator_running_avg, plus generator / epoch / iteration / curves when the file
+        has an 'epoch' (the shipped checkpoints hold generator_running_avg only).  Parameters and buffers are copied in
+        place, so the weight banks keep their packed pointers and an FIDEvaluator built on generator_running_avg
+        evaluates the loaded weights."""
+        if mode not in ('resume', 'evaluate'):
+            raise ValueError(f"load_checkpoint: mode={mode!r}; expected 'resume' or 'evaluate'")
+        t = self.trainer
+        chk = checkpoint_io.load(path, next(t.generator_running_avg.parameters()).device)
+        if 'epoch' in chk:
+            self.epoch, self.total_it = chk['epoch'], chk['iteration']
+            self.g_curve, self.d_fake_curve = list(chk['g_curve']), list(chk['d_fake_curve'])
+            self.d_real_curve, self.flat_curve = list(chk['d_real_curve']), list(chk['flat_curve'])
+            t.generator.load_state_dict(chk['generator'])
+        t.generator_running_avg.load_state_dict(chk['generator_running_avg'])
+        if mode == 'resume':
+            load_optimizer_state_dict(self.optimizer_g, chk['optimizer_g'])
+            t.discriminator.load_state_dict(chk['discriminator'])
+            load_optimizer_state_dict(self.optimizer_d, chk['optimizer_d'])

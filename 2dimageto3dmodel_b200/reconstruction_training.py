@@ -10,7 +10,8 @@ it in a script with argparse, dataset loading and .cuda() at import time): `Reco
 
 with the flat-loss warm-up factor 10 -> 1 in steps of 0.1 (:356, :438-439) and the criterion of --loss (mse|l1)
 (:347-352).  `ReconTrainer.evaluate` is the validation pass evaluate_all (:255-319) and `ReconTrainer.render_multiview`
-its turntable render (:188-221).  CUDA path: wgmma convolutions (models.reconstruction), ONE fused vertex-pipeline launch
+its turntable render (:188-221); `train_epoch` the epoch loop with its learning-rate halving (:466-470) and
+`save_checkpoint` / `load_checkpoint` the checkpoints (:359-382, :472-481).  CUDA path: wgmma convolutions (models.reconstruction), ONE fused vertex-pipeline launch
 (b3d.vertex), tiled DIB-R rasteriser + fused shader, fused RGBA-MSE|L1 / IoU and flat-loss kernels.  One process per
 GPU; under torch.distributed the batch is sharded per rank, the gradients are all-reduced (mean) and the network's BatchNorm layers synchronise their statistics (SyncBN — the
 reference never ran this script multi-GPU; SURVEY §8e states the deviation that keeps N-GPU == 1-GPU on the same
@@ -21,6 +22,8 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+import checkpoint_io
+from checkpoint_io import load_optimizer_state_dict, optimizer_state_dict
 from b3d.mesh import rgba_l1_iou, rgba_mse_iou
 from models.reconstruction import DatasetParams, ReconstructionNetwork
 from rendering.renderer import Renderer
@@ -29,9 +32,10 @@ from utils.losses import loss_flat
 
 
 def default_args(**kw):
-    """run_reconstruction.py's argparse defaults (:37-65) for the fields the step reads."""
+    """run_reconstruction.py's argparse defaults (:37-65) for the fields the step and the epoch loop read."""
     a = dict(symmetric=True, texture_resolution=128, mesh_resolution=32, image_resolution=256, loss='mse',
-             optimize_deltas=True, optimize_z0=False, mesh_regularization=0.00005, lr=0.0001, lr_dataset=0.0001)
+             optimize_deltas=True, optimize_z0=False, mesh_regularization=0.00005, lr=0.0001, lr_dataset=0.0001,
+             epochs=1000, lr_decay_every=250)
     a.update(kw)
     return types.SimpleNamespace(**a)
 
@@ -58,6 +62,7 @@ class ReconTrainer:
                                                       capturable=capturable, fused=fused)
         # flat-loss warm-up (:356, :438-439) as a device scalar so that a captured step keeps counting
         self.flat_warmup = torch.full((), 10.0, device=device)
+        self.epoch = self.total_it = 0
 
     def criterion(self, image_pred, alpha_pred, X_real):
         """criterion(X_fake, X_real) over [B,4,H,W] + mean IoU on alpha, in one fused kernel (:347-352, :429-436)."""
@@ -99,6 +104,64 @@ class ReconTrainer:
         if self.optimizer_dataset is not None:
             self.optimizer_dataset.step()
         return loss.detach(), recon_loss.detach(), flat_loss.detach(), miou
+
+    # ------------------------------------------------------------------------------------------------ the epoch layer
+    def train_epoch(self, batches):
+        """One epoch of run_reconstruction.py's training loop (:407-470): `step` on every batch (X_real, gt_scale,
+        gt_translation, gt_rot, gt_idx [B]), then epoch += 1 and, every args.lr_decay_every (default 250) epochs, the
+        network optimiser's learning rate is halved (the DatasetParams optimiser keeps its rate).  -> the per-iteration
+        step outputs.  A CUDA graph captured from `step` keeps the learning rate it was captured with: capture it again
+        after this changes the rate, and after load_checkpoint."""
+        outs = []
+        for b in batches:
+            outs.append(self.step(*b))
+            self.total_it += 1
+        self.epoch += 1
+        if self.epoch % getattr(self.args, 'lr_decay_every', 250) == 0:
+            for group in self.optimizer.param_groups:
+                group['lr'] *= 0.5
+        return outs
+
+    def checkpoint(self):
+        """The dict run_reconstruction.py's save_checkpoint writes (:472-481), plus 'flat_warmup': the flat-loss warm-up
+        factor (the reference does not store it, and ignores the extra key)."""
+        dp, od = self.dataset_params, self.optimizer_dataset
+        return {
+            'optimizer': optimizer_state_dict(self.optimizer),
+            'generator': self.generator.state_dict(),
+            'optimizer_dataset_params': optimizer_state_dict(od) if od is not None else None,
+            'dataset_params': dp.state_dict() if dp is not None else None,
+            'epoch': self.epoch,
+            'iteration': self.total_it,
+            'args': dict(vars(self.args)),
+            'flat_warmup': float(self.flat_warmup),
+        }
+
+    def save_checkpoint(self, path):
+        """Write checkpoint() to path (rank 0 under torch.distributed, then a barrier)."""
+        checkpoint_io.save(self.checkpoint(), path)
+
+    def load_checkpoint(self, path, mode='resume'):
+        """run_reconstruction.py:359-377, loaded onto this trainer's device.  Both modes load the network and the
+        DatasetParams (a trainer without DatasetParams accepts only a file without them), and epoch / iteration when
+        present.  mode 'resume' (--continue_train) also loads both optimisers and the flat-loss warm-up factor; a file
+        without 'flat_warmup' (one the reference wrote) restarts it at 10, as the reference does.  mode 'evaluate'
+        (--evaluate, --generate_pseudogt) loads nothing more.  Parameters and buffers are copied in place."""
+        if mode not in ('resume', 'evaluate'):
+            raise ValueError(f"load_checkpoint: mode={mode!r}; expected 'resume' or 'evaluate'")
+        chk = checkpoint_io.load(path, self.flat_warmup.device)
+        if 'epoch' in chk:
+            self.epoch, self.total_it = chk['epoch'], chk['iteration']
+        self.generator.load_state_dict(chk['generator'])
+        if self.dataset_params is not None:
+            self.dataset_params.load_state_dict(chk['dataset_params'])
+        elif chk.get('dataset_params') is not None:
+            raise AssertionError("the checkpoint has DatasetParams but this trainer optimises neither deltas nor z0")
+        if mode == 'resume':
+            load_optimizer_state_dict(self.optimizer, chk['optimizer'])
+            if self.optimizer_dataset is not None:
+                load_optimizer_state_dict(self.optimizer_dataset, chk['optimizer_dataset_params'])
+            self.flat_warmup.fill_(chk.get('flat_warmup', 10.0))
 
     @torch.no_grad()
     def evaluate(self, batches, distributed=False):

@@ -1,6 +1,8 @@
 """One-pass NHWC helper ops between the convolutions (libb3d csrc/ew_kernels.cu), with autograd."""
 import ctypes
+import math
 import os
+import struct
 
 import torch
 
@@ -98,6 +100,11 @@ def pad_x(x_nchw, amount, mode):
 # ------------------------------------------------------------------------------------------------------------------
 # fused conditional-batch-norm -> LeakyReLU -> (+ residual) -> (LeakyReLU) -> x2 nearest upsample -> replicate pad
 # ------------------------------------------------------------------------------------------------------------------
+def _f32(v):
+    """v rounded to the nearest fp32 value, as a Python float."""
+    return struct.unpack("f", struct.pack("f", float(v)))[0]
+
+
 def _dist_world():
     import torch.distributed as dist
     return dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
@@ -158,7 +165,9 @@ class BNAffine(CBNBatch):
 class _CBNActPad(torch.autograd.Function):
     """y [N,H,W,C] (conv output, NHWC) -> out [N, up*H, up*W + 2*pad, C]; gb = CBNBatch.gb (gamma / beta of this layer at
     column offsets goff / boff).  `skip` (optional) [N,H,Ws,C] read at pixel offset skip_off.  Statistics, running buffers
-    and the per-sample affine come from one b3d_cbn_prepare launch (modes: 0 eval, 1 batch statistics, 2 SyncBN)."""
+    and the per-sample affine come from one b3d_cbn_prepare launch (modes: 0 eval, 1 batch statistics, 2 SyncBN).
+    As in F.batch_norm, a norm without running buffers (track_running_stats=False) uses batch statistics in eval mode too,
+    and momentum=None makes the running buffers a cumulative average (factor 1 / num_batches_tracked)."""
 
     @staticmethod
     def forward(ctx, y, gb, cb, key, bn, skip, skip_off, up, pad, post_leaky, sums_in=None, slope=0.2):
@@ -170,14 +179,15 @@ class _CBNActPad(torch.autograd.Function):
         goff, boff = cb.offsets[key]
         st = stream_ptr(y)
         mode, sums, count, sync, peers = 0, None, 1.0, False, None
-        if bn.training:
+        # F.batch_norm normalises with the batch statistics in training, and in eval too when there are no running buffers
+        if bn.training or bn.running_mean is None:
             if sums_in is not None:                     # accumulated by the epilogue of the convolution that produced y
                 sums = sums_in
             else:
                 sums = torch.empty(2 * C, device=y.device, dtype=torch.float64)
                 check(lib.b3d_bn_sums(ptr(y), N * H * W, C, ptr(sums), st))
             mode, count = 1, float(N * H * W)
-            if _dist_world() > 1 and bn.__class__.__name__.startswith("Synchronized"):
+            if bn.training and _dist_world() > 1 and bn.__class__.__name__.startswith("Synchronized"):
                 import torch.distributed as dist
                 from .sync import peer_sync
                 mode, count, sync = 2, count * dist.get_world_size(), True
@@ -189,15 +199,16 @@ class _CBNActPad(torch.autograd.Function):
         scale = torch.empty(N, C, device=y.device, dtype=torch.float32)
         shift, gt = torch.empty_like(scale), torch.empty_like(scale)
         track = bn.training and bn.track_running_stats
+        momentum = -1.0 if bn.momentum is None else float(bn.momentum)    # < 0: cumulative average, as torch for None
         if peers is not None:
             # statistics all-reduce over NVLink peer memory fused into the kernel that consumes them (csrc/ew_kernels.cu)
             check(lib.b3d_cbn_prepare_sync(peers.data, peers.flag, peers.rank, peers.world, ptr(peers.epoch), ptr(peers.err),
-                                           ptr(gbd), gp, goff, boff, ptr(sums), count, float(bn.eps), float(bn.momentum or 0.0),
+                                           ptr(gbd), gp, goff, boff, ptr(sums), count, float(bn.eps), momentum,
                                            ptr(bn.running_mean) if track else None, ptr(bn.running_var) if track else None,
                                            ptr(bn.num_batches_tracked) if track else None,
                                            ptr(mean), ptr(invstd), ptr(scale), ptr(shift), ptr(gt), N, C, st))
         else:
-            check(lib.b3d_cbn_prepare(ptr(gbd), gp, goff, boff, ptr(sums), count, float(bn.eps), float(bn.momentum or 0.0), mode,
+            check(lib.b3d_cbn_prepare(ptr(gbd), gp, goff, boff, ptr(sums), count, float(bn.eps), momentum, mode,
                                       ptr(bn.running_mean) if (track or mode == 0) else None,
                                       ptr(bn.running_var) if (track or mode == 0) else None,
                                       ptr(bn.num_batches_tracked) if track else None,
@@ -212,6 +223,8 @@ class _CBNActPad(torch.autograd.Function):
         ctx.cfg = (skip_off, up, pad, post_leaky, mode != 0, sync, count, sk is not None, skip.shape if skip is not None else None,
                    P, goff, boff, float(slope))
         ctx.peers = peers
+        # mode 2's inv_std of a clamped channel, as the kernels round it: (float)(1 / sqrt((double)eps))
+        ctx.clamp_lim = _f32(1.0 / math.sqrt(_f32(bn.eps))) if sync else None
         return out
 
     @staticmethod
@@ -246,6 +259,10 @@ class _CBNActPad(torch.autograd.Function):
                 if sync:
                     import torch.distributed as dist
                     dist.all_reduce(red)
+            if sync:
+                # the SyncBN formulas differentiate clamp(var, eps): where the variance is clamped, inv_std is a constant and
+                # the xhat coupling term vanishes (such channels carry exactly the clamp's inv_std = eps^-1/2)
+                red[C:].mul_(invstd < ctx.clamp_lim)
             inv_m = 1.0 / count
         else:
             red = torch.zeros(2 * C, device=y.device, dtype=torch.float32)

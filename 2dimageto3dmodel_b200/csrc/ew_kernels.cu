@@ -523,6 +523,20 @@ extern "C" int b3d_bn_stats(const float* y, long long rows, int C, float eps, fl
 // mode 0: eval (running statistics).  mode 1: batch statistics from fp64 sums [2][C] over `count` values per channel with
 // F.batch_norm's formulas (biased variance + eps under the root; running variance unbiased).  mode 2: the reference's
 // SyncBN formulas on the (all-reduced) sums: inv_std = clamp(var, eps)^-1/2 (sync_batchnorm/batchnorm.py:133-150).
+// momentum < 0 selects torch's cumulative average (BatchNorm momentum=None): factor 1 / (num_batches_tracked + 1).
+__device__ __forceinline__ void cbn_batch_stats(const double* __restrict__ sums, double count, float eps, int mode, int C, int c,
+                                                float& mean, float& invstd, double& var_b) {
+    const double m = sums[c] / count;
+    var_b = mode == 1 ? sums[C + c] / count - m * m : (sums[C + c] - sums[c] * m) / count;
+    if (mode == 1) var_b = var_b > 0.0 ? var_b : 0.0;
+    mean = (float)m;
+    invstd = mode == 1 ? (float)(1.0 / sqrt(var_b + (double)eps)) : (float)(1.0 / sqrt(var_b > (double)eps ? var_b : (double)eps));
+}
+
+__device__ __forceinline__ float cbn_momentum(float momentum, const long long* nbt) {
+    return momentum >= 0.f ? momentum : (nbt != nullptr ? (float)(1.0 / (double)(*nbt + 1)) : 0.f);
+}
+
 __global__ void __launch_bounds__(NT)
 cbn_prepare_kernel(const float* __restrict__ gb, int gb_pitch, int gamma_off, int beta_off, const double* __restrict__ sums,
                    double count, float eps, float momentum, int mode, float* __restrict__ running_mean,
@@ -530,33 +544,39 @@ cbn_prepare_kernel(const float* __restrict__ gb, int gb_pitch, int gamma_off, in
                    float* __restrict__ invstd_out, float* __restrict__ scale, float* __restrict__ shift, float* __restrict__ gt,
                    int N, int C) {
     const int i = blockIdx.x * NT + threadIdx.x;
-    if (i >= N * C) return;
-    const int n = i / C, c = i - n * C;
-    float mean, invstd;
-    double var_b = 0.0;
-    if (mode == 0) {
-        mean = running_mean[c];
-        invstd = rsqrtf(running_var[c] + eps);
-    } else {
-        const double m = sums[c] / count;
-        var_b = mode == 1 ? sums[C + c] / count - m * m : (sums[C + c] - sums[c] * m) / count;
-        if (mode == 1) var_b = var_b > 0.0 ? var_b : 0.0;
-        mean = (float)m;
-        invstd = mode == 1 ? (float)(1.0 / sqrt(var_b + (double)eps)) : (float)(1.0 / sqrt(var_b > (double)eps ? var_b : (double)eps));
-    }
-    const float g1 = 1.f + gb[(long long)n * gb_pitch + gamma_off + c];
-    const float sc = invstd * g1;
-    scale[i] = sc;
-    shift[i] = gb[(long long)n * gb_pitch + beta_off + c] - mean * sc;
-    gt[i] = g1;
-    if (n == 0) {
-        mean_out[c] = mean;
-        invstd_out[c] = invstd;
-        if (mode != 0 && running_mean != nullptr) {      // all reads of the running buffers above happen in mode 0 only
-            running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mean;
-            running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)(var_b * (count / (count > 1.0 ? count - 1.0 : 1.0)));
-            if (c == 0 && nbt != nullptr) *nbt += 1;
+    if (i < N * C) {
+        const int n = i / C, c = i - n * C;
+        float mean, invstd;
+        double var_b;
+        if (mode == 0) {
+            mean = running_mean[c];
+            invstd = rsqrtf(running_var[c] + eps);
+        } else {
+            cbn_batch_stats(sums, count, eps, mode, C, c, mean, invstd, var_b);
         }
+        const float g1 = 1.f + gb[(long long)n * gb_pitch + gamma_off + c];
+        const float sc = invstd * g1;
+        scale[i] = sc;
+        shift[i] = gb[(long long)n * gb_pitch + beta_off + c] - mean * sc;
+        gt[i] = g1;
+        if (n == 0) {
+            mean_out[c] = mean;
+            invstd_out[c] = invstd;
+        }
+    }
+    // Running buffers (modes 1, 2; mode 0 is the only one that reads them above): block 0 alone updates every channel, so
+    // all its threads read num_batches_tracked (the momentum=None factor) before the barrier and thread 0 increments after it.
+    if (blockIdx.x == 0 && mode != 0 && running_mean != nullptr) {
+        const float f = cbn_momentum(momentum, nbt);
+        for (int c = threadIdx.x; c < C; c += NT) {
+            float mean, invstd;
+            double var_b;
+            cbn_batch_stats(sums, count, eps, mode, C, c, mean, invstd, var_b);
+            running_mean[c] = (1.f - f) * running_mean[c] + f * mean;
+            running_var[c] = (1.f - f) * running_var[c] + f * (float)(var_b * (count / (count > 1.0 ? count - 1.0 : 1.0)));
+        }
+        __syncthreads();
+        if (threadIdx.x == 0 && nbt != nullptr) *nbt += 1;
     }
 }
 
@@ -626,6 +646,7 @@ cbn_prepare_sync_kernel(SyncPeers P, int rank, int world, unsigned* epoch_ctr, i
                         float* __restrict__ scale, float* __restrict__ shift, float* __restrict__ gt, int N, int C) {
     __shared__ double tot[SYNC_MAX];
     __shared__ float mean_s[SYNC_MAX / 2], inv_s[SYNC_MAX / 2];
+    const float f = cbn_momentum(momentum, nbt);            // read before the barriers in peer_allreduce, incremented after
     for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) tot[i] = sums_local[i];
     __syncthreads();
     peer_allreduce(P, rank, world, epoch_ctr, err, tot, 2 * C);
@@ -638,8 +659,8 @@ cbn_prepare_sync_kernel(SyncPeers P, int rank, int world, unsigned* epoch_ctr, i
         mean_out[c] = mean;
         invstd_out[c] = invstd;
         if (running_mean != nullptr) {
-            running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mean;
-            running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)(var_b * (count / (count > 1.0 ? count - 1.0 : 1.0)));
+            running_mean[c] = (1.f - f) * running_mean[c] + f * mean;
+            running_var[c] = (1.f - f) * running_var[c] + f * (float)(var_b * (count / (count > 1.0 ? count - 1.0 : 1.0)));
             if (c == 0 && nbt != nullptr) *nbt += 1;
         }
     }

@@ -30,20 +30,21 @@ class _SyncStats(torch.autograd.Function):
         inv_std = var.clamp(min=eps) ** -0.5
         shape = [1, C] + [1] * (x.dim() - 2)
         xhat = (x - mean.view(shape)) * inv_std.view(shape)
-        ctx.save_for_backward(xhat, inv_std)
+        ctx.save_for_backward(xhat, inv_std, var >= eps)
         ctx.group, ctx.n = group, n
         ctx.mark_non_differentiable(mean, var)
         return xhat, mean, var
 
     @staticmethod
     def backward(ctx, g, _gm, _gv):
-        xhat, inv_std = ctx.saved_tensors
+        xhat, inv_std, unclamped = ctx.saved_tensors
         C = xhat.shape[1]
         red = [0] + list(range(2, xhat.dim()))
         sums = torch.stack((g.sum(dim=red), (g * xhat).sum(dim=red)))
         dist.all_reduce(sums, group=ctx.group)
         shape = [1, C] + [1] * (xhat.dim() - 2)
-        gx = (g - sums[0].view(shape) / ctx.n - xhat * (sums[1].view(shape) / ctx.n)) * inv_std.view(shape)
+        # d clamp(var, eps) / d var = 0 where the variance is clamped: no xhat coupling term in those channels
+        gx = (g - sums[0].view(shape) / ctx.n - xhat * (sums[1] * unclamped / ctx.n).view(shape)) * inv_std.view(shape)
         return gx, None, None
 
 

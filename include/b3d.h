@@ -404,7 +404,9 @@ B3D_API int b3d_bn_stats(const float* y, long long rows, int C, float eps, float
  *       pitch s_pitch floats (>= C; slices of the batched d(gamma, beta) buffer), zeroed by the call
  * bwd2 (in place on ga): dy = inv_std * (ga * gamma_t - m1 - xhat * m2), (m1, m2) [C] = inv_m * (sums of d xhat, d xhat * xhat)
  * b3d_cbn_prepare / b3d_cbn_bwd_reduce / b3d_bn_sums: the per-layer scalar math around these passes, one launch each
- *       (statistics -> mean / inv_std / running buffers / scale / shift; coupling-term reduction; fp64 channel sums).       */
+ *       (statistics -> mean / inv_std / running buffers / scale / shift; coupling-term reduction; fp64 channel sums).
+ *       momentum < 0 updates the running buffers as a cumulative average (torch's momentum=None): factor
+ *       1 / (num_batches_tracked + 1), read on the device before the counter is incremented.                               */
 B3D_API int b3d_cbn_act_fwd(const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch,
                             int skip_off, float* out, int N, int H, int W, int C, int up, int pad, float slope,
                             int post_leaky, void* stream);

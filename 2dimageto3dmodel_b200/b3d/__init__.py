@@ -50,9 +50,6 @@ def _sig(name, *argtypes):
 
 
 _sig("b3d_pc_bin_count", _i)
-_sig("b3d_pc_tma_staging")
-_sig("b3d_pc_stage_records")
-_sig("b3d_pc_stream_plan", _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i)
 _sig("b3d_inception_input", _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp)
 _sig("b3d_maxpool3x3s2_nhwc", _vp, _i, _i, _i, _i, _vp, _i, _vp)
 _sig("b3d_mean_hw_nhwc", _vp, _i, _i, _i, _vp, _vp)
@@ -60,15 +57,12 @@ _sig("b3d_fid_accumulate", _vp, _i, _i, _vp, _vp, _vp)
 _sig("b3d_pc_project", _vp, _vp, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp)
 _sig("b3d_pc_silhouette_fwd_hosttaps", _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp)
 _sig("b3d_pc_silhouette_bwd_hosttaps", _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp)
-_sig("b3d_pc_silhouette_fwd", _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _sz, _vp)
-_sig("b3d_pc_silhouette_bwd", _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp)
 _sig("b3d_pc_project_bwd", _vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _vp, _vp, _vp)
 _sig("b3d_pc_splat_grid", _vp, _i, _i, _i, _i, _vp, _vp)
 _sig("b3d_mesh_face_setup", _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp)
 _sig("b3d_mesh_render_fwd", _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp)
 _sig("b3d_conv2d_tf32", _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i,
-     _f, _i, _vp, _i, _vp, _i, _i, _vp, _vp)
-_sig("b3d_conv2d_flat_tf32", _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _f, _vp)
+     _f, _vp, _i, _vp, _i, _i, _vp, _vp)
 _sig("b3d_conv2d_wgrad_tf32", _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp)
 _sig("b3d_conv2d_thin_fwd", _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _vp)
 _sig("b3d_conv2d_thin_wgrad", _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp)
@@ -94,7 +88,6 @@ _sig("b3d_vox_termination_bwd", _vp, _vp, _i, _i, _i, _vp, _vp)
 _sig("b3d_vox_splat_sorted", _vp, _vp, _i, _i, _i, _i, _vp, _vp)
 _sig("b3d_vox_clamp01", _vp, ctypes.c_longlong, _vp)
 _sig("b3d_vox_gather", _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp)
-_sig("b3d_bn_stats", _vp, _ll, _i, _f, _vp, _vp, _vp, _vp)
 _sig("b3d_cbn_act_fwd", _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _f, _i, _vp)
 _sig("b3d_cbn_act_bwd1", _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _i, _vp)
 _sig("b3d_cbn_act_bwd2", _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _vp)
@@ -218,6 +211,6 @@ def prof_disable():
 
 _TIMED = ("b3d_pc_project", "b3d_pc_silhouette_fwd_hosttaps", "b3d_pc_silhouette_bwd_hosttaps", "b3d_pc_project_bwd",
           "b3d_pc_splat_grid", "b3d_mesh_face_setup", "b3d_mesh_render_fwd", "b3d_mesh_render_bwd", "b3d_face_normals_fwd", "b3d_face_normals_bwd", "b3d_flat_loss_fwd",
-          "b3d_flat_loss_bwd", "b3d_rgba_mse_iou_fwd", "b3d_rgba_mse_bwd", "b3d_rgba_l1_iou_fwd", "b3d_rgba_l1_bwd", "b3d_chamfer_nn", "b3d_chamfer_bwd", "b3d_conv2d_tf32", "b3d_conv2d_flat_tf32", "b3d_conv2d_wgrad_tf32", "b3d_conv2d_thin_fwd", "b3d_conv2d_thin_wgrad", "b3d_pad_x_fwd", "b3d_pad_x_bwd", "b3d_stem_input_fwd", "b3d_stem_input_bwd",
-          "b3d_leaky_bwd", "b3d_bn_stats", "b3d_wrap_x_inplace", "b3d_wrap_x_bwd_inplace", "b3d_pad_leaky_bias_bwd", "b3d_fold_rows_fwd", "b3d_fold_rows_bwd", "b3d_cbn_act_fwd", "b3d_cbn_act_bwd1", "b3d_cbn_act_bwd2", "b3d_bn_sums", "b3d_cbn_prepare", "b3d_cbn_bwd_reduce",
+          "b3d_flat_loss_bwd", "b3d_rgba_mse_iou_fwd", "b3d_rgba_mse_bwd", "b3d_rgba_l1_iou_fwd", "b3d_rgba_l1_bwd", "b3d_chamfer_nn", "b3d_chamfer_bwd", "b3d_conv2d_tf32", "b3d_conv2d_wgrad_tf32", "b3d_conv2d_thin_fwd", "b3d_conv2d_thin_wgrad", "b3d_pad_x_fwd", "b3d_pad_x_bwd", "b3d_stem_input_fwd", "b3d_stem_input_bwd",
+          "b3d_leaky_bwd", "b3d_wrap_x_inplace", "b3d_wrap_x_bwd_inplace", "b3d_pad_leaky_bias_bwd", "b3d_fold_rows_fwd", "b3d_fold_rows_bwd", "b3d_cbn_act_fwd", "b3d_cbn_act_bwd1", "b3d_cbn_act_bwd2", "b3d_bn_sums", "b3d_cbn_prepare", "b3d_cbn_bwd_reduce",
           "b3d_bank_forward", "b3d_bank_backward", "b3d_vertex_pipeline_fwd", "b3d_vertex_pipeline_bwd")

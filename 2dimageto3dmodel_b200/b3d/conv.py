@@ -4,7 +4,6 @@ Reference call sites: nn.Conv2d layers of /root/reference/code/models/gan.py (:5
 :359, :364) — 3x3 / 1x1 / 5x5 stride 1 and 4x4 stride 2, zero padding along y only (x padding is explicit:
 replicate / circular pads are materialised by the caller exactly as the reference does)."""
 import ctypes
-import os
 
 import torch
 
@@ -32,11 +31,10 @@ def taps_layout(weight):
 
 
 def _thin(Cout, Cin, kh, kw, stride):
-    return Cout <= 4 and Cin % 64 == 0 and kh == 5 and kw == 5 and stride == 1 and not os.environ.get("B3D_NO_THIN")
+    return Cout <= 4 and Cin % 64 == 0 and kh == 5 and kw == 5 and stride == 1
 
 
-def conv2d_nhwc(x, weight, bias=None, pad_y=0, stride=1, leaky=1.0, wt=None, cin_major=False, pad_out=0, pad_mode=1,
-                x_crop=0):
+def conv2d_nhwc(x, weight, bias=None, pad_y=0, stride=1, leaky=1.0, wt=None, pad_out=0, pad_mode=1, x_crop=0):
     """x [N,H,W,Cin] (Cin % 32 == 0), weight [Cout,Cin,kh,kw] -> [N,Hout,Wout,Cout]; zero pad along y only.
     pad_out > 0: the result is written into the interior of a [N,Hout,Wout + 2*pad_out,Cout] buffer whose pad columns
     are then filled in place (replicate / circular) — the next convolution's padded input without a copy.
@@ -47,7 +45,7 @@ def conv2d_nhwc(x, weight, bias=None, pad_y=0, stride=1, leaky=1.0, wt=None, cin
     if Cin_w != Cin:
         raise B3DError(f"conv2d: input has {Cin} channels, weight expects {Cin_w}")
     if wt is None:
-        wt = weight.permute(2, 3, 1, 0).reshape(kh * kw, Cin, Cout).contiguous() if cin_major else taps_layout(weight)
+        wt = taps_layout(weight)
     wt = dev(wt, "weight")
     Hout = (H + 2 * pad_y - kh) // stride + 1
     if x_crop and stride != 1:
@@ -58,7 +56,7 @@ def conv2d_nhwc(x, weight, bias=None, pad_y=0, stride=1, leaky=1.0, wt=None, cin
     optr = ctypes.c_void_p(out.data_ptr() + 4 * pad_out * Cout)          # pixel (n, y, pad_out) of the padded buffer
     if pad_out and Cout % 4:
         raise B3DError("conv2d: pad_out needs Cout % 4 == 0")
-    if _thin(Cout, Cin, kh, kw, stride) and not cin_major:
+    if _thin(Cout, Cin, kh, kw, stride):
         # 1-4 output channels: fp32 CUDA-core reduction kernel (csrc/thin_kernels.cu), not a 64-wide MMA tile
         check(_conv_call(lib.b3d_conv2d_thin_fwd, ptr(x), ptr(wt), ptr(dev(bias, "bias") if bias is not None else None), optr, N, H, W,
                                       Cin, Hout, Wout, Cout, kh, kw, pad_y, x_crop, OW, Cout, float(leaky), stream_ptr(x)))
@@ -69,7 +67,7 @@ def conv2d_nhwc(x, weight, bias=None, pad_y=0, stride=1, leaky=1.0, wt=None, cin
     dx = [s + x_crop for _ in range(kh) for s in range(kw)]
     b = dev(bias, "bias") if bias is not None else None
     check(_conv_call(lib.b3d_conv2d_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw, _ints(dy),
-                              _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), int(cin_major), None, 0, None, 0, 0,
+                              _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), None, 0, None, 0, 0,
                               None, stream_ptr(x)))
     if pad_out:
         check(lib.b3d_wrap_x_inplace(ptr(out), N * Hout, Wout, Cout, pad_out, pad_mode, stream_ptr(x)))
@@ -104,7 +102,7 @@ def conv2d_dgrad_nhwc(dy_, weight, in_hw, pad_y=0, stride=1, x_crop=0):
         dy = [pad_y - r for r in range(kh) for _ in range(kw)]
         dx = [-s - x_crop for _ in range(kh) for s in range(kw)]
         check(_conv_call(lib.b3d_conv2d_tf32, ptr(g), ptr(wt), None, ptr(dxo), N, Hout, Wout, Cout, H, W, Cin, kh * kw, _ints(dy),
-                                  _ints(dx), 1, 1, H, W, Cin, 1, 1, 0, 0, 1.0, 0, None, 0, None, 0, 0, None, st))
+                                  _ints(dx), 1, 1, H, W, Cin, 1, 1, 0, 0, 1.0, None, 0, None, 0, 0, None, st))
         return dxo
     if stride != 2 or x_crop:
         raise B3DError("conv2d_dgrad: stride must be 1 or 2 (x_crop: stride 1 only)")
@@ -114,7 +112,7 @@ def conv2d_dgrad_nhwc(dy_, weight, in_hw, pad_y=0, stride=1, x_crop=0):
             continue
         wt = torch.stack([weight[:, :, r, s].t() for r, s in rs]).contiguous()      # [taps][Cin][Cout]
         check(_conv_call(lib.b3d_conv2d_tf32, ptr(g), ptr(wt), None, ptr(dxo), N, Hout, Wout, Cout, Ha, Wa, Cin, len(rs),
-                                  _ints(dy), _ints(dx), 1, 1, H, W, Cin, 2, 2, cy, cx, 1.0, 0, None, 0, None, 0, 0, None, st))
+                                  _ints(dy), _ints(dx), 1, 1, H, W, Cin, 2, 2, cy, cx, 1.0, None, 0, None, 0, 0, None, st))
     return dxo
 
 
@@ -213,16 +211,13 @@ def fold_kh_weight(weight, cpad=0):
     return torch.nn.functional.pad(w, (0, 0, 0, 0, 0, cpad)) if cpad else w
 
 
-_FOLD = os.environ.get("B3D_FOLD", "kh")
-
-
 def conv2d(x_nchw, weight, bias=None, pad_y=0, stride=1, leaky=1.0, pad_out=0, pad_mode=1, x_crop=0):
     """Drop-in for F.conv2d(x, w, b, stride, padding=(pad_y, 0)) on logically-NCHW tensors: runs on the wgmma
     kernels over the channels-last storage (a no-copy view when x is already channels_last) and returns a
     logically-NCHW, channels-last tensor."""
     x = x_nchw.permute(0, 2, 3, 1)
     Cout, Cin, kh, kw = weight.shape
-    if stride == 1 and kh > 1 and Cin * kh <= 64 and _FOLD == "kh":
+    if stride == 1 and kh > 1 and Cin * kh <= 64:
         # thin stems (discriminator conv1: 8 or 11 input channels, 5x5): fold the kh vertical taps into the channel
         # dimension — X'[n,y,x, r*Cin + c] = X[n, y+r-pad_y, x, c] (zero rows = the y padding) — so the tensor cores see
         # kw taps of kh*Cin real channels instead of kh*kw taps of Cin channels zero-padded to 32.  The remaining taps
@@ -232,17 +227,6 @@ def conv2d(x_nchw, weight, bias=None, pad_y=0, stride=1, leaky=1.0, pad_out=0, p
         x = fold_rows(x, kh, pad_y, kh * Cin + cpad)
         weight = fold_kh_weight(weight, cpad)
         pad_y = 0
-    elif stride == 1 and kw > 1 and Cin * kw <= 64:
-        # same fold along x (B3D_FOLD=kw): X'[n,y,x, s*Cin + c] = X[n,y,x+s,c], kh vertical taps remain
-        Wout = x.shape[2] - kw + 1
-        cpad = (-kw * Cin) % 32
-        parts = [x[:, :, s:s + Wout, :] for s in range(kw)]
-        if cpad:
-            parts.append(x.new_zeros(x.shape[0], x.shape[1], Wout, cpad))
-        x = torch.cat(parts, dim=3)
-        weight = weight.permute(0, 3, 1, 2).reshape(Cout, kw * Cin, kh, 1)          # [co, s*Cin + c, r, 0]
-        if cpad:
-            weight = torch.nn.functional.pad(weight, (0, 0, 0, 0, 0, cpad))
     y = _Conv2dNHWC.apply(x, weight, bias, int(pad_y), int(stride), float(leaky), int(pad_out), int(pad_mode), int(x_crop))
     return y.permute(0, 3, 1, 2)
 
@@ -271,6 +255,12 @@ class ActLink:
     def __init__(self):
         self.armed = self.done = False
         self.gb = None
+
+
+def _merge_parity_classes(classes):
+    """One launch for the four parity classes of a stride-2 input gradient when they have the same extent and tap count
+    (even H, W; 4x4 kernels); otherwise one launch per class."""
+    return len(classes) == 4 and all(c[2] for c in classes) and len({(len(c[2]), c[5], c[6]) for c in classes}) == 1
 
 
 class _ConvBanked(torch.autograd.Function):
@@ -316,7 +306,7 @@ class _ConvBanked(torch.autograd.Function):
             if stats is not None and (bias is not None or leaky != 1.0 or stride != 1):
                 raise B3DError("banked conv: output statistics are taken before bias / activation (plain stride-1 convs only)")
             check(_conv_call(lib.b3d_conv2d_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw,
-                             _ints(dy), _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), 0, None, 0, ptr(stats),
+                             _ints(dy), _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), None, 0, ptr(stats),
                              fold_raw, fold_pad, None, st))
         if pad_out:
             check(lib.b3d_wrap_x_inplace(ptr(out), N * Hout, Wout, Cout, pad_out, pad_mode, st))
@@ -386,9 +376,7 @@ class _ConvBanked(torch.autograd.Function):
             link_in = ctx.link_in if (stride == 1 or (stride == 2 and not x_crop)) else None
             opts, sums = None, None
             classes = stride2_classes(kh, kw, pad_y, H, W) if (stride == 2 and not x_crop) else []
-            # one launch for the four parity classes when they have the same extent and tap count (even H, W; 4x4 kernels)
-            merged = (len(classes) == 4 and all(c[2] for c in classes) and len({(len(c[2]), c[5], c[6]) for c in classes}) == 1
-                      and not os.environ.get("B3D_DGRAD_PER_CLASS"))
+            merged = _merge_parity_classes(classes)
             if g_pitch or link_in is not None or merged:
                 opts = _ConvOpts(None, 1.0, 0, g_pitch, 0)
                 if link_in is not None:                                # LeakyReLU adjoint of the PRODUCER of x in this epilogue
@@ -400,7 +388,7 @@ class _ConvBanked(torch.autograd.Function):
                 dy = [pad_y - r for r in range(kh) for _ in range(kw)]
                 dx = [-s - x_crop for _ in range(kh) for s in range(kw)]
                 check(_conv_call(lib.b3d_conv2d_tf32, gptr, ptr(wd), None, ptr(gx), N, Hout, Wout, Cop, H, W, Cin, kh * kw,
-                                 _ints(dy), _ints(dx), 1, 1, H, W, Cin, 1, 1, 0, 0, 1.0, 0, None, 0, ptr(sums), 0, 0, optr_, st))
+                                 _ints(dy), _ints(dx), 1, 1, H, W, Cin, 1, 1, 0, 0, 1.0, None, 0, ptr(sums), 0, 0, optr_, st))
             elif merged:
                 opts.nclass = 4
                 for i, c in enumerate(classes):
@@ -409,7 +397,7 @@ class _ConvBanked(torch.autograd.Function):
                 dx = [v for c in classes for v in c[4]]
                 taps = [r * kw + s for c in classes for r, s in c[2]]   # rows of the tap-major D array: no gathered copy
                 check(_conv_call(lib.b3d_conv2d_tf32, gptr, ptr(wd), None, ptr(gx), N, Hout, Wout, Cop, classes[0][5], classes[0][6], Cin,
-                                 len(taps), _ints(dy), _ints(dx), 1, 1, H, W, Cin, 2, 2, 0, 0, 1.0, 0, _ints(taps), kh * kw,
+                                 len(taps), _ints(dy), _ints(dx), 1, 1, H, W, Cin, 2, 2, 0, 0, 1.0, _ints(taps), kh * kw,
                                  ptr(sums), 0, 0, optr_, st))
             elif stride == 2 and not x_crop:
                 for cy, cx, rs, dy, dx, Ha, Wa in classes:
@@ -418,7 +406,7 @@ class _ConvBanked(torch.autograd.Function):
                         continue
                     taps = [r * kw + s for r, s in rs]                  # rows of the tap-major D array: no gathered copy
                     check(_conv_call(lib.b3d_conv2d_tf32, gptr, ptr(wd), None, ptr(gx), N, Hout, Wout, Cop, Ha, Wa, Cin,
-                                     len(rs), _ints(dy), _ints(dx), 1, 1, H, W, Cin, 2, 2, cy, cx, 1.0, 0, _ints(taps), kh * kw,
+                                     len(rs), _ints(dy), _ints(dx), 1, 1, H, W, Cin, 2, 2, cy, cx, 1.0, _ints(taps), kh * kw,
                                      ptr(sums), 0, 0, optr_, st))
             else:
                 raise B3DError("conv2d_dgrad: stride must be 1 or 2 (x_crop: stride 1 only)")
@@ -461,7 +449,7 @@ def conv2d_banked(x_nchw, lw, pad_y=0, stride=1, leaky=1.0, pad_out=0, pad_mode=
         Wout = x.shape[2] - lw.kw + 1
         need_wgrad = torch.is_grad_enabled() and lw.wf.requires_grad
         if (lw.Cin == 8 and stride == 1 and not x_crop and Wout % 128 == 0 and x.shape[0] * x.shape[1] * (Wout // 128) >= 2 * torch.cuda.get_device_properties(x.device).multi_processor_count
-                and not need_wgrad and not os.environ.get("B3D_FOLD_MATERIALIZE")):
+                and not need_wgrad):
             # 8-channel stems of wide images when no weight gradient is taken (generator step: the discriminator is frozen):
             # the forward kernel folds the kh rows on the fly (TMA boxes of 4 rows x 8 channels), no folded tensor is written.
             fold_raw = lw.kh

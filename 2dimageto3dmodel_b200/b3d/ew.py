@@ -1,7 +1,6 @@
 """One-pass NHWC helper ops between the convolutions (libb3d csrc/ew_kernels.cu), with autograd."""
 import ctypes
 import math
-import os
 import struct
 
 import torch
@@ -276,23 +275,6 @@ class _CBNActPad(torch.autograd.Function):
                     raise RuntimeError(f"CBNBatch: {cb.done} of {cb.n_layers} layers ran their backward before the first layer's")
                 ggb = sink.sum(dim=0, keepdim=True) if cb.shared else sink
         return ga, ggb, None, None, None, gskip, None, None, None, None, None, None
-
-
-_BN_STATS_IMPL = os.environ.get("B3D_BN_STATS", "torch")
-
-
-def bn_stats(y_nhwc, eps, impl=None):
-    """(mean, invstd) per channel of an NHWC tensor = torch.batch_norm_stats on the NCHW view.  impl "b3d" = the one-pass
-    libb3d kernel, "torch" = the stock op."""
-    y = dev(y_nhwc, "y")
-    C = y.shape[-1]
-    if C % 4 or 256 % (C // 4) or (impl or _BN_STATS_IMPL) != "b3d":     # odd channel counts: always the stock op
-        return torch.batch_norm_stats(y.permute(0, 3, 1, 2), eps)
-    mean = torch.empty(C, device=y.device, dtype=torch.float32)
-    invstd = torch.empty_like(mean)
-    ws = torch.empty(2 * C, device=y.device, dtype=torch.float64)
-    check(lib.b3d_bn_stats(ptr(y), y.numel() // C, C, float(eps), ptr(mean), ptr(invstd), ptr(ws), stream_ptr(y)))
-    return mean, invstd
 
 
 def bn_act_pad(y_nchw, bn, skip_nchw=None, skip_off=0, up=1, pad=1, post_relu=False, slope=0.0):

@@ -3,10 +3,9 @@ all-reduce over NVLink / NVSwitch fused into the kernel that consumes the statis
 of the reference does a thread rendezvous + two comm ops per layer; round 1 here did one NCCL all-reduce per layer).
 
 One process per GPU (torch.distributed, NCCL): a symmetric buffer from torch's symmetric-memory allocator is mapped into
-every peer; the kernels get the table of peer pointers.  Falls back to NCCL collectives (b3d.ew) when symmetric memory is
-unavailable or B3D_SYNC_FUSED=0."""
+every peer; the kernels get the table of peer pointers.  Falls back to NCCL collectives (b3d.ew) when the backend is not
+NCCL or symmetric memory is unavailable."""
 import ctypes
-import os
 
 import torch
 import torch.distributed as dist
@@ -51,10 +50,10 @@ class PeerSync:
 
 
 def peer_sync(device):
-    """The process-wide PeerSync, or None (single process, disabled, or symmetric memory unavailable -> NCCL path)."""
+    """The process-wide PeerSync, or None (single process, another backend, or symmetric memory unavailable -> NCCL path)."""
     if _state["inst"] is None:
         inst = False
-        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and os.environ.get("B3D_SYNC_FUSED", "1") != "0" \
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 \
                 and dist.get_backend() == "nccl":
             try:
                 inst = PeerSync(device)

@@ -442,14 +442,14 @@ int b3d_leaky_bwd(const float* gy, const float* y, float* out, long long n, floa
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Batch statistics of an NHWC activation for the generator's (Sync)BatchNorm layers (models/gan.py:211-232 ->
-// F.batch_norm / sync_batchnorm/batchnorm.py:150): per-channel mean and 1/sqrt(biased var + eps) in one pass over the
-// tensor.  Threads own a channel quad and stride over the pixels (fp32 partial sums of ~50-100 values), a block folds its
-// pixel lanes in shared memory and adds into fp64 accumulators; a second tiny kernel finishes.
+// Per-channel fp64 sums and sums of squares of an NHWC activation for the (Sync)BatchNorm layers (models/gan.py:211-232 ->
+// F.batch_norm / sync_batchnorm/batchnorm.py:150) in one pass over the tensor.  Threads own a channel quad and stride over
+// the pixels (fp32 partial sums of ~50-100 values), a block folds its pixel lanes in shared memory and adds into fp64
+// accumulators.
 // ------------------------------------------------------------------------------------------------------------------
 namespace {
 __global__ void __launch_bounds__(NT)
-bn_stats_partial_kernel(const float4* __restrict__ y, long long rows, int C4, double* __restrict__ ws) {
+bn_sums_kernel(const float4* __restrict__ y, long long rows, int C4, double* __restrict__ ws) {
     __shared__ float4 rs[NT], rq[NT];
     const int c = threadIdx.x % C4, lane_p = threadIdx.x / C4, PPB = NT / C4;
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = s;
@@ -485,36 +485,7 @@ bn_stats_partial_kernel(const float4* __restrict__ y, long long rows, int C4, do
         atomicAdd(ws + C + 4 * c + 2, (double)n.z); atomicAdd(ws + C + 4 * c + 3, (double)n.w);
     }
 }
-
-__global__ void bn_stats_finish_kernel(const double* __restrict__ ws, long long rows, int C, float eps, float* __restrict__ mean,
-                                       float* __restrict__ invstd) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= C) return;
-    const double m = ws[c] / (double)rows;
-    double var = ws[C + c] / (double)rows - m * m;
-    var = var > 0.0 ? var : 0.0;
-    mean[c] = (float)m;
-    invstd[c] = (float)(1.0 / sqrt(var + (double)eps));
-}
 }  // namespace
-
-extern "C" int b3d_bn_stats(const float* y, long long rows, int C, float eps, float* mean, float* invstd, double* workspace,
-                            void* stream) {
-    B3D_REQUIRE(rows > 0 && C >= 4 && C % 4 == 0 && C / 4 <= NT && NT % (C / 4) == 0, B3D_EINVAL,
-                "b3d_bn_stats: C=%d must be 4 * a divisor of %d", C, NT);
-    B3D_REQUIRE(y && mean && invstd && workspace, B3D_EINVAL, "b3d_bn_stats: null pointer");
-    B3D_CHECK_ALIGNED(y);
-    cudaStream_t st = (cudaStream_t)stream;
-    B3D_CUDA_OK(cudaMemsetAsync(workspace, 0, sizeof(double) * 2 * (size_t)C, st));
-    const int ppb = NT / (C / 4);
-    long long blocks = (rows + ppb - 1) / ppb;
-    if (blocks > 132 * 2) blocks = 132 * 2;                 // few blocks: every block ends with 2C same-address fp64 atomics
-    bn_stats_partial_kernel<<<(int)blocks, NT, 0, st>>>((const float4*)y, rows, C / 4, workspace);
-    B3D_LAUNCH_OK();
-    bn_stats_finish_kernel<<<(C + 127) / 128, 128, 0, st>>>(workspace, rows, C, eps, mean, invstd);
-    B3D_LAUNCH_OK();
-    return B3D_OK;
-}
 
 // ------------------------------------------------------------------------------------------------------------------
 // Per-layer scalar math of ConditionalBatchNorm2d in ONE launch (was ~15 tiny torch kernels per layer and forward):
@@ -933,8 +904,8 @@ int b3d_cbn_act_bwd2(float* ga, const float* y, const float* gamma_t, const floa
     return B3D_OK;
 }
 
-// fp64 per-channel sums [2][C] (sum, sum of squares) of y [rows, C]: the first half of b3d_bn_stats, for callers that
-// all-reduce the sums across ranks (SyncBN) and finish in b3d_cbn_prepare.  `sums` is zeroed here.
+// fp64 per-channel sums [2][C] (sum, sum of squares) of y [rows, C], for callers that all-reduce the sums across ranks
+// (SyncBN) and finish in b3d_cbn_prepare.  `sums` is zeroed here.
 int b3d_bn_sums(const float* y, long long rows, int C, double* sums, void* stream) {
     B3D_REQUIRE(rows > 0 && C >= 4 && C % 4 == 0 && C / 4 <= NT && NT % (C / 4) == 0, B3D_EINVAL,
                 "b3d_bn_sums: C=%d must be 4 * a divisor of %d", C, NT);
@@ -944,8 +915,8 @@ int b3d_bn_sums(const float* y, long long rows, int C, double* sums, void* strea
     B3D_CUDA_OK(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * (size_t)C, st));
     const int ppb = NT / (C / 4);
     long long blocks = (rows + ppb - 1) / ppb;
-    if (blocks > 132 * 2) blocks = 132 * 2;
-    bn_stats_partial_kernel<<<(int)blocks, NT, 0, st>>>((const float4*)y, rows, C / 4, sums);
+    if (blocks > 132 * 2) blocks = 132 * 2;                 // few blocks: every block ends with 2C same-address fp64 atomics
+    bn_sums_kernel<<<(int)blocks, NT, 0, st>>>((const float4*)y, rows, C / 4, sums);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }

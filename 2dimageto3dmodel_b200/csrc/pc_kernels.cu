@@ -238,7 +238,9 @@ __device__ __forceinline__ float scaled(float S, bool has_scale, float sc) {
 constexpr int TILE_THREADS = 512;
 
 // One sorted record (gz, gy, gx, bits(index)) splatted into a shared patch covering cells [cy0, cy1] x [cx0, cx1]
-// (row pitch `pitch`), depth-major.  zlo / zhi [ncol]: occupied depth range of every column (see splat_bins).
+// (row pitch `pitch`), depth-major.  zlo / zhi [ncol] (initialised to V / -1 by the caller): occupied depth range of every
+// column — cells outside it are exactly zero, so their blur, clamp and ray-march terms are constants (the sparsity skip of
+// the fwd / bwd kernels).
 __device__ __forceinline__ void splat_record(const float4 g, int cy0, int cy1, int cx0, int cx1, int pitch, int ncol,
                                              int mode, float* A, int* zlo, int* zhi) {
     const float fzf = floorf(g.x), fyf = floorf(g.y), fxf = floorf(g.z);
@@ -266,123 +268,13 @@ __device__ __forceinline__ void splat_record(const float4 g, int cy0, int cy1, i
     }
 }
 
-// Splat the points of the bins overlapping base cells [cy0-1, cy1] x [cx0-1, cx1] into a shared patch
-// covering cells [cy0, cy1] x [cx0, cx1] (row pitch `pitch`), depth-major.
-// zlo / zhi [ncol] (initialised to V / -1 by the caller): occupied depth range of every column — cells outside it are
-// exactly zero, so their blur, clamp and ray-march terms are constants (the sparsity skip of the fwd / bwd kernels).
-__device__ __forceinline__ void splat_bins(const float4* __restrict__ sorted, const int32_t* __restrict__ bs,
-                                           int nbx, int nby, int cy0, int cy1, int cx0, int cx1, int pitch,
-                                           int ncol, int mode, float* A, int* zlo, int* zhi) {
-    const int by_lo = max(cy0 - 1, 0) / BIN_Y, by_hi = min(cy1 / BIN_Y, nby - 1);
-    const int bx_lo = max(cx0 - 1, 0) / BIN_X, bx_hi = min(cx1 / BIN_X, nbx - 1);
+// fn(record) for every record of bins [bx_lo, bx_hi] x [by_lo, by_hi], all threads of the CTA taking part
+template <typename F>
+__device__ __forceinline__ void for_each_record(const float4* __restrict__ sorted, const int32_t* __restrict__ bs, int nbx,
+                                                int by_lo, int by_hi, int bx_lo, int bx_hi, F fn) {
     for (int by = by_lo; by <= by_hi; ++by) {
         const int lo = bs[by * nbx + bx_lo], hi = bs[by * nbx + bx_hi + 1];
-        for (int n = lo + threadIdx.x; n < hi; n += TILE_THREADS)
-            splat_record(__ldg(sorted + n), cy0, cy1, cx0, cx1, pitch, ncol, mode, A, zlo, zhi);
-    }
-}
-
-// ----------------------------------------------------------------------------------------------
-// TMA staging of the bin records (B3D_PC_TMA).  After the counting sort the records of the bins [bx_lo, bx_hi] of one bin
-// row are contiguous, so the records a patch needs are a handful of contiguous runs: one elected thread streams them into
-// a two-stage shared-memory ring with cp.async.bulk (the TMA's 1-D bulk copy, completion counted in bytes on an mbarrier)
-// and the CTA consumes them from shared memory.  The first two stages are issued BEFORE the patch is zero-filled, so the
-// global-memory latency of the records hides behind the 64-190 KB of shared-memory stores instead of following them.
-// ----------------------------------------------------------------------------------------------
-constexpr int STG_REC = 512;       // records per stage (8 KB): one per thread
-constexpr int STG_N = 2;
-constexpr size_t STG_BYTES = (size_t)STG_N * STG_REC * sizeof(float4);
-
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    // bounded: a byte count that never completes (a bug, or a fault of the copy) traps instead of hanging the GPU
-    for (uint32_t tries = 0; tries < (1u << 22); ++tries) {
-        uint32_t done;
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n"
-            "}\n"
-            : "=r"(done)
-            : "r"(smem_addr(bar)), "r"(parity)
-            : "memory");
-        if (done) return;
-    }
-    __trap();
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_addr(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_addr(bar))
-                 : "memory");
-}
-
-// Records [c0, c1) of the sequence "bins [bx_lo, bx_hi] of bin row by_lo, then of by_lo + 1, ... by_hi" as contiguous runs of
-// the sorted array: f(offset inside the chunk, first record, count) per run.  Host + device: b3d_pc_stream_plan exposes it
-// to the CPU tests.
-template <typename F>
-__host__ __device__ __forceinline__ void chunk_runs(const int32_t* bs, int nbx, int by_lo, int by_hi, int bx_lo, int bx_hi, int c0,
-                                                    int c1, F f) {
-    int pos = 0;
-    for (int by = by_lo; by <= by_hi && pos < c1; ++by) {
-        const int lo = bs[by * nbx + bx_lo], n = bs[by * nbx + bx_hi + 1] - lo;
-        const int a = c0 > pos ? c0 : pos, e = c1 < pos + n ? c1 : pos + n;
-        if (a < e) f(a - c0, lo + (a - pos), e - a);
-        pos += n;
-    }
-}
-
-// The records of bins [bx_lo, bx_hi] of bin rows [by_lo, by_hi], as one sequence cut into chunks of STG_REC.
-struct BinStream {
-    const float4* sp;
-    const int32_t* bs;
-    float4* stg;          // [STG_N][STG_REC]
-    uint64_t* bars;       // [STG_N]
-    int nbx, by_lo, by_hi, bx_lo, bx_hi, total, nchunks;
-
-    __device__ __forceinline__ void open(const float4* sp_, const int32_t* bs_, float4* stg_, uint64_t* bars_, int nbx_, int by_lo_,
-                                         int by_hi_, int bx_lo_, int bx_hi_) {
-        sp = sp_; bs = bs_; stg = stg_; bars = bars_; nbx = nbx_;
-        by_lo = by_lo_; by_hi = by_hi_; bx_lo = bx_lo_; bx_hi = bx_hi_;
-        total = 0;
-        for (int by = by_lo; by <= by_hi; ++by) total += bs[by * nbx + bx_hi + 1] - bs[by * nbx + bx_lo];
-        nchunks = (total + STG_REC - 1) / STG_REC;
-    }
-    __device__ __forceinline__ int count(int c) const { return min(STG_REC, total - c * STG_REC); }
-    // one thread: bulk copies of chunk c into stage c % STG_N (one copy per bin row the chunk intersects)
-    __device__ __forceinline__ void issue(int c) const {
-        const int c0 = c * STG_REC, c1 = min(c0 + STG_REC, total);
-        uint64_t* bar = bars + (c % STG_N);
-        float4* dst = stg + (c % STG_N) * STG_REC;
-        mbar_expect_tx(bar, (uint32_t)(c1 - c0) * (uint32_t)sizeof(float4));
-        const float4* src = sp;
-        chunk_runs(bs, nbx, by_lo, by_hi, bx_lo, bx_hi, c0, c1, [=](int off, int first, int cnt) {
-            bulk_g2s(dst + off, src + first, (uint32_t)cnt * (uint32_t)sizeof(float4), bar);
-        });
-    }
-    __device__ __forceinline__ void prefetch() const {       // one thread: fill the ring
-        for (int c = 0; c < nchunks && c < STG_N; ++c) issue(c);
-    }
-};
-
-// Consume a prefetched BinStream: fn(record) for every record, all threads of the CTA taking part.  `parity` carries the
-// mbarrier phase bits of the stages from one stream to the next (bit s = the phase the next wait on stage s expects).
-template <typename F>
-__device__ __forceinline__ void stream_consume(const BinStream& st, uint32_t& parity, F fn) {
-    for (int c = 0; c < st.nchunks; ++c) {
-        const int s = c % STG_N;
-        mbar_wait(st.bars + s, (parity >> s) & 1u);
-        parity ^= 1u << s;
-        const int cnt = st.count(c);
-        for (int i = threadIdx.x; i < cnt; i += TILE_THREADS) fn(st.stg[s * STG_REC + i]);
-        __syncthreads();                                     // every thread is done with stage s before it is refilled
-        if (threadIdx.x == 0 && c + STG_N < st.nchunks) st.issue(c + STG_N);
+        for (int n = lo + threadIdx.x; n < hi; n += TILE_THREADS) fn(__ldg(sorted + n));
     }
 }
 
@@ -400,16 +292,15 @@ __device__ __forceinline__ void clamp_patch(float* A, int n) {
 // occupancies and reduces it to (transmittance of the block, silhouette gathered inside the block);
 // a second, short pass chains the blocks of each column.
 // ----------------------------------------------------------------------------------------------
-template <int KT, bool TMA>
+template <int KT>
 __global__ void __launch_bounds__(TILE_THREADS)
 pc_sil_fwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__ bin_start, const Taps taps,
                   const float* __restrict__ scale, int N, int V, int TY, int mode, int nbx, int nby,
                   float* __restrict__ sil) {
     extern __shared__ __align__(128) float sm[];
-    __shared__ __align__(8) uint64_t bars[STG_N];
     const int b = blockIdx.z, ty0 = blockIdx.y * TY, tx0 = blockIdx.x * TX;
     const int ncol = TY * TX, nzb = (V + ZB - 1) / ZB;
-    float* A = sm + (TMA ? STG_BYTES / sizeof(float) : 0);   // [V][ncol] (behind the record ring when staging with TMA)
+    float* A = sm;                       // [V][ncol]
     float* blkP = A + V * ncol;          // [nzb][ncol] transmittance of the block
     float* blkS = blkP + nzb * ncol;     // [nzb][ncol] silhouette collected inside the block
     int* zlo = reinterpret_cast<int*>(blkS + nzb * ncol);    // [ncol] first / last occupied depth of the column
@@ -418,25 +309,13 @@ pc_sil_fwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__
     const int cy1 = min(ty0 + TY, V) - 1, cx1 = min(tx0 + TX, V) - 1;
     const float4* sp = sorted + (size_t)b * N;
     const int32_t* bs = bin_start + (size_t)b * (nbx * nby + 1);
-    BinStream st;
-    uint32_t parity = 0;
-    if (TMA) {
-        st.open(sp, bs, reinterpret_cast<float4*>(sm), bars, nbx, max(ty0 - 1, 0) / BIN_Y, min(cy1 / BIN_Y, nby - 1),
-                max(tx0 - 1, 0) / BIN_X, min(cx1 / BIN_X, nbx - 1));
-        if (tid == 0) {                  // the records are on their way while the CTA zero-fills the patch
-            for (int s = 0; s < STG_N; ++s) mbar_init(bars + s, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // the barriers as the bulk copies' async proxy sees them
-            st.prefetch();
-        }
-    }
     for (int i = tid; i < V * ncol; i += TILE_THREADS) A[i] = 0.f;
     for (int i = tid; i < ncol; i += TILE_THREADS) { zlo[i] = V; zhi[i] = -1; }
     __syncthreads();
-    if (TMA)
-        stream_consume(st, parity, [&](const float4 g) { splat_record(g, ty0, cy1, tx0, cx1, TX, ncol, mode, A, zlo, zhi); });
-    else
-        splat_bins(sp, bs, nbx, nby, ty0, cy1, tx0, cx1, TX, ncol, mode, A, zlo, zhi);
+    // the points of the bins overlapping base cells [ty0-1, cy1] x [tx0-1, cx1]
+    for_each_record(sp, bs, nbx, max(ty0 - 1, 0) / BIN_Y, min(cy1 / BIN_Y, nby - 1), max(tx0 - 1, 0) / BIN_X,
+                    min(cx1 / BIN_X, nbx - 1),
+                    [&](const float4 g) { splat_record(g, ty0, cy1, tx0, cx1, TX, ncol, mode, A, zlo, zhi); });
     __syncthreads();
     clamp_patch(A, V * ncol);
     __syncthreads();
@@ -486,18 +365,17 @@ pc_sil_fwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__
 // ----------------------------------------------------------------------------------------------
 // backward (patch with a +1 halo so that every point is owned by exactly one CTA)
 // ----------------------------------------------------------------------------------------------
-template <int KT, bool TMA>
+template <int KT>
 __global__ void __launch_bounds__(TILE_THREADS)
 pc_sil_bwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__ bin_start, const Taps taps,
                   const float* __restrict__ scale, const float* __restrict__ dsil, int N, int V, int TY, int mode,
                   int nbx, int nby, float4* __restrict__ dpg, float* __restrict__ dscale) {
     extern __shared__ __align__(128) float sm[];
     __shared__ float red[32];
-    __shared__ __align__(8) uint64_t bars[STG_N];
     const int b = blockIdx.z, ty0 = blockIdx.y * TY, tx0 = blockIdx.x * TX;
     const int cy1 = min(ty0 + TY, V - 1), cx1 = min(tx0 + TX, V - 1);     // extended patch, clipped to the grid
     const int EX = TX + 1, ncol = (TY + 1) * EX, nzb = (V + ZB - 1) / ZB;
-    float* A1 = sm + (TMA ? STG_BYTES / sizeof(float) : 0);   // clamped occupancy (sign = clamp mask) -> dG
+    float* A1 = sm;                      // clamped occupancy (sign = clamp mask) -> dG
     float* A2 = A1 + V * ncol;           // blurred S -> dS
     float* blkA = A2 + V * ncol;         // [nzb][ncol] transmittance of the block
     float* blkB = blkA + nzb * ncol;     // [nzb][ncol] offset of the block's Q recurrence -> Q just after the block
@@ -507,34 +385,16 @@ pc_sil_bwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__
     const int tid = threadIdx.x;
     const float4* sp = sorted + (size_t)b * N;
     const int32_t* bs = bin_start + (size_t)b * (nbx * nby + 1);
-    BinStream st;
-    uint32_t parity = 0;
-    if (TMA) {
-        st.open(sp, bs, reinterpret_cast<float4*>(sm), bars, nbx, max(ty0 - 1, 0) / BIN_Y, min(cy1 / BIN_Y, nby - 1),
-                max(tx0 - 1, 0) / BIN_X, min(cx1 / BIN_X, nbx - 1));
-        if (tid == 0) {                  // the records are on their way while the CTA zero-fills the patch
-            for (int s = 0; s < STG_N; ++s) mbar_init(bars + s, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // the barriers as the bulk copies' async proxy sees them
-            st.prefetch();
-        }
-    }
     for (int i = tid; i < V * ncol; i += TILE_THREADS) A1[i] = 0.f;
     for (int i = tid; i < ncol; i += TILE_THREADS) { zlo[i] = V; zhi[i] = -1; }
     __syncthreads();
-    if (TMA)
-        stream_consume(st, parity, [&](const float4 g) { splat_record(g, ty0, cy1, tx0, cx1, EX, ncol, mode, A1, zlo, zhi); });
-    else
-        splat_bins(sp, bs, nbx, nby, ty0, cy1, tx0, cx1, EX, ncol, mode, A1, zlo, zhi);
+    for_each_record(sp, bs, nbx, max(ty0 - 1, 0) / BIN_Y, min(cy1 / BIN_Y, nby - 1), max(tx0 - 1, 0) / BIN_X,
+                    min(cx1 / BIN_X, nbx - 1),
+                    [&](const float4 g) { splat_record(g, ty0, cy1, tx0, cx1, EX, ncol, mode, A1, zlo, zhi); });
     __syncthreads();
-    // the records of the OWNED bins (the gather at the end of the kernel) stream in under the four passes below
-    const int oy1 = min(ty0 + TY, V) - 1, ox1 = min(tx0 + TX, V) - 1;   // owned base cells
+    const int oy1 = min(ty0 + TY, V) - 1, ox1 = min(tx0 + TX, V) - 1;   // owned base cells (the gather at the end)
     const int gby_lo = ty0 / BIN_Y, gby_hi = min(oy1 / BIN_Y, nby - 1);
     const int gbx_lo = tx0 / BIN_X, gbx_hi = min(ox1 / BIN_X, nbx - 1);
-    if (TMA) {
-        st.open(sp, bs, reinterpret_cast<float4*>(sm), bars, nbx, gby_lo, gby_hi, gbx_lo, gbx_hi);
-        if (tid == 0) st.prefetch();
-    }
     clamp_patch(A1, V * ncol);
     __syncthreads();
 
@@ -669,14 +529,7 @@ pc_sil_bwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__
                 }
         dp[__float_as_int(g.w)] = make_float4(dz, dy, dx, 0.f);
     };
-    if (TMA) {
-        stream_consume(st, parity, gather);
-    } else {
-        for (int by = gby_lo; by <= gby_hi; ++by) {
-            const int lo = bs[by * nbx + gbx_lo], hi = bs[by * nbx + gbx_hi + 1];
-            for (int n = lo + tid; n < hi; n += TILE_THREADS) gather(__ldg(sp + n));
-        }
-    }
+    for_each_record(sp, bs, nbx, gby_lo, gby_hi, gbx_lo, gbx_hi, gather);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -766,7 +619,7 @@ __global__ void __launch_bounds__(NTHREADS) clamp01_kernel(float* __restrict__ x
 // ----------------------------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------------------------
-constexpr size_t SMEM_BUDGET = 210 * 1024;      // the patch; + 16 KB record ring (B3D_PC_TMA) + static barriers <= 227 KB
+constexpr size_t SMEM_BUDGET = 210 * 1024;      // the patch, within the 227 KB a CTA may use
 
 size_t patch_bytes(int V, int ty, bool bwd) {
     const size_t nzb = (V + ZB - 1) / ZB;
@@ -779,24 +632,9 @@ size_t patch_bytes(int V, int ty, bool bwd) {
 }
 
 int pick_ty(int V, bool bwd) {
-    if (const char* e = getenv(bwd ? "B3D_PC_TY_BWD" : "B3D_PC_TY_FWD")) {
-        const int v = atoi(e);
-        if (v >= 1 && v <= 64 && patch_bytes(V, v, bwd) <= SMEM_BUDGET) return v;
-    }
     for (int ty = 16; ty >= 1; ty >>= 1)
         if (patch_bytes(V, ty, bwd) <= SMEM_BUDGET) return ty;
     return 0;
-}
-
-int load_taps(const float* taps_dev, int ktaps, Taps& t, cudaStream_t st) {
-    // taps in device memory: 21 floats read back on the caller's stream (the hosttaps entry avoids this)
-    B3D_CUDA_OK(cudaMemcpyAsync(t.w, taps_dev, sizeof(float) * ktaps, cudaMemcpyDeviceToHost, st));
-    B3D_CUDA_OK(cudaStreamSynchronize(st));
-    t.n = ktaps;
-    t.finite = 1;
-    for (int i = 0; i < ktaps; ++i)
-        if (!(fabsf(t.w[i]) <= 3.0e38f)) t.finite = 0;
-    return B3D_OK;
 }
 
 inline int bins_x(int V) { return (V + BIN_X - 1) / BIN_X; }
@@ -808,19 +646,12 @@ int set_smem(K kernel, size_t bytes) {
     return B3D_OK;
 }
 
-// B3D_PC_TMA=0/1: stage the bin records through shared memory with cp.async.bulk (default: see pc_tma_default)
-constexpr int pc_tma_default = 0;
-bool pc_tma() {
-    static const int v = getenv("B3D_PC_TMA") ? atoi(getenv("B3D_PC_TMA")) : pc_tma_default;
-    return v != 0;
-}
-
-template <int KT, bool TMA>
+template <int KT>
 int launch_sil_fwd(dim3 grid, size_t smem, cudaStream_t st, const float* sorted, const int32_t* bin_start, const Taps& t,
                    const float* scale, int N, int V, int TY, int mode, float* sil) {
-    if (int rc = set_smem(pc_sil_fwd_kernel<KT, TMA>, smem)) return rc;
-    pc_sil_fwd_kernel<KT, TMA><<<grid, TILE_THREADS, smem, st>>>((const float4*)sorted, bin_start, t, scale, N, V, TY, mode,
-                                                                 bins_x(V), bins_y(V), sil);
+    if (int rc = set_smem(pc_sil_fwd_kernel<KT>, smem)) return rc;
+    pc_sil_fwd_kernel<KT><<<grid, TILE_THREADS, smem, st>>>((const float4*)sorted, bin_start, t, scale, N, V, TY, mode,
+                                                            bins_x(V), bins_y(V), sil);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }
@@ -829,23 +660,18 @@ int sil_fwd_impl(const float* sorted, const int32_t* bin_start, const Taps& t, c
                  int V, int mode, float* sil, cudaStream_t st) {
     const int TY = pick_ty(V, false);
     B3D_REQUIRE(TY > 0, B3D_EINVAL, "b3d_pc_silhouette_fwd: V=%d does not fit the shared-memory patch", V);
-    const bool tma = pc_tma();
-    const size_t smem = patch_bytes(V, TY, false) + (tma ? STG_BYTES : 0);
-    if (tma) B3D_CHECK_ALIGNED(sorted);
+    const size_t smem = patch_bytes(V, TY, false);
     dim3 grid(b3d::ceil_div(V, TX), b3d::ceil_div(V, TY), B);
-    if (t.n == 21)
-        return tma ? launch_sil_fwd<21, true>(grid, smem, st, sorted, bin_start, t, scale, N, V, TY, mode, sil)
-                   : launch_sil_fwd<21, false>(grid, smem, st, sorted, bin_start, t, scale, N, V, TY, mode, sil);
-    return tma ? launch_sil_fwd<0, true>(grid, smem, st, sorted, bin_start, t, scale, N, V, TY, mode, sil)
-               : launch_sil_fwd<0, false>(grid, smem, st, sorted, bin_start, t, scale, N, V, TY, mode, sil);
+    if (t.n == 21) return launch_sil_fwd<21>(grid, smem, st, sorted, bin_start, t, scale, N, V, TY, mode, sil);
+    return launch_sil_fwd<0>(grid, smem, st, sorted, bin_start, t, scale, N, V, TY, mode, sil);
 }
 
-template <int KT, bool TMA>
+template <int KT>
 int launch_sil_bwd(dim3 grid, size_t smem, cudaStream_t st, const float* sorted, const int32_t* bin_start, const Taps& t,
                    const float* scale, const float* dsil, int N, int V, int TY, int mode, float* dpg, float* dscale) {
-    if (int rc = set_smem(pc_sil_bwd_kernel<KT, TMA>, smem)) return rc;
-    pc_sil_bwd_kernel<KT, TMA><<<grid, TILE_THREADS, smem, st>>>((const float4*)sorted, bin_start, t, scale, dsil, N, V, TY, mode,
-                                                                 bins_x(V), bins_y(V), (float4*)dpg, dscale);
+    if (int rc = set_smem(pc_sil_bwd_kernel<KT>, smem)) return rc;
+    pc_sil_bwd_kernel<KT><<<grid, TILE_THREADS, smem, st>>>((const float4*)sorted, bin_start, t, scale, dsil, N, V, TY, mode,
+                                                            bins_x(V), bins_y(V), (float4*)dpg, dscale);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }
@@ -854,16 +680,11 @@ int sil_bwd_impl(const float* sorted, const int32_t* bin_start, const Taps& t, c
                  const float* dsil, int B, int N, int V, int mode, float* dpg, float* dscale, cudaStream_t st) {
     const int TY = pick_ty(V, true);
     B3D_REQUIRE(TY > 0, B3D_EINVAL, "b3d_pc_silhouette_bwd: V=%d does not fit the shared-memory patch", V);
-    const bool tma = pc_tma();
-    const size_t smem = patch_bytes(V, TY, true) + (tma ? STG_BYTES : 0);
-    if (tma) B3D_CHECK_ALIGNED(sorted);
+    const size_t smem = patch_bytes(V, TY, true);
     if (dscale) B3D_CUDA_OK(cudaMemsetAsync(dscale, 0, sizeof(float) * B, st));
     dim3 grid(b3d::ceil_div(V, TX), b3d::ceil_div(V, TY), B);
-    if (t.n == 21)
-        return tma ? launch_sil_bwd<21, true>(grid, smem, st, sorted, bin_start, t, scale, dsil, N, V, TY, mode, dpg, dscale)
-                   : launch_sil_bwd<21, false>(grid, smem, st, sorted, bin_start, t, scale, dsil, N, V, TY, mode, dpg, dscale);
-    return tma ? launch_sil_bwd<0, true>(grid, smem, st, sorted, bin_start, t, scale, dsil, N, V, TY, mode, dpg, dscale)
-               : launch_sil_bwd<0, false>(grid, smem, st, sorted, bin_start, t, scale, dsil, N, V, TY, mode, dpg, dscale);
+    if (t.n == 21) return launch_sil_bwd<21>(grid, smem, st, sorted, bin_start, t, scale, dsil, N, V, TY, mode, dpg, dscale);
+    return launch_sil_bwd<0>(grid, smem, st, sorted, bin_start, t, scale, dsil, N, V, TY, mode, dpg, dscale);
 }
 
 int check_sil_args(const char* who, const void* sorted, const void* bin_start, const void* taps, int ktaps, int B,
@@ -891,25 +712,6 @@ void fill_taps(Taps& t, const float* host, int n) {
 extern "C" {
 
 int b3d_pc_bin_count(int V) { return V >= 2 ? bins_x(V) * bins_y(V) : 0; }
-
-int b3d_pc_tma_staging(void) { return pc_tma() ? 1 : 0; }
-
-int b3d_pc_stage_records(void) { return STG_REC; }
-
-int b3d_pc_stream_plan(const int32_t* bin_start_host, int nbx, int by_lo, int by_hi, int bx_lo, int bx_hi, int chunk, int* dst_off,
-                       int* src_first, int* count, int cap) {
-    B3D_REQUIRE(bin_start_host && nbx > 0 && by_lo >= 0 && by_hi >= by_lo && bx_lo >= 0 && bx_hi >= bx_lo && bx_hi < nbx && chunk >= 0 &&
-                    (cap == 0 || (dst_off && src_first && count)), B3D_EINVAL, "b3d_pc_stream_plan: bad arguments");
-    int total = 0;
-    for (int by = by_lo; by <= by_hi; ++by) total += bin_start_host[by * nbx + bx_hi + 1] - bin_start_host[by * nbx + bx_lo];
-    const int c0 = chunk * STG_REC, c1 = c0 + STG_REC < total ? c0 + STG_REC : total;
-    int runs = 0;
-    chunk_runs(bin_start_host, nbx, by_lo, by_hi, bx_lo, bx_hi, c0, c1, [&](int off, int first, int cnt) {
-        if (runs < cap) { dst_off[runs] = off; src_first[runs] = first; count[runs] = cnt; }
-        ++runs;
-    });
-    return runs;
-}
 
 int b3d_pc_project(const float* points, const float* quat, int B, int N, int V, float fov, float cam_dist,
                    float* pg, float* coords, int32_t* base, uint8_t* inb, float* sorted, int32_t* bin_start,
@@ -944,7 +746,7 @@ size_t b3d_pc_silhouette_workspace_bytes(int B, int V, int mode) {
 }
 
 // taps given in HOST memory (the Python wrapper computes them with the reference's torch expression on
-// the CPU, 21 floats): avoids the device->host sync of the device-taps entry points.
+// the CPU, 21 floats) and passed to the kernel by value, so no device->host read is needed.
 int b3d_pc_silhouette_fwd_hosttaps(const float* sorted, const int32_t* bin_start, const float* taps_host, int ktaps,
                                    const float* scale, int B, int N, int V, int mode, float* sil, void* workspace,
                                    size_t workspace_bytes, void* stream) {
@@ -955,19 +757,6 @@ int b3d_pc_silhouette_fwd_hosttaps(const float* sorted, const int32_t* bin_start
     B3D_REQUIRE(sil, B3D_EINVAL, "b3d_pc_silhouette_fwd: null output");
     Taps t;
     fill_taps(t, taps_host, ktaps);
-    return sil_fwd_impl(sorted, bin_start, t, scale, B, N, V, mode, sil, (cudaStream_t)stream);
-}
-
-int b3d_pc_silhouette_fwd(const float* sorted, const int32_t* bin_start, const float* taps, int ktaps,
-                          const float* scale, int B, int N, int V, int mode, float* sil, void* workspace,
-                          size_t workspace_bytes, void* stream) {
-    (void)workspace;
-    (void)workspace_bytes;
-    if (int rc = check_sil_args("b3d_pc_silhouette_fwd", sorted, bin_start, taps, ktaps, B, N, V, mode)) return rc;
-    if (B == 0) return B3D_OK;
-    B3D_REQUIRE(sil, B3D_EINVAL, "b3d_pc_silhouette_fwd: null output");
-    Taps t;
-    if (int rc = load_taps(taps, ktaps, t, (cudaStream_t)stream)) return rc;
     return sil_fwd_impl(sorted, bin_start, t, scale, B, N, V, mode, sil, (cudaStream_t)stream);
 }
 
@@ -983,21 +772,6 @@ int b3d_pc_silhouette_bwd_hosttaps(const float* sorted, const int32_t* bin_start
                 "b3d_pc_silhouette_bwd: scale and dscale must both be given or both be NULL");
     Taps t;
     fill_taps(t, taps_host, ktaps);
-    return sil_bwd_impl(sorted, bin_start, t, scale, dsil, B, N, V, mode, dpg, dscale, (cudaStream_t)stream);
-}
-
-int b3d_pc_silhouette_bwd(const float* sorted, const int32_t* bin_start, const float* taps, int ktaps,
-                          const float* scale, const float* dsil, int B, int N, int V, int mode, float* dpg,
-                          float* dscale, void* workspace, size_t workspace_bytes, void* stream) {
-    (void)workspace;
-    (void)workspace_bytes;
-    if (int rc = check_sil_args("b3d_pc_silhouette_bwd", sorted, bin_start, taps, ktaps, B, N, V, mode)) return rc;
-    if (B == 0) return B3D_OK;
-    B3D_REQUIRE(dsil && (dpg || N == 0), B3D_EINVAL, "b3d_pc_silhouette_bwd: null pointer");
-    B3D_REQUIRE((scale == nullptr) == (dscale == nullptr), B3D_EINVAL,
-                "b3d_pc_silhouette_bwd: scale and dscale must both be given or both be NULL");
-    Taps t;
-    if (int rc = load_taps(taps, ktaps, t, (cudaStream_t)stream)) return rc;
     return sil_bwd_impl(sorted, bin_start, t, scale, dsil, B, N, V, mode, dpg, dscale, (cudaStream_t)stream);
 }
 

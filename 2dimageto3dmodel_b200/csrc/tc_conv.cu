@@ -217,19 +217,6 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     }
 }
 
-// [taps][K][N] -> [taps][N][K]: the input gradient's weights arrive cin-major (N-major B operand), wgmma reads tf32 K-major
-__global__ void transpose_taps_kernel(const float* __restrict__ in, float* __restrict__ out, int K, int N) {
-    __shared__ float t[32][33];
-    const int tap = blockIdx.z, k0 = blockIdx.y * 32, n0 = blockIdx.x * 32;
-    const float* src = in + (size_t)tap * K * N;
-    float* dst = out + (size_t)tap * K * N;
-    for (int i = threadIdx.y; i < 32; i += blockDim.y)
-        if (k0 + i < K && n0 + (int)threadIdx.x < N) t[i][threadIdx.x] = src[(size_t)(k0 + i) * N + n0 + threadIdx.x];
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y)
-        if (n0 + i < N && k0 + (int)threadIdx.x < K) dst[(size_t)(n0 + i) * K + k0 + threadIdx.x] = t[threadIdx.x][i];
-}
-
 // ----------------------------------------------------------------------------------------------
 // wgrad:  dW[co, ci, r, s] += sum_{n,y,x} dY[n, y, x, co] * X[n, st*y + r - pad_y, st*x + s, ci]      (NHWC operands)
 // GEMM with M = Cout (128), N = Cin (BN), K = output pixels.  In NHWC the reduction index (pixel) is the SLOW index
@@ -467,11 +454,11 @@ int pow2_floor(int v) {
 extern "C" {
 
 // x   [N, H, W, Cin]  NHWC fp32, Cin % 32 == 0
-// wt  [ntaps, Cout, Cin] fp32 (tap-major, K-major rows); w_cin_major: [ntaps, Cin, Cout]
+// wt  [ntaps, Cout, Cin] fp32 (tap-major, K-major rows)
 // out [N, OH, OW, OC]; the tile grid covers (Hout, Wout) logical outputs, written to (osy*y+ooy, osx*x+oox)
 int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* out, int N, int H, int W, int Cin,
                     int Hout, int Wout, int Cout, int ntaps, const int* dy, const int* dx, int sy, int sx, int OH,
-                    int OW, int OC, int osy, int osx, int ooy, int oox, float leaky, int w_cin_major, const int* wtap,
+                    int OW, int OC, int osy, int osx, int ooy, int oox, float leaky, const int* wtap,
                     int wtaps_total, double* stats, int fold_kh, int fold_pad, const b3d_conv_opts* opts, void* stream) {
     B3D_REQUIRE(N > 0 && H > 0 && W > 0 && Hout > 0 && Wout > 0 && Cout > 0, B3D_EINVAL, "b3d_conv2d_tf32: bad sizes");
     B3D_REQUIRE(Cin > 0 && Cin % BK == 0, B3D_EINVAL, "b3d_conv2d_tf32: Cin=%d must be a multiple of %d", Cin, BK);
@@ -501,7 +488,7 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
     if (fold_kh > 0) {
         // x is the RAW stem input [N, H, W, 8]; the convolution is kh x kw with the kh rows folded into the K dimension:
         // Cin = 32 * ceil(8 kh / 32) "channels", taps = the kw horizontal ones (dy ignored), zero rows = the y padding
-        B3D_REQUIRE(fold_kh <= 8 && Cin == 32 * ((8 * fold_kh + 31) / 32) && sy == 1 && sx == 1 && !w_cin_major && !wtap && Wout % BM == 0,
+        B3D_REQUIRE(fold_kh <= 8 && Cin == 32 * ((8 * fold_kh + 31) / 32) && sy == 1 && sx == 1 && !wtap && Wout % BM == 0,
                     B3D_EINVAL, "b3d_conv2d_tf32: on-the-fly fold needs 8 input channels, stride 1 and Wout %% 128 == 0 (Wout=%d)", Wout);
     }
     B3D_REQUIRE(!stats || mask || (osy == 1 && osx == 1), B3D_EINVAL, "b3d_conv2d_tf32: statistics need a dense output");
@@ -510,30 +497,12 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
     const bool bn256 = Cout % 256 == 0 && (long long)N * Hout * Wout / BM * (Cout / 256) * ncls >= tc::num_sms();
     const int BN = bn256 ? 256 : Cout > 64 ? 128 : 64;
     cudaStream_t st = (cudaStream_t)stream;
-    // wgmma reads tf32 operands K-major only: cin-major weights (the input gradient's, [ntaps, Cin, Cout]) are transposed
-    // once per call into a stream-ordered temporary
-    float* wk = nullptr;
-    if (w_cin_major) {
-        B3D_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&wk), (size_t)wtaps_total * Cin * Cout * sizeof(float), st));
-        transpose_taps_kernel<<<dim3(b3d::ceil_div(Cout, 32), b3d::ceil_div(Cin, 32), wtaps_total), dim3(32, 8), 0, st>>>(wt, wk, Cin, Cout);
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) {
-            cudaFreeAsync(wk, st);
-            b3d::set_error("b3d_conv2d_tf32: weight transpose launch failed: %s", cudaGetErrorString(e));
-            return B3D_ECUDA;
-        }
-        b3d::count_launch();
-    }
-    const float* wkm = w_cin_major ? wk : wt;
     CUtensorMap mw;
     {
         const uint64_t dims[3] = {(uint64_t)Cin, (uint64_t)Cout, (uint64_t)wtaps_total};
         const uint64_t strides[2] = {(uint64_t)Cin * 4, (uint64_t)Cout * Cin * 4};
         const uint32_t box[3] = {(uint32_t)BK, (uint32_t)BN, 1};
-        if (int rc = tc::make_tmap_f32(&mw, wkm, 3, dims, strides, box)) {
-            if (wk) cudaFreeAsync(wk, st);
-            return rc;
-        }
+        if (int rc = tc::make_tmap_f32(&mw, wt, 3, dims, strides, box)) return rc;
     }
 
     // Filter-grid detection for the row window (stride 1, no fold): every class has kh rows of kw in {2, 3, 5} horizontally
@@ -591,7 +560,7 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
             const uint64_t wstrides[2] = {(uint64_t)Cin * 4, (uint64_t)Cout * Cin * 4};
             const uint32_t wbox[3] = {(uint32_t)BK, (uint32_t)BN, (uint32_t)((g_kw - 1) * g_wstep + 1)};
             const uint32_t wes[3] = {1, 1, (uint32_t)g_wstep};
-            if (int rc = tc::make_tmap_f32(&mwr, wkm, 3, wdims, wstrides, wbox, wes)) return rc;
+            if (int rc = tc::make_tmap_f32(&mwr, wt, 3, wdims, wstrides, wbox, wes)) return rc;
             return BN == 128 ? launch_rowwin<128>(g_kw, mx, mwr, p, bias, out, tiles, st) : launch_rowwin<64>(g_kw, mx, mwr, p, bias, out, tiles, st);
         }
         if (fold_kh > 0) {
@@ -614,25 +583,11 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
     };
     const int bw_full = pow2_floor(Wout < BM ? Wout : BM);
     const int rem = Wout % bw_full;
-    int rc;
     if (rem != 0 && rem * 8 <= bw_full && Wout > bw_full) {
-        rc = run(0, Wout - rem);
-        if (rc == 0) rc = run(Wout - rem, Wout);
-    } else {
-        rc = run(0, Wout);
+        const int rc = run(0, Wout - rem);
+        return rc ? rc : run(Wout - rem, Wout);
     }
-    if (wk) cudaFreeAsync(wk, st);
-    return rc;
-}
-
-// Stride-1 convolution over an x-padded input of row pitch P (include/b3d.h): the same work as b3d_conv2d_tf32 with
-// unit strides and a dense output, which stages the row windows / tap tiles itself.
-int b3d_conv2d_flat_tf32(const float* x, const float* wt, const float* bias, float* out, int N, int H, int P, int Cin,
-                         int Hout, int Wout, int Cout, int ntaps, const int* dy, const int* dx, int OH, int OW, int OC,
-                         float leaky, void* stream) {
-    B3D_REQUIRE(Wout <= P, B3D_EINVAL, "b3d_conv2d_flat_tf32: Wout=%d exceeds the input pitch %d", Wout, P);
-    return b3d_conv2d_tf32(x, wt, bias, out, N, H, P, Cin, Hout, Wout, Cout, ntaps, dy, dx, 1, 1, OH, OW, OC, 1, 1, 0, 0, leaky, 0,
-                           nullptr, 0, nullptr, 0, 0, nullptr, stream);
+    return run(0, Wout);
 }
 
 // dy [N,Hout,Wout,Cout], x [N,H,W,Cin] NHWC (x already padded along x; Cin, Cout multiples of 32),

@@ -287,8 +287,8 @@ int launch_wgrad(const float* gy, const float* x, float* dw, const ThinGeom& g, 
     if (bpc > (rows + NT / 32 - 1) / (NT / 32)) bpc = (rows + NT / 32 - 1) / (NT / 32);
     const size_t smem = (size_t)COUT * KS * KS * 32 * VEC * 4;
     B3D_CUDA_OK(cudaFuncSetAttribute(conv_thin_wgrad_kernel<COUT, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    static const bool plain = getenv("B3D_THIN_NOWIN") != nullptr;
-    if (COUT * VEC <= 6 && !plain) {               // window (25 * VEC) + accumulators (COUT * 25 * VEC) fit the register file
+    constexpr bool win = COUT * VEC <= 6;          // window (25 * VEC) + accumulators (COUT * 25 * VEC) fit the register file
+    if (win) {
         B3D_CUDA_OK(cudaFuncSetAttribute(conv_thin_wgrad_win_kernel<COUT, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         conv_thin_wgrad_win_kernel<COUT, VEC><<<bpc * chunks, NT, smem, st>>>(gy, x, dw, g);
     } else {
@@ -296,7 +296,7 @@ int launch_wgrad(const float* gy, const float* x, float* dw, const ThinGeom& g, 
     }
     B3D_LAUNCH_OK();
     b3d::clear_variant();
-    b3d::add_variant(COUT * VEC <= 6 && !plain ? "conv_thin_wgrad_win<%d,%d>" : "conv_thin_wgrad<%d,%d>", COUT, VEC);
+    b3d::add_variant(win ? "conv_thin_wgrad_win<%d,%d>" : "conv_thin_wgrad<%d,%d>", COUT, VEC);
     return B3D_OK;
 }
 

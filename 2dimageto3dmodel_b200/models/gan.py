@@ -11,7 +11,6 @@ kernels read; x-padding (replicate for the symmetric generator, circular for the
 as in the reference, y-padding is the convolution's zero padding (TMA out-of-bounds fill).
 """
 import math
-import os
 
 import torch
 import torch.nn as nn
@@ -133,7 +132,7 @@ class _DiscriminatorBase(nn.Module):
     def _links(self, n, W):
         """ActLinks for the first n conv -> conv hand-overs of the stack (the last padded activation also feeds the
         projection, so it keeps the stand-alone backward pass)."""
-        on = bool(W) and self.circular and not getattr(self, 'disable_act_chain', False) and not os.environ.get("B3D_NO_ACT_CHAIN")
+        on = bool(W) and self.circular and not getattr(self, 'disable_act_chain', False)
         return [ActLink() if on else None for _ in range(n)]
 
     def _project(self, y, feat, c, caption):

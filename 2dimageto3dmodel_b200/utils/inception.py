@@ -274,7 +274,7 @@ class InceptionV3(nn.Module):
                 raise B3DError("inception: bad output slice")
         optr = ctypes.c_void_p(out.data_ptr() + 4 * coff)
         check(lib.b3d_conv2d_tf32(ptr(x), ptr(f.wt), ptr(f.bias), optr, N, H, W, C, Ho, Wo, cout, f.ntaps, f.dy, f.dx, f.stride, f.stride,
-                                  Ho, Wo, out.shape[3], 1, 1, 0, 0, 0.0, 0, None, 0, None, 0, 0, None, stream_ptr(x)))
+                                  Ho, Wo, out.shape[3], 1, 1, 0, 0, 0.0, None, 0, None, 0, 0, None, stream_ptr(x)))
         return out
 
     def _maxpool(self, x, out=None, coff=0):

@@ -10,8 +10,7 @@
  *   - plain pointers + sizes, no torch types; every pointer is DEVICE memory,
  *     contiguous, fp32 unless stated, base pointers 16-byte aligned;
  *   - the caller owns every buffer (inputs, outputs, workspaces); the library never
- *     allocates or frees persistent device memory (b3d_conv2d_tf32 with cin-major weights
- *     takes a stream-ordered temporary for their transpose and frees it on the same stream);
+ *     allocates or frees device memory;
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it, no
  *     internal synchronisation;
  *   - return 0 on success, a negative B3D_E* code otherwise; b3d_last_error()
@@ -46,7 +45,7 @@ extern "C" {
 B3D_API const char* b3d_last_error(void);
 B3D_API int b3d_version(void);
 /* ';'-joined names of the kernel template instances launched by the calling thread's most recent convolution
- * entry point (b3d_conv2d_tf32 / _flat_tf32 / _wgrad_tf32 / _thin_*), e.g. "conv_wgmma<256,4>":
+ * entry point (b3d_conv2d_tf32 / _wgrad_tf32 / _thin_*), e.g. "conv_wgmma<256,4>":
  * the parity tests assert WHICH variant they exercised, so dispatch drift cannot silently un-test a kernel. */
 B3D_API const char* b3d_last_variant(void);
 /* number of kernels this library has launched in the calling process (bench.py's gpu_launches) */
@@ -73,17 +72,6 @@ B3D_API uint64_t b3d_launch_count(void);
  * sorted    [B,N,4]  out, nullable: (gz,gy,gx, bits(point index)) of the in-bounds points, bin-sorted
  * bin_start [B, b3d_pc_bin_count(V)+1] out, int32 (with sorted): start of every bin in `sorted`      */
 B3D_API int b3d_pc_bin_count(int V);
-/* 1 when the silhouette kernels stage the bin records through shared memory with cp.async.bulk (the TMA's 1-D bulk copy,
- * mbarrier byte-count completion; the first stages are in flight while the patch is zero-filled), 0 when they read them with
- * plain loads.  Process-wide, read once: environment B3D_PC_TMA=0/1 overrides the built-in default. */
-B3D_API int b3d_pc_tma_staging(void);
-/* Host-only view of that staging (CPU tests): records per ring stage, and the contiguous runs of `sorted` that bulk copies
- * bring in for chunk `chunk` of the record sequence "bins [bx_lo, bx_hi] of bin rows by_lo .. by_hi" given one sample's
- * bin_start (HOST memory): run r copies count[r] records starting at record src_first[r] to offset dst_off[r] of the stage.
- * Returns the number of runs (the arrays hold the first `cap`), negative on bad arguments. */
-B3D_API int b3d_pc_stage_records(void);
-B3D_API int b3d_pc_stream_plan(const int32_t* bin_start_host, int nbx, int by_lo, int by_hi, int bx_lo, int bx_hi, int chunk,
-                               int* dst_off, int* src_first, int* count, int cap);
 B3D_API int b3d_pc_project(const float* points, const float* quat, int B, int N, int V, float fov,
                            float cam_dist, float* pg, float* coords, int32_t* base, uint8_t* inb,
                            float* sorted, int32_t* bin_start, void* stream);
@@ -96,12 +84,8 @@ B3D_API int b3d_pc_project(const float* points, const float* quat, int B, int N,
  * (sorted, bin_start) from b3d_pc_project; taps [ktaps] the 1-D smoothing kernel (the host computes it with
  * the reference's expression, smooth_voxels.py:24-31); scale [B] nullable; sil [B,V,V] out.
  * workspace: b3d_pc_silhouette_workspace_bytes(B,V,mode) bytes (0 for mode R; may be NULL then).
- * The *_hosttaps variants take the taps from HOST memory (no device->host read of 21 floats); they are what
- * the Python wrapper calls.                                                                           */
+ * The taps are read from HOST memory (no device->host read of 21 floats).                              */
 B3D_API size_t b3d_pc_silhouette_workspace_bytes(int B, int V, int mode);
-B3D_API int b3d_pc_silhouette_fwd(const float* sorted, const int32_t* bin_start, const float* taps, int ktaps,
-                                  const float* scale, int B, int N, int V, int mode, float* sil,
-                                  void* workspace, size_t workspace_bytes, void* stream);
 B3D_API int b3d_pc_silhouette_fwd_hosttaps(const float* sorted, const int32_t* bin_start,
                                            const float* taps_host, int ktaps, const float* scale, int B,
                                            int N, int V, int mode, float* sil, void* workspace,
@@ -109,10 +93,6 @@ B3D_API int b3d_pc_silhouette_fwd_hosttaps(const float* sorted, const int32_t* b
 
 /* Backward of the above: dsil [B,V,V] -> dpg [B,N,4] (d/d grid coords, indexed by ORIGINAL point index,
  * written for in-bounds points only; .w unused), dscale [B] (nullable iff scale is NULL; zeroed by the call). */
-B3D_API int b3d_pc_silhouette_bwd(const float* sorted, const int32_t* bin_start, const float* taps, int ktaps,
-                                  const float* scale, const float* dsil, int B, int N, int V, int mode,
-                                  float* dpg, float* dscale, void* workspace, size_t workspace_bytes,
-                                  void* stream);
 B3D_API int b3d_pc_silhouette_bwd_hosttaps(const float* sorted, const int32_t* bin_start,
                                            const float* taps_host, int ktaps, const float* scale,
                                            const float* dsil, int B, int N, int V, int mode, float* dpg,
@@ -237,7 +217,7 @@ B3D_API int b3d_chamfer_bwd(const float* query, const float* cand, const int32_t
  * as a wgmma / TMA implicit GEMM (tf32 inputs, fp32 accumulate — cuDNN's default TF32 class, SURVEY §2.2).
  *   out[n, osy*y+ooy, osx*x+oox, co] = leaky( bias[co] + sum_t sum_ci x[n, sy*y+dy[t], sx*x+dx[t], ci] * wt[t, co, ci] )
  * x [N,H,W,Cin] NHWC fp32 (Cin % 32 == 0; reads outside [0,H)x[0,W) are zero = the conv's zero padding),
- * wt [ntaps,Cout,Cin] (w_cin_major = 0) or [ntaps,Cin,Cout] (w_cin_major = 1: transposed to the K-major layout once per call, in a stream-ordered temporary),
+ * wt [ntaps,Cout,Cin] (tap-major),
  * bias [Cout] nullable, out [N,OH,OW,OC]; (y,x) run over [0,Hout)x[0,Wout).
  * fprop: dy = r - pad_y, dx = s.  dgrad: dy = pad_y - r, dx = -s with wt[t] = W[:,:,r,s]^T (strided dgrad = one
  * call per output parity class with osy = osx = 2).  leaky = negative slope of the fused LeakyReLU (1 = none).
@@ -269,7 +249,7 @@ typedef struct b3d_conv_opts {
 B3D_API int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* out, int N, int H, int W,
                             int Cin, int Hout, int Wout, int Cout, int ntaps, const int* dy, const int* dx,
                             int sy, int sx, int OH, int OW, int OC, int osy, int osx, int ooy, int oox,
-                            float leaky, int w_cin_major, const int* wtap, int wtaps_total, double* stats, int fold_kh,
+                            float leaky, const int* wtap, int wtaps_total, double* stats, int fold_kh,
                             int fold_pad, const b3d_conv_opts* opts, void* stream);
 /* wtap (nullable): loop tap t reads weight tap wtap[t] of a tap-major array that holds wtaps_total taps — the stride-2
  * input-gradient parity classes address their tap subsets of the full weight array without a gathered copy.
@@ -280,14 +260,6 @@ B3D_API int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, 
  * taps are folded into the K dimension ON THE FLY by the TMA boxes (four image rows x 8 channels = one 32-channel K slice, rows
  * outside the image = the zero padding fold_pad) — Cin is the folded channel count (32 * ceil(8 kh / 32)), the taps are the kw
  * horizontal ones, wt is the folded tap-major layout [kw][Cout][Cin] (b3d/bank.py `fold`).  Needs Wout % 128 == 0.            */
-
-/* Stride-1 convolution of an x-padded input x [N,H,P,Cin] (P = padded width = row pitch), taps (dy, dx >= 0); same
- * weights / bias / LeakyReLU semantics as b3d_conv2d_tf32, output out[n,y,x,co] for y < Hout, x < Wout of a tensor
- * [N,OH,OW,OC].  Runs b3d_conv2d_tf32 with unit strides (its row-window kernel stages one window of 128 + kw - 1
- * pixels per filter row and channel slice).                                                                         */
-B3D_API int b3d_conv2d_flat_tf32(const float* x, const float* wt, const float* bias, float* out, int N, int H, int P,
-                                 int Cin, int Hout, int Wout, int Cout, int ntaps, const int* dy, const int* dx,
-                                 int OH, int OW, int OC, float leaky, void* stream);
 
 /* Weight gradient of the same convolution (split-K wgmma GEMM over the output pixels; the M/N-major operands are read
  * straight from the NHWC tensors and transposed slice by slice in shared memory):
@@ -388,12 +360,6 @@ B3D_API int b3d_wrap_x_bwd_inplace(float* g, long long rows, int W, int C, int a
 B3D_API int b3d_pad_leaky_bias_bwd(const float* gout_pad, const float* y_pad, float* gy, float* gbias, long long rows, int W,
                                    int C, int amount, int mode, float slope, void* stream);
 B3D_API int b3d_leaky_bwd(const float* gy, const float* y, float* out, long long n, float slope, void* stream);
-
-/* Batch-norm statistics of an NHWC activation y [rows = N*H*W, C] in one pass: mean[c] and invstd[c] = 1/sqrt(biased
- * variance + eps) — what F.batch_norm / torch.batch_norm_stats compute for the generator's BatchNorm2d(affine=False)
- * layers (models/gan.py:211-232).  workspace: 2*C doubles (zeroed by the call).  C = 4 * a divisor of 256. */
-B3D_API int b3d_bn_stats(const float* y, long long rows, int C, float eps, float* mean, float* invstd, double* workspace,
-                         void* stream);
 
 /* Fused generator glue between two convolutions (models/gan.py:282-286 ConditionalBatchNorm2d, :309-311 LeakyReLU and
  * residual add, :319 nearest x2 upsample, :329 replicate pad), NHWC, C % 4 == 0:

@@ -23,6 +23,24 @@ def test_library_exports_every_declared_symbol():
     assert not missing, f"declared in b3d.h but not exported: {missing}"
 
 
+def declared_parameter_counts():
+    """{function: number of parameters} of every prototype in include/b3d.h."""
+    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "b3d.h")).read(), flags=re.S)
+    return {name: 0 if params.strip() in ("", "void") else params.count(",") + 1
+            for name, params in re.findall(r"B3D_API[^;(]*?\b(b3d_\w+)\s*\(([^)]*)\)\s*;", text)}
+
+
+def test_argtypes_match_the_header():
+    """ctypes passes surplus trailing arguments without an error, so a binding whose argtypes disagree with the prototype
+    would shift the arguments of its call sites instead of failing."""
+    import b3d
+    counts = declared_parameter_counts()
+    typed = {n: len(getattr(b3d.lib, n).argtypes) for n in counts if getattr(b3d.lib, n).argtypes is not None}
+    assert "b3d_conv2d_tf32" in typed and "b3d_pc_project" in typed
+    bad = {n: (k, counts[n]) for n, k in typed.items() if k != counts[n]}
+    assert not bad, f"(argtypes, parameters in b3d.h) differ: {bad}"
+
+
 def test_error_reporting_without_gpu():
     import b3d
     # argument validation happens before any CUDA call

@@ -55,12 +55,12 @@ def _conv_args(x, wt, out, Hout, Wout, dy, dx, stats, opts):
     N, H, W, Cin = x.shape
     Cout = wt.shape[1]
     return (ptr(wt), None, ptr(out), N, H, W, Cin, Hout, Wout, Cout, len(dy), _ints(dy), _ints(dx), 1, 1, out.shape[1], out.shape[2],
-            Cout, 1, 1, 0, 0, 1.0, 0, None, 0, ptr(stats), 0, 0, ctypes.cast(ctypes.pointer(opts), ctypes.c_void_p) if opts else None,
+            Cout, 1, 1, 0, 0, 1.0, None, 0, ptr(stats), 0, 0, ctypes.cast(ctypes.pointer(opts), ctypes.c_void_p) if opts else None,
             stream_ptr(x))
 
 
 @pytest.mark.parametrize("N,H,W,Cin,Cout", [(2, 16, 130, 64, 64), (8, 80, 256, 64, 64), (1, 8, 40, 32, 128), (1, 16, 16, 256, 256)])
-def test_conv_epilogue_mask_and_row_pitch(N, H, W, Cin, Cout):
+def test_conv_opts_mask_and_row_pitch(N, H, W, Cin, Cout):
     """3x3 stride-1 conv through b3d_conv2d_tf32 (row-window or per-tap kernel, whichever the shape dispatches) with
     (a) the activation mask + sum statistics and (b) the input read as the interior of a wider buffer."""
     from b3d import check, lib, ptr
@@ -172,12 +172,12 @@ def test_chained_backward_equals_stand_alone_passes(res, nd, B):
     assert passes[1] == len(discs) and passes[0] == sum(4 if isinstance(d, gan.TextureDiscriminator) else 3 for d in discs), passes
 
 
-def test_chain_is_off_without_the_weight_bank_and_by_switch(monkeypatch):
+def test_chain_is_off_without_the_weight_bank_or_when_disabled():
     from models import gan
     args = GC.make_args(256, 2)
     _, D = GC.build(gan, args)
     assert all(lk is None for lk in D.d1._links(3, None))
-    monkeypatch.setenv("B3D_NO_ACT_CHAIN", "1")
+    D.d1.disable_act_chain = True
     assert all(lk is None for lk in D.d1._links(3, {"x": 1}))
 
 
@@ -187,6 +187,7 @@ def test_merged_parity_classes_equal_per_class_launches(res, nd, B, monkeypatch)
     launches: the same taps per output pixel.  The merged launch has four times the work items, so the dispatcher may pick
     another kernel variant (stacked tiles / row window) whose K loop runs in another order: fp32 summation-order differences
     only, 2e-5 of the largest magnitude on the input gradients (they pass through input-gradient kernels only)."""
+    import b3d.conv as b3d_conv
     from models import gan
     args = GC.make_args(res, nd)
     _, D = GC.build(gan, args)
@@ -195,11 +196,11 @@ def test_merged_parity_classes_equal_per_class_launches(res, nd, B, monkeypatch)
     x0 = torch.cat((tex, alpha), dim=1)
     saved = {n: b.clone() for n, b in D.named_buffers()}
     got = []
-    for per_class in ("1", None):
+    for per_class in (True, False):
         if per_class:
-            monkeypatch.setenv("B3D_DGRAD_PER_CLASS", per_class)
+            monkeypatch.setattr(b3d_conv, "_merge_parity_classes", lambda classes: False)
         else:
-            monkeypatch.delenv("B3D_DGRAD_PER_CLASS")
+            monkeypatch.undo()
         with torch.no_grad():
             for n, b in D.named_buffers():
                 b.copy_(saved[n])

@@ -283,13 +283,12 @@ def test_statistics_from_conv_epilogue_and_from_bn_sums(Cin, C, H, W):
 
 @pytest.mark.parametrize("N,C,H,W", [(32, 64, 64, 32), (32, 256, 16, 8), (2, 1024, 33, 17)])
 @pytest.mark.parametrize("offset,bound", [(16.0, 1e-5), (64.0, 1.5e-4)])
-def test_statistics_with_large_channel_means(N, C, H, W, offset, bound):
-    """Channel means 16x / 64x their standard deviation.  b3d_bn_stats / b3d_bn_sums add fp32 per-thread partials and fp64
+def test_bn_sums_with_large_channel_means(N, C, H, W, offset, bound):
+    """Channel means 16x / 64x their standard deviation.  b3d_bn_sums adds fp32 per-thread partials and fp64
     block totals.  On an H100 the largest relative inv_std error over the channels of these shapes is 2.4e-6 at 16x and
     5.7e-5 at 64x (a numpy emulation of the summation order agrees channel by channel in magnitude); the bounds are ~3x
     that.  Adding the block totals in fp32 would miss them by orders of magnitude."""
     from b3d import lib, ptr, stream_ptr
-    from b3d.ew import bn_stats
     g = torch.Generator().manual_seed(C + int(offset))
     sd = 0.5 + torch.rand(C, generator=g, dtype=torch.float64)
     y64 = (offset + torch.randn(N, H, W, C, generator=g, dtype=torch.float64)) * sd
@@ -297,18 +296,15 @@ def test_statistics_with_large_channel_means(N, C, H, W, offset, bound):
     y64 = y.double()
     m_ref, v_ref = y64.mean(dim=(0, 1, 2)), y64.var(dim=(0, 1, 2), unbiased=False)
     inv_ref = (v_ref + EPS).rsqrt()
-    mean, invstd = bn_stats(y, EPS, impl="b3d")
     sums = torch.empty(2 * C, device=DEV, dtype=torch.float64)
     assert lib.b3d_bn_sums(ptr(y), N * H * W, C, ptr(sums), stream_ptr(y)) == 0
     torch.cuda.synchronize()
     n = N * H * W
     m_s = sums[:C] / n
     inv_s = ((sums[C:] / n - m_s * m_s).clamp(min=0) + EPS).rsqrt()
-    for name, inv in (("b3d_bn_stats", invstd.double()), ("b3d_bn_sums", inv_s)):
-        rel = float(((inv - inv_ref) / inv_ref).abs().max())
-        print(f"  {name} offset {offset:g}: rel inv_std error {rel:.2e}")
-        assert rel <= bound, f"{name}: relative inv_std error {rel:.2e} > {bound:g}"
-    assert float(((mean.double() - m_ref) / m_ref).abs().max()) <= 1e-6
+    rel = float(((inv_s - inv_ref) / inv_ref).abs().max())
+    print(f"  b3d_bn_sums offset {offset:g}: rel inv_std error {rel:.2e}")
+    assert rel <= bound, f"b3d_bn_sums: relative inv_std error {rel:.2e} > {bound:g}"
     assert float(((m_s - m_ref) / m_ref).abs().max()) <= 1e-6
 
 

@@ -1,7 +1,6 @@
-"""Device timing of the point-cloud silhouette kernels at cfg3's size (B 32, N 8000, V 128) for the record path chosen by
-B3D_PC_TMA (read once per process: run this once per value).  CUDA events around the libb3d entry points, L2 flushed
-between iterations, median of 20.  Also compares the result bit-for-bit-or-close with the other path's saved output when
-tools/time_pc.py is given a file name (written by the first run, read by the second)."""
+"""Device timing of the point-cloud silhouette kernels at cfg3's size (B 32, N 8000, V 128).  CUDA events around the libb3d
+entry points, L2 flushed between iterations, median of 20.  Given a file name, the first run saves its outputs there and a
+later run (e.g. of another build) prints its difference to them."""
 import os
 import statistics
 import sys
@@ -36,14 +35,13 @@ for it in range(ITERS):
     if it >= 5:
         for k, v in b3d.prof_disable().items():
             rec.setdefault(k, []).append(sum(v))
-print(f"B3D_PC_TMA={os.environ.get('B3D_PC_TMA', '(default)')} staging={b3d.lib.b3d_pc_tma_staging()}  " +
-      "  ".join(f"{k.replace('b3d_pc_', '')} {statistics.median(v) * 1e3:.1f} us" for k, v in sorted(rec.items())))
+print("  ".join(f"{k.replace('b3d_pc_', '')} {statistics.median(v) * 1e3:.1f} us" for k, v in sorted(rec.items())))
 out = {"sil": sil.detach().cpu(), "dp": p.grad.cpu(), "dq": q.grad.cpu(), "ds": s.grad.cpu()}
 if len(sys.argv) > 1:
     f = sys.argv[1]
     if os.path.exists(f):
         other = torch.load(f)
-        print("max |difference| to the other record path:", {k: float((out[k] - other[k]).abs().max()) for k in out},
+        print(f"max |difference| to {f}:", {k: float((out[k] - other[k]).abs().max()) for k in out},
               "scale", {k: float(other[k].abs().max()) for k in out})
     else:
         torch.save(out, f)

@@ -32,6 +32,6 @@ void count_launch(int n) { g_launches.fetch_add((uint64_t)n, std::memory_order_r
 extern "C" {
 const char* b3d_last_error(void) { return b3d::g_err; }
 const char* b3d_last_variant(void) { return b3d::g_variant; }
-int b3d_version(void) { return 300; }   // 3.0: b3d_conv2d_tf32 takes tap-major weights only; unused exports removed
+int b3d_version(void) { return 310; }   // 3.1: b3d_gather_fields (GAN training data)
 uint64_t b3d_launch_count(void) { return b3d::g_launches.load(std::memory_order_relaxed); }
 }

@@ -425,6 +425,33 @@ B3D_API int b3d_maxpool3x3s2_nhwc(const float* x, int N, int H, int W, int C, fl
 B3D_API int b3d_mean_hw_nhwc(const float* x, int N, int HW, int C, float* out, void* stream);
 B3D_API int b3d_fid_accumulate(const float* feat, int n, int D, double* sum, double* outer, void* stream);
 
+/* ---- GAN training data (reference: data/abstract_dataset.py:68-107 load_pseudo_ground_truth / __getitem__ / mirror_tex,
+ * main.py:672-690 the loader's batch -> X_tex / X_alpha / X_mesh / C) ---------------------------------------------------
+ * b3d_gather_fields  one launch assembles a batch from packed per-record stores: for every field, sample b < B and plane
+ *                    c < C:  dst[b,c] = scale * widen(src[idx[b], c]) + bias  (the plain value when scale == 1, bias == 0,
+ *                    so -0 stays -0).  When field.mirror and flip[b] are set, output column j reads source column
+ *                    W-1-((j + W/2) mod W): mirror_tex's flip along u + half-turn shift.  flip may be NULL (no mirroring).
+ *                    B3D_GATHER_I64 fields copy int64 rows (the class labels) unchanged and cannot mirror.
+ *                    An index outside [0, n) writes NaN (int64: -1) instead of reading outside the store.
+ *                    src may be device memory or pinned (page-locked, mapped) host memory read over PCIe through its UVA
+ *                    pointer; pageable host memory is rejected with B3D_EINVAL.  dst: [B,C,H,W] fp32 (int64 for I64),
+ *                    device memory.  nfields <= B3D_GATHER_MAX_FIELDS; C <= C_src.                                    */
+#define B3D_GATHER_F32 0
+#define B3D_GATHER_F16 1
+#define B3D_GATHER_I64 2
+#define B3D_GATHER_MAX_FIELDS 8
+typedef struct {
+    const void* src; /* [n, C_src, H, W] of src_type */
+    int src_type;    /* B3D_GATHER_F32 / _F16 / _I64 */
+    int n;           /* records in src */
+    int C_src, C, H, W;
+    int mirror;
+    float scale, bias;
+    void* dst;
+} b3d_gather_field;
+B3D_API int b3d_gather_fields(const b3d_gather_field* fields, int nfields, const int32_t* idx, const uint8_t* flip, int B,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif

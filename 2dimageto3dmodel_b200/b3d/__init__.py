@@ -109,6 +109,7 @@ _sig("b3d_rgba_l1_iou_fwd", _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp)
 _sig("b3d_rgba_l1_bwd", _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp)
 _sig("b3d_mesh_render_bwd", _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp)
 _sig("b3d_gather_fields", _vp, _i, _vp, _vp, _i, _vp)
+_sig("b3d_image_batch", _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp)
 
 
 def mode_id(mode):
@@ -214,4 +215,4 @@ _TIMED = ("b3d_pc_project", "b3d_pc_silhouette_fwd_hosttaps", "b3d_pc_silhouette
           "b3d_pc_splat_grid", "b3d_mesh_face_setup", "b3d_mesh_render_fwd", "b3d_mesh_render_bwd", "b3d_face_normals_fwd", "b3d_face_normals_bwd", "b3d_flat_loss_fwd",
           "b3d_flat_loss_bwd", "b3d_rgba_mse_iou_fwd", "b3d_rgba_mse_bwd", "b3d_rgba_l1_iou_fwd", "b3d_rgba_l1_bwd", "b3d_chamfer_nn", "b3d_chamfer_bwd", "b3d_conv2d_tf32", "b3d_conv2d_wgrad_tf32", "b3d_conv2d_thin_fwd", "b3d_conv2d_thin_wgrad", "b3d_pad_x_fwd", "b3d_pad_x_bwd", "b3d_stem_input_fwd", "b3d_stem_input_bwd",
           "b3d_leaky_bwd", "b3d_wrap_x_inplace", "b3d_wrap_x_bwd_inplace", "b3d_pad_leaky_bias_bwd", "b3d_fold_rows_fwd", "b3d_fold_rows_bwd", "b3d_cbn_act_fwd", "b3d_cbn_act_bwd1", "b3d_cbn_act_bwd2", "b3d_bn_sums", "b3d_cbn_prepare", "b3d_cbn_bwd_reduce",
-          "b3d_bank_forward", "b3d_bank_backward", "b3d_vertex_pipeline_fwd", "b3d_vertex_pipeline_bwd", "b3d_gather_fields")
+          "b3d_bank_forward", "b3d_bank_backward", "b3d_vertex_pipeline_fwd", "b3d_vertex_pipeline_bwd", "b3d_gather_fields", "b3d_image_batch")

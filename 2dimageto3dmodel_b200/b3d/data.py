@@ -1,5 +1,8 @@
-"""Binding of b3d_gather_fields: one launch that assembles a batch from packed per-record stores (gather by index,
-fp16 -> fp32, UV mirroring).  The stores may sit in device memory or in pinned host memory (read over PCIe)."""
+"""Bindings of the training-data kernels.
+b3d_gather_fields: one launch that assembles a GAN batch from packed per-record stores (gather by index, fp16 -> fp32, UV
+mirroring).  The stores may sit in device memory or in pinned host memory (read over PCIe).
+b3d_image_batch: one launch that builds a reconstruction batch (crop, cv2-style resize, mirror, poses) from packed photo
+windows in device memory."""
 import ctypes
 
 import torch
@@ -56,3 +59,54 @@ def gather_fields(fields, idx, flip=None):
         arr[i] = GatherField(src.data_ptr(), _TYPES[src.dtype], n, C_src, C, H, W, int(bool(mirror)), float(scale),
                              float(bias), dst.data_ptr())
     check(lib.b3d_gather_fields(ctypes.cast(arr, ctypes.c_void_p), len(fields), ptr(idx), ptr(flip), B, stream_ptr(idx)))
+
+
+MAX_RES = 4          # B3D_IMAGE_MAX_RES
+MAX_SIDE = 2048      # B3D_IMAGE_MAX_SIDE
+
+
+def _cuda(t, dtype, name, dim=None):
+    if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dtype and t.is_contiguous()
+            and (dim is None or t.dim() == dim)):
+        raise B3DError(f"image_batch: {name} must be a contiguous {dtype} CUDA tensor"
+                       + (f" with {dim} dimensions" if dim is not None else ""))
+
+
+def image_batch(pixels, offsets, geometry, poses, idx, flip, images, scale, translation, rot, ind):
+    """b3d_image_batch: one launch builds a reconstruction batch from packed photo windows.
+    Store: pixels int32 [words] (RGBM bytes per word), offsets int64 [n], geometry int32 [n, 5] (ww, wh, wx0, wy0, S),
+    poses fp32 [n, 2, 8].  idx int32 [B], flip uint8 [B] or None.  Outputs (fp32 unless noted, on the device):
+    images [[B,4,R0,R0], [B,3,R1,R1], ...], scale [B,1], translation [B,3], rot [B,4], ind int64 [B]."""
+    _cuda(pixels, torch.int32, 'pixels', 1)
+    _cuda(offsets, torch.int64, 'offsets', 1)
+    n = offsets.shape[0]
+    _cuda(geometry, torch.int32, 'geometry')
+    _cuda(poses, torch.float32, 'poses')
+    if tuple(geometry.shape) != (n, 5) or tuple(poses.shape) != (n, 2, 8):
+        raise B3DError(f"image_batch: geometry {tuple(geometry.shape)} / poses {tuple(poses.shape)} do not fit {n} records")
+    _cuda(idx, torch.int32, 'idx', 1)
+    B = idx.shape[0]
+    if flip is not None:
+        _cuda(flip, torch.uint8, 'flip', 1)
+        if flip.shape[0] != B:
+            raise B3DError(f"image_batch: flip has {flip.shape[0]} entries for {B} samples")
+    if not 1 <= len(images) <= MAX_RES:
+        raise B3DError(f"image_batch: 1 to {MAX_RES} image outputs, got {len(images)}")
+    res = []
+    for k, im in enumerate(images):
+        _cuda(im, torch.float32, f'image output {k}', 4)
+        R = im.shape[-1]
+        if tuple(im.shape) != (B, 4 if k == 0 else 3, R, R):
+            raise B3DError(f"image_batch: image output {k} has shape {tuple(im.shape)}; expected "
+                           f"[{B}, {4 if k == 0 else 3}, R, R]")
+        res.append(R)
+    for t, name, dt, shape in ((scale, 'scale', torch.float32, (B, 1)), (translation, 'translation', torch.float32, (B, 3)),
+                               (rot, 'rot', torch.float32, (B, 4)), (ind, 'ind', torch.int64, (B,))):
+        _cuda(t, dt, name)
+        if tuple(t.shape) != shape:
+            raise B3DError(f"image_batch: {name} has shape {tuple(t.shape)}; expected {list(shape)}")
+    res_arr = (ctypes.c_int32 * len(res))(*res)
+    img_arr = (ctypes.c_void_p * len(images))(*[im.data_ptr() for im in images])
+    check(lib.b3d_image_batch(ptr(pixels), ptr(offsets), ptr(geometry), ptr(poses), n, ptr(idx), ptr(flip), B, len(res),
+                              ctypes.cast(res_arr, ctypes.c_void_p), ctypes.cast(img_arr, ctypes.c_void_p), ptr(scale),
+                              ptr(translation), ptr(rot), ptr(ind), stream_ptr(idx)))

@@ -120,6 +120,179 @@ int check_accessible(const void* p, const char* what, int field) {
     return B3D_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Reconstruction training data: crop + cv2-style bilinear resize (double) + mirror of a batch of packed RGBM windows
+// (cmr_data/base.py:58-130, run_reconstruction.py:104-133).
+
+constexpr int IMG_NT = 256;
+constexpr int IMG_ROWS = 4;   // output rows per CTA
+
+struct ImageArgs {
+    const uint32_t* pixels;
+    const int64_t* offsets;
+    const int32_t* geometry;  // [n, 5]: ww, wh, wx0, wy0, S
+    const float* poses;       // [n, 2, 8]
+    int n;
+    const int32_t* idx;
+    const uint8_t* flip;
+    int nres;
+    int res[B3D_IMAGE_MAX_RES];
+    int vec[B3D_IMAGE_MAX_RES];        // 4: float4 stores, 1: scalar
+    int block_end[B3D_IMAGE_MAX_RES];  // exclusive prefix of the CTAs of each resolution
+    float* images[B3D_IMAGE_MAX_RES];
+    float* scale;
+    float* translation;
+    float* rot;
+    int64_t* ind;
+};
+
+// cv2 INTER_LINEAR taps of output sample d of an S -> R axis: scale = 1 / (R / S), fx = (d + 0.5) scale - 0.5, clamped to
+// the edge.  Every operation rounds on its own (no fused multiply-add), as the numpy restatement does.
+__device__ __forceinline__ void linear_tap(int d, int S, double scale, int& s0, double& w1) {
+    double fx = __dsub_rn(__dmul_rn((double)d + 0.5, scale), 0.5);
+    const double fl = floor(fx);
+    fx = __dsub_rn(fx, fl);
+    int s = (int)fl;
+    if (s < 0) s = 0, fx = 0.0;
+    if (s >= S - 1) s = S - 1, fx = 0.0;
+    s0 = s;
+    w1 = fx;
+}
+
+__device__ __forceinline__ double lerp2(double a, double b, double w0, double w1) {
+    return __dadd_rn(__dmul_rn(a, w0), __dmul_rn(b, w1));
+}
+
+// RGBM word of crop pixel (u, v): the window's word, or the crop background (RGB 255 -> 1.0, mask 0) outside the photo
+__device__ __forceinline__ uint32_t crop_word(const uint32_t* win, int ww, int wh, int wx0, int wy0, int u, int v) {
+    const unsigned x = (unsigned)(u - wx0), y = (unsigned)(v - wy0);
+    return (x < (unsigned)ww && y < (unsigned)wh) ? __ldg(win + (long long)y * ww + x) : 0x00FFFFFFu;
+}
+
+struct ImageTile {
+    const uint32_t* win;
+    int ww, wh, wx0, wy0, S;
+    int R, C, y_base, rows;
+    bool mirrored;
+    float* out;
+    long long plane;
+};
+
+// The CTA's rows of one sample at one resolution, VEC consecutive output pixels per thread and step.
+template <int VEC>
+__device__ __forceinline__ void image_rows(const ImageTile& q, const int* col_s0, const double* col_w1, const int* row_s0,
+                                           const double* row_w1, const double* lut) {
+    const int groups = q.R / VEC;
+    for (int t = threadIdx.x; t < q.rows * groups; t += IMG_NT) {
+        const int r = t / groups, x_base = (t % groups) * VEC;
+        const int v0 = row_s0[r], v1 = min(v0 + 1, q.S - 1);
+        const double b1 = row_w1[r], b0 = 1.0 - b1;
+        float px[4][VEC];  // [channel][pixel]
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) {
+            const int xr = q.mirrored ? q.R - 1 - (x_base + j) : x_base + j;   // resized column this output column shows
+            const int u0 = col_s0[xr], u1 = min(u0 + 1, q.S - 1);
+            const double a1 = col_w1[xr], a0 = 1.0 - a1;
+            const uint32_t p00 = crop_word(q.win, q.ww, q.wh, q.wx0, q.wy0, u0, v0);
+            const uint32_t p01 = crop_word(q.win, q.ww, q.wh, q.wx0, q.wy0, u1, v0);
+            const uint32_t p10 = crop_word(q.win, q.ww, q.wh, q.wx0, q.wy0, u0, v1);
+            const uint32_t p11 = crop_word(q.win, q.ww, q.wh, q.wx0, q.wy0, u1, v1);
+            // mask: the raw annotation value (0 / 1), interpolated like the image
+            const double m = lerp2(lerp2((double)(p00 >> 24), (double)(p01 >> 24), a0, a1),
+                                   lerp2((double)(p10 >> 24), (double)(p11 >> 24), a0, a1), b0, b1);
+            const float mf = __double2float_rn(m);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const int sh = 8 * c;
+                const double v = lerp2(lerp2(lut[(p00 >> sh) & 255u], lut[(p01 >> sh) & 255u], a0, a1),
+                                       lerp2(lut[(p10 >> sh) & 255u], lut[(p11 >> sh) & 255u], a0, a1), b0, b1);
+                // ImageDataset: float32(img) * 2 - 1, then * float32(mask), each op rounded in fp32
+                px[c][j] = __fmul_rn(__fadd_rn(__fmul_rn(__double2float_rn(v), 2.f), -1.f), mf);
+            }
+            px[3][j] = mf;
+        }
+        const long long o = (long long)(q.y_base + r) * q.R + x_base;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            if (c == q.C) break;
+            float* dst = q.out + c * q.plane + o;
+            if constexpr (VEC == 4)
+                *reinterpret_cast<float4*>(dst) = make_float4(px[c][0], px[c][1], px[c][2], px[c][3]);
+            else
+                dst[0] = px[c][0];
+        }
+    }
+}
+
+__global__ void __launch_bounds__(IMG_NT) image_batch_kernel(const __grid_constant__ ImageArgs a) {
+    __shared__ int col_s0[B3D_IMAGE_MAX_SIDE];
+    __shared__ double col_w1[B3D_IMAGE_MAX_SIDE];
+    __shared__ int row_s0[IMG_ROWS];
+    __shared__ double row_w1[IMG_ROWS];
+    __shared__ double lut[256];  // byte / 255.0, as imread(...) / 255.0
+
+    int k = 0;
+    while ((int)blockIdx.x >= a.block_end[k]) ++k;
+    const int R = a.res[k];
+    const int tiles = (R + IMG_ROWS - 1) / IMG_ROWS;
+    const int local = blockIdx.x - (k ? a.block_end[k - 1] : 0);
+    const int b = local / tiles, y_base = (local % tiles) * IMG_ROWS;
+    const int rows = min(IMG_ROWS, R - y_base);
+    const int C = k == 0 ? 4 : 3;
+    const long long plane = (long long)R * R;
+    float* out = a.images[k] + (long long)b * C * plane;
+
+    const int s = a.idx[b];
+    const bool in_range = s >= 0 && s < a.n;
+    int ww = 0, wh = 0, wx0 = 0, wy0 = 0, S = 0;
+    if (in_range) {
+        const int32_t* g = a.geometry + 5LL * s;
+        ww = g[0], wh = g[1], wx0 = g[2], wy0 = g[3], S = g[4];
+    }
+    const bool ok = in_range && S >= 1 && ww >= 0 && wh >= 0;
+    const bool mirrored = a.flip && a.flip[b];
+
+    if (k == 0 && y_base == 0 && threadIdx.x < 8) {
+        const int f = mirrored ? 1 : 0;
+        const float p = ok ? a.poses[(2LL * s + f) * 8 + threadIdx.x] : __int_as_float(0x7fc00000);
+        if (threadIdx.x == 0) {
+            a.scale[b] = p;
+            a.ind[b] = ok ? (int64_t)s + (int64_t)a.n * f : -1;
+        } else if (threadIdx.x < 4) {
+            a.translation[3LL * b + threadIdx.x - 1] = p;
+        } else {
+            a.rot[4LL * b + threadIdx.x - 4] = p;
+        }
+    }
+    if (!ok) {
+        const float nan = __int_as_float(0x7fc00000);
+        for (int c = 0; c < C; ++c)
+            for (int t = threadIdx.x; t < rows * R; t += IMG_NT) out[c * plane + (long long)y_base * R + t] = nan;
+        return;
+    }
+
+    const double scale = __ddiv_rn(1.0, __ddiv_rn((double)R, (double)S));
+    for (int d = threadIdx.x; d < R; d += IMG_NT) linear_tap(d, S, scale, col_s0[d], col_w1[d]);
+    if (threadIdx.x < rows) linear_tap(y_base + threadIdx.x, S, scale, row_s0[threadIdx.x], row_w1[threadIdx.x]);
+    lut[threadIdx.x] = __ddiv_rn((double)threadIdx.x, 255.0);
+    __syncthreads();
+
+    const uint32_t* win = a.pixels + a.offsets[s];
+    const ImageTile tile{win, ww, wh, wx0, wy0, S, R, C, y_base, rows, mirrored, out, plane};
+    if (a.vec[k] == 4)
+        image_rows<4>(tile, col_s0, col_w1, row_s0, row_w1, lut);
+    else
+        image_rows<1>(tile, col_s0, col_w1, row_s0, row_w1, lut);
+}
+
+int check_device_ptr(const void* p, const char* what) {
+    cudaPointerAttributes at;
+    B3D_CUDA_OK(cudaPointerGetAttributes(&at, p));
+    B3D_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged, B3D_EINVAL,
+                "b3d_image_batch: %s is not device memory", what);
+    return B3D_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -163,6 +336,51 @@ int b3d_gather_fields(const b3d_gather_field* fields, int nfields, const int32_t
     if (rc == B3D_OK && flip) rc = check_accessible(flip, "flip", -1);
     if (rc != B3D_OK) return rc;
     gather_fields_kernel<<<(unsigned)blocks, NT, 0, (cudaStream_t)stream>>>(a);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+int b3d_image_batch(const uint32_t* pixels, const int64_t* offsets, const int32_t* geometry, const float* poses, int n,
+                    const int32_t* idx, const uint8_t* flip, int B, int nres, const int32_t* res, float* const* images,
+                    float* scale, float* translation, float* rot, int64_t* ind, void* stream) {
+    static_assert(IMG_NT == 256, "the byte / 255 table is filled one entry per thread");
+    B3D_REQUIRE(n >= 1 && B >= 0 && nres >= 1 && nres <= B3D_IMAGE_MAX_RES && res && images, B3D_EINVAL,
+                "b3d_image_batch: bad arguments (n %d, B %d, nres %d)", n, B, nres);
+    B3D_REQUIRE(pixels && offsets && geometry && poses, B3D_EINVAL, "b3d_image_batch: null store pointer");
+    if (B == 0) return B3D_OK;
+    B3D_REQUIRE(idx && scale && translation && rot && ind, B3D_EINVAL, "b3d_image_batch: null idx or pose output");
+    ImageArgs a = {};
+    a.pixels = pixels, a.offsets = offsets, a.geometry = geometry, a.poses = poses, a.n = n;
+    a.idx = idx, a.flip = flip, a.nres = nres;
+    a.scale = scale, a.translation = translation, a.rot = rot, a.ind = ind;
+    long long blocks = 0;
+    for (int k = 0; k < nres; ++k) {
+        B3D_REQUIRE(images[k], B3D_EINVAL, "b3d_image_batch: null image output %d", k);
+        B3D_REQUIRE(res[k] >= 1 && res[k] <= B3D_IMAGE_MAX_SIDE, B3D_EINVAL,
+                    "b3d_image_batch: resolution %d of output %d outside [1, %d]", res[k], k, B3D_IMAGE_MAX_SIDE);
+        a.res[k] = res[k];
+        a.images[k] = images[k];
+        a.vec[k] = (res[k] % 4 == 0 && (reinterpret_cast<uintptr_t>(images[k]) & 15u) == 0) ? 4 : 1;
+        blocks += (long long)B * ((res[k] + IMG_ROWS - 1) / IMG_ROWS);
+        B3D_REQUIRE(blocks < (1LL << 31), B3D_EINVAL, "b3d_image_batch: batch too large");
+        a.block_end[k] = (int)blocks;
+    }
+    for (int k = nres; k < B3D_IMAGE_MAX_RES; ++k) a.block_end[k] = (int)blocks;
+    const void* dev[] = {pixels, offsets, geometry, poses, idx, scale, translation, rot, ind};
+    const char* names[] = {"pixels", "offsets", "geometry", "poses", "idx", "scale", "translation", "rot", "ind"};
+    for (int i = 0; i < 9; ++i) {
+        const int rc = check_device_ptr(dev[i], names[i]);
+        if (rc != B3D_OK) return rc;
+    }
+    if (flip) {
+        const int rc = check_device_ptr(flip, "flip");
+        if (rc != B3D_OK) return rc;
+    }
+    for (int k = 0; k < nres; ++k) {
+        const int rc = check_device_ptr(images[k], "an image output");
+        if (rc != B3D_OK) return rc;
+    }
+    image_batch_kernel<<<(unsigned)blocks, IMG_NT, 0, (cudaStream_t)stream>>>(a);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }

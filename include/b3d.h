@@ -452,6 +452,32 @@ typedef struct {
 B3D_API int b3d_gather_fields(const b3d_gather_field* fields, int nfields, const int32_t* idx, const uint8_t* flip, int B,
                               void* stream);
 
+/* ---- Reconstruction training data (reference: cmr_data/base.py:58-130 forward_img / crop_image / scale_image /
+ * mirror_image / normalize_kp, cmr_data/image_utils.py:8-91 resize_img / crop, run_reconstruction.py:104-133
+ * ImageDataset.__getitem__) ------------------------------------------------------------------------------------------
+ * b3d_image_batch  one launch builds a batch of run_reconstruction.py's loader from packed photo windows.  Record s is
+ *                  the part of its S x S crop square that lies inside the photo: geometry[s] = (ww, wh, wx0, wy0, S), the
+ *                  window's size and origin inside the square, and pixels[offsets[s] ...] its ww * wh RGBM words (byte 0
+ *                  R, 1 G, 2 B, 3 the raw mask value), row-major.  For sample b < B (s = idx[b], mirrored when flip &&
+ *                  flip[b]) and output k < nres of side R = res[k]:
+ *                    crop pixels outside the window are RGB 1.0, mask 0; RGB = byte / 255.0, mask = byte, in double;
+ *                    cv2.resize INTER_LINEAR S -> R in double (taps and weights of each axis: scale = 1 / (R / S),
+ *                    fx = (d + 0.5) scale - 0.5, clamped to the edge; horizontal then vertical pass, no fused
+ *                    multiply-add); mirrored, output column x shows resized column R-1-x;
+ *                    img = fp32(rgb) * 2 - 1, then * fp32(mask), in fp32 round-to-nearest.
+ *                  images[0]: [B,4,R0,R0] fp32 (img, mask); images[k > 0]: [B,3,Rk,Rk] fp32 (img).
+ *                  poses[s, f] (f = mirrored) = (scale, tx, ty, 0, qw, qx, qy, qz) fp32: scale[b] (= [B,1]),
+ *                  translation[3b..] = (tx, ty, 0), rot[4b..] = q; ind[b] = s + n * f.
+ *                  An index outside [0, n) or a record with S < 1 writes NaN rows (ind -1).  Every pointer must be device
+ *                  memory (B3D_EINVAL otherwise); res and images are host arrays of nres <= B3D_IMAGE_MAX_RES entries,
+ *                  1 <= res[k] <= B3D_IMAGE_MAX_SIDE.                                                                  */
+#define B3D_IMAGE_MAX_RES 4
+#define B3D_IMAGE_MAX_SIDE 2048
+B3D_API int b3d_image_batch(const uint32_t* pixels, const int64_t* offsets, const int32_t* geometry, const float* poses,
+                            int n, const int32_t* idx, const uint8_t* flip, int B, int nres, const int32_t* res,
+                            float* const* images, float* scale, float* translation, float* rot, int64_t* ind,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,12 +2,16 @@
 
 Reference call sites: nn.Conv2d layers of /root/reference/code/models/gan.py (:57-65, :163-177, :294-302,
 :359, :364) — 3x3 / 1x1 / 5x5 stride 1 and 4x4 stride 2, zero padding along y only (x padding is explicit:
-replicate / circular pads are materialised by the caller exactly as the reference does)."""
+replicate / circular pads are materialised by the caller exactly as the reference does).
+
+Both entry points, conv2d (a module's own weight) and conv2d_banked (weights from b3d.bank.WeightBank), run one autograd
+function over the same three launch helpers; they differ only in where the kernel weight layouts come from."""
 import ctypes
 
 import torch
 
 from . import B3DError, check, dev, last_variant, lib, ptr, stream_ptr
+from .bank import LayerWeights
 
 VARIANT_LOG = None      # tests set this to a list: every kernel template instance the conv entry points launch is appended
 
@@ -24,53 +28,68 @@ def _ints(v):
     return (ctypes.c_int * len(v))(*v)
 
 
+def _pad_last(t, mult):
+    c = t.shape[-1]
+    return t if c % mult == 0 else torch.nn.functional.pad(t, (0, mult - c % mult))
+
+
 def taps_layout(weight):
     """[Cout,Cin,kh,kw] -> tap-major K-major rows [kh*kw, Cout, Cin]."""
     co, ci, kh, kw = weight.shape
     return weight.permute(2, 3, 0, 1).reshape(kh * kw, co, ci).contiguous()
 
 
+def _d_layout(wf):
+    """F [T][Cout][Cin] -> D [T][Cin][Cout'], its per-tap transpose with Cout zero-padded to a multiple of 32 (the input
+    gradient's operand)."""
+    return _pad_last(wf.transpose(1, 2), 32).contiguous()
+
+
 def _thin(Cout, Cin, kh, kw, stride):
     return Cout <= 4 and Cin % 64 == 0 and kh == 5 and kw == 5 and stride == 1
 
 
-def conv2d_nhwc(x, weight, bias=None, pad_y=0, stride=1, leaky=1.0, wt=None, pad_out=0, pad_mode=1, x_crop=0):
-    """x [N,H,W,Cin] (Cin % 32 == 0), weight [Cout,Cin,kh,kw] -> [N,Hout,Wout,Cout]; zero pad along y only.
-    pad_out > 0: the result is written into the interior of a [N,Hout,Wout + 2*pad_out,Cout] buffer whose pad columns
-    are then filled in place (replicate / circular) — the next convolution's padded input without a copy.
-    x_crop > 0 (stride 1): convolve x[:, :, x_crop:W - x_crop] without materialising the slice (taps are shifted)."""
-    x = dev(x, "x")
-    N, H, W, Cin = x.shape
-    Cout, Cin_w, kh, kw = weight.shape
-    if Cin_w != Cin:
-        raise B3DError(f"conv2d: input has {Cin} channels, weight expects {Cin_w}")
-    if wt is None:
-        wt = taps_layout(weight)
-    wt = dev(wt, "weight")
-    Hout = (H + 2 * pad_y - kh) // stride + 1
+class _ConvOpts(ctypes.Structure):
+    """b3d_conv_opts (include/b3d.h)."""
+    _fields_ = [("mask", ctypes.c_void_p), ("mask_slope", ctypes.c_float), ("stats_sum_only", ctypes.c_int),
+                ("x_row_pitch", ctypes.c_int), ("nclass", ctypes.c_int), ("class_ooy", ctypes.c_int * 4), ("class_oox", ctypes.c_int * 4)]
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# launch helpers: one per direction
+# ------------------------------------------------------------------------------------------------------------------
+def _fprop(x, wt, bias, kh, kw, pad_y=0, stride=1, leaky=1.0, pad_out=0, pad_mode=1, x_crop=0, stats=None, fold_kh=0,
+           fold_pad=0):
+    """conv2d_nhwc on F = wt [kh*kw][Cout][Cin'].  stats: zeroed fp64 [2*Cout] that the epilogue accumulates the output's
+    per-channel sum / sum of squares into.  fold_kh > 0: x is the RAW 8-channel stem input whose fold_kh vertical taps (y
+    padding fold_pad) the kernel folds into the K dimension on the fly (kh = 1, pad_y = 0)."""
+    N, H, W, _ = x.shape
+    _, Cout, Cin = wt.shape
     if x_crop and stride != 1:
         raise B3DError("conv2d: x_crop needs stride 1")
+    if pad_out and Cout % 4:
+        raise B3DError("conv2d: pad_out needs Cout % 4 == 0")
+    Hout = (H + 2 * fold_pad - fold_kh + 1) if fold_kh else (H + 2 * pad_y - kh) // stride + 1
     Wout = (W - 2 * x_crop - kw) // stride + 1
     OW = Wout + 2 * pad_out
     out = torch.empty(N, Hout, OW, Cout, device=x.device, dtype=torch.float32)
     optr = ctypes.c_void_p(out.data_ptr() + 4 * pad_out * Cout)          # pixel (n, y, pad_out) of the padded buffer
-    if pad_out and Cout % 4:
-        raise B3DError("conv2d: pad_out needs Cout % 4 == 0")
+    b = dev(bias, "bias") if bias is not None else None
+    st = stream_ptr(x)
     if _thin(Cout, Cin, kh, kw, stride):
         # 1-4 output channels: fp32 CUDA-core reduction kernel (csrc/thin_kernels.cu), not a 64-wide MMA tile
-        check(_conv_call(lib.b3d_conv2d_thin_fwd, ptr(x), ptr(wt), ptr(dev(bias, "bias") if bias is not None else None), optr, N, H, W,
-                                      Cin, Hout, Wout, Cout, kh, kw, pad_y, x_crop, OW, Cout, float(leaky), stream_ptr(x)))
-        if pad_out:
-            check(lib.b3d_wrap_x_inplace(ptr(out), N * Hout, Wout, Cout, pad_out, pad_mode, stream_ptr(x)))
-        return out
-    dy = [r - pad_y for r in range(kh) for _ in range(kw)]
-    dx = [s + x_crop for _ in range(kh) for s in range(kw)]
-    b = dev(bias, "bias") if bias is not None else None
-    check(_conv_call(lib.b3d_conv2d_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw, _ints(dy),
-                              _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), None, 0, None, 0, 0,
-                              None, stream_ptr(x)))
+        check(_conv_call(lib.b3d_conv2d_thin_fwd, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh, kw, pad_y,
+                         x_crop, OW, Cout, float(leaky), st))
+    else:
+        if stats is not None and (bias is not None or leaky != 1.0 or stride != 1):
+            raise B3DError("conv2d: output statistics are taken before bias / activation (plain stride-1 convs only)")
+        dy = [r - pad_y for r in range(kh) for _ in range(kw)]
+        dx = [s + x_crop for _ in range(kh) for s in range(kw)]
+        check(_conv_call(lib.b3d_conv2d_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw, _ints(dy),
+                         _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), None, 0, ptr(stats), fold_kh,
+                         fold_pad, None, st))
     if pad_out:
-        check(lib.b3d_wrap_x_inplace(ptr(out), N * Hout, Wout, Cout, pad_out, pad_mode, stream_ptr(x)))
+        check(lib.b3d_wrap_x_inplace(ptr(out), N * Hout, Wout, Cout, pad_out, pad_mode, st))
     return out
 
 
@@ -89,159 +108,114 @@ def stride2_classes(kh, kw, pad_y, H, W):
     return out
 
 
-def conv2d_dgrad_nhwc(dy_, weight, in_hw, pad_y=0, stride=1, x_crop=0):
-    """Gradient w.r.t. the (x-padded) input [N,H,W,Cin] of conv2d_nhwc, from dy_ [N,Hout,Wout,Cout] (Cout % 32 == 0)."""
-    g = dev(dy_, "grad_output")
-    N, Hout, Wout, Cout = g.shape
-    Cout_w, Cin, kh, kw = weight.shape
+def _merge_parity_classes(classes):
+    """One launch for the four parity classes of a stride-2 input gradient when they have the same extent and tap count
+    (even H, W; 4x4 kernels); otherwise one launch per class."""
+    return len(classes) == 4 and all(c[2] for c in classes) and len({(len(c[2]), c[5], c[6]) for c in classes}) == 1
+
+
+def _dgrad(gy, wd, in_hw, kh, kw, pad_y=0, stride=1, x_crop=0, g_pitch=0, mask=None, slope=1.0, sums=None):
+    """Gradient w.r.t. the (x-padded) input [N,H,W,Cin'] from gy [N,Hout,Wout,Cout] (zero-padded here to Cout', a multiple
+    of 32) and D = wd [kh*kw][Cin'][Cout'].  Stride-2 parity classes address their taps as rows of D (wtap).
+    g_pitch > 0: gy is the interior of a padded gradient whose rows are g_pitch pixels apart, read in place.
+    mask: the activation this input gradient flows into; the epilogue multiplies by its LeakyReLU'(slope) and, when `sums`
+    (zeroed fp64 [2*Cin']) is given, accumulates the per-channel sums of the result into it."""
+    gy = _pad_last(gy, 32)                                           # heads with 1 / 3 output channels: zero-pad K
+    N, Hout, Wout, Cop = gy.shape
+    Cin = wd.shape[1]
     H, W = in_hw
-    dxo = torch.empty(N, H, W, Cin, device=g.device, dtype=torch.float32)
-    st = stream_ptr(g)
-    if stride == 1:
-        wt = weight.permute(2, 3, 1, 0).reshape(kh * kw, Cin, Cout).contiguous()        # [tap][Cin][Cout]
-        dy = [pad_y - r for r in range(kh) for _ in range(kw)]
-        dx = [-s - x_crop for _ in range(kh) for s in range(kw)]
-        check(_conv_call(lib.b3d_conv2d_tf32, ptr(g), ptr(wt), None, ptr(dxo), N, Hout, Wout, Cout, H, W, Cin, kh * kw, _ints(dy),
-                                  _ints(dx), 1, 1, H, W, Cin, 1, 1, 0, 0, 1.0, None, 0, None, 0, 0, None, st))
-        return dxo
-    if stride != 2 or x_crop:
+    classes = stride2_classes(kh, kw, pad_y, H, W) if stride == 2 and not x_crop else []
+    if stride != 1 and not classes:
         raise B3DError("conv2d_dgrad: stride must be 1 or 2 (x_crop: stride 1 only)")
-    for cy, cx, rs, dy, dx, Ha, Wa in stride2_classes(kh, kw, pad_y, H, W):
-        if not rs:
-            dxo[:, cy::2, cx::2] = 0
-            continue
-        wt = torch.stack([weight[:, :, r, s].t() for r, s in rs]).contiguous()      # [taps][Cin][Cout]
-        check(_conv_call(lib.b3d_conv2d_tf32, ptr(g), ptr(wt), None, ptr(dxo), N, Hout, Wout, Cout, Ha, Wa, Cin, len(rs),
-                                  _ints(dy), _ints(dx), 1, 1, H, W, Cin, 2, 2, cy, cx, 1.0, None, 0, None, 0, 0, None, st))
-    return dxo
+    merged = _merge_parity_classes(classes)
+    opts = None
+    if g_pitch or mask is not None or merged:
+        opts = _ConvOpts(None, 1.0, 0, g_pitch, 0)
+        if mask is not None:
+            opts.mask, opts.mask_slope, opts.stats_sum_only = mask.data_ptr(), slope, 1
+        if merged:
+            opts.nclass = 4
+            for i, c in enumerate(classes):
+                opts.class_ooy[i], opts.class_oox[i] = c[0], c[1]
+    optr = ctypes.cast(ctypes.pointer(opts), ctypes.c_void_p) if opts is not None else None
+    gx = torch.empty(N, H, W, Cin, device=gy.device, dtype=torch.float32)
+    gptr, st = ctypes.c_void_p(gy.data_ptr()), stream_ptr(gy)      # (a pitched view's data_ptr = its first interior pixel)
+
+    def launch(Ha, Wa, dy, dx, osy, ooy, oox, taps):
+        check(_conv_call(lib.b3d_conv2d_tf32, gptr, ptr(wd), None, ptr(gx), N, Hout, Wout, Cop, Ha, Wa, Cin, len(dy), _ints(dy),
+                         _ints(dx), 1, 1, H, W, Cin, osy, osy, ooy, oox, 1.0, _ints(taps) if taps else None,
+                         kh * kw if taps else 0, ptr(sums), 0, 0, optr, st))
+
+    if stride == 1:
+        launch(H, W, [pad_y - r for r in range(kh) for _ in range(kw)], [-s - x_crop for _ in range(kh) for s in range(kw)],
+               1, 0, 0, None)
+    elif merged:
+        launch(classes[0][5], classes[0][6], [v for c in classes for v in c[3]], [v for c in classes for v in c[4]], 2, 0, 0,
+               [r * kw + s for c in classes for r, s in c[2]])
+    else:
+        for cy, cx, rs, dy, dx, Ha, Wa in classes:
+            if not rs:
+                gx[:, cy::2, cx::2] = 0
+                continue
+            launch(Ha, Wa, dy, dx, 2, cy, cx, [r * kw + s for r, s in rs])
+    return gx
+
+
+def _wgrad(gy, x, kh, kw, pad_y=0, stride=1, x_crop=0, sink=None, g_pitch=0):
+    """Weight gradient from gy [N,Hout,Wout,Cout] and the (x-padded) input x [N,H,W,Cin].
+    sink = None: returns a new [Cout,Cin,kh,kw] tensor (channel counts that are not multiples of 32 are zero-padded here);
+    otherwise the gradient is accumulated into sink, the bank's tap-major [kh*kw][Cout][Cin] buffer.
+    g_pitch > 0: gy is the interior of a padded gradient whose rows are g_pitch pixels apart, read in place."""
+    N, Hout, Wout, Cout = gy.shape
+    _, H, W, Cin = x.shape
+    tap_major = int(sink is not None)
+    st = stream_ptr(gy)
+    if _thin(Cout, Cin, kh, kw, stride):
+        dw = sink if tap_major else torch.zeros(Cout, Cin, kh, kw, device=gy.device, dtype=torch.float32)
+        check(_conv_call(lib.b3d_conv2d_thin_wgrad, ptr(gy), ptr(x), ptr(dw), N, H, W, Cin, Hout, Wout, Cout, kh, kw, pad_y,
+                         x_crop, tap_major, st))
+        return dw
+    if tap_major:
+        if Cout % 32:
+            raise B3DError(f"conv2d: tap-major weight gradient needs Cout % 32 == 0 or a thin head (Cout={Cout})")
+        dw = sink
+    else:
+        gy, x = _pad_last(gy, 32), _pad_last(x, 32)
+        dw = torch.zeros(gy.shape[3], x.shape[3], kh, kw, device=gy.device, dtype=torch.float32)
+    check(_conv_call(lib.b3d_conv2d_wgrad_tf32, ctypes.c_void_p(gy.data_ptr()), ptr(x), ptr(dw), N, H, W, x.shape[3], Hout, Wout,
+                     gy.shape[3], kh, kw, pad_y, stride, x_crop, tap_major, 0, g_pitch, st))
+    return dw if tap_major else dw[:Cout, :Cin]
+
+
+def conv2d_nhwc(x, weight, bias=None, pad_y=0, stride=1, leaky=1.0, wt=None, pad_out=0, pad_mode=1, x_crop=0):
+    """x [N,H,W,Cin] (Cin % 32 == 0), weight [Cout,Cin,kh,kw] -> [N,Hout,Wout,Cout]; zero pad along y only.
+    pad_out > 0: the result is written into the interior of a [N,Hout,Wout + 2*pad_out,Cout] buffer whose pad columns
+    are then filled in place (replicate / circular) — the next convolution's padded input without a copy.
+    x_crop > 0 (stride 1): convolve x[:, :, x_crop:W - x_crop] without materialising the slice (taps are shifted)."""
+    x = dev(x, "x")
+    Cout, Cin_w, kh, kw = weight.shape
+    if Cin_w != x.shape[3]:
+        raise B3DError(f"conv2d: input has {x.shape[3]} channels, weight expects {Cin_w}")
+    wt = dev(wt if wt is not None else taps_layout(weight), "weight")
+    return _fprop(x, wt, bias, kh, kw, pad_y, stride, leaky, pad_out, pad_mode, x_crop)
+
+
+def conv2d_dgrad_nhwc(dy_, weight, in_hw, pad_y=0, stride=1, x_crop=0):
+    """Gradient w.r.t. the (x-padded) input [N,H,W,Cin] of conv2d_nhwc, from dy_ [N,Hout,Wout,Cout]."""
+    Cout, Cin, kh, kw = weight.shape
+    wd = _d_layout(weight.permute(2, 3, 0, 1).reshape(kh * kw, Cout, Cin))
+    return _dgrad(dev(dy_, "grad_output"), wd, in_hw, kh, kw, pad_y, stride, x_crop)
 
 
 def conv2d_wgrad_nhwc(dy_, x, kh, kw, pad_y=0, stride=1, x_crop=0):
     """dW [Cout,Cin,kh,kw] from dy_ [N,Hout,Wout,Cout] and the (x-padded) input x [N,H,W,Cin], both NHWC
     (channel counts that are not multiples of 32 are zero-padded here)."""
-    co_real, ci_real = dy_.shape[3], x.shape[3]
-    if _thin(co_real, ci_real, kh, kw, stride):
-        g, x = dev(dy_, "grad_output"), dev(x, "input")
-        N, Hout, Wout, _ = g.shape
-        dw = torch.zeros(co_real, ci_real, kh, kw, device=g.device, dtype=torch.float32)
-        check(_conv_call(lib.b3d_conv2d_thin_wgrad, ptr(g), ptr(x), ptr(dw), N, x.shape[1], x.shape[2], ci_real, Hout, Wout, co_real, kh, kw,
-                                        pad_y, x_crop, 0, stream_ptr(g)))
-        return dw
-    g, x = dev(_pad_last(dy_, 32), "grad_output"), dev(_pad_last(x, 32), "input")
-    N, Hout, Wout, Cout = g.shape
-    _, H, W, Cin = x.shape
-    dw = torch.zeros(Cout, Cin, kh, kw, device=g.device, dtype=torch.float32)
-    check(_conv_call(lib.b3d_conv2d_wgrad_tf32, ptr(g), ptr(x), ptr(dw), N, H, W, Cin, Hout, Wout, Cout, kh, kw, pad_y, stride,
-                                    x_crop, 0, 0, 0, stream_ptr(g)))
-    return dw if (co_real, ci_real) == (Cout, Cin) else dw[:co_real, :ci_real]
+    return _wgrad(dev(dy_, "grad_output"), dev(x, "input"), kh, kw, pad_y, stride, x_crop)
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# autograd: y = conv(x, w) + b on NHWC tensors; fprop / dgrad / wgrad all on the wgmma kernels
+# autograd: y = conv(x, w) + b on NHWC tensors for both entry points
 # ------------------------------------------------------------------------------------------------------------------
-def _pad_last(t, mult):
-    c = t.shape[-1]
-    return t if c % mult == 0 else torch.nn.functional.pad(t, (0, mult - c % mult))
-
-
-class _Conv2dNHWC(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, weight, bias, pad_y, stride, leaky=1.0, pad_out=0, pad_mode=1, x_crop=0):
-        """pad_out > 0 (needs Cout = 4 * power of two): also applies the NEXT layer's x padding — the result is
-        [N,Hout,Wout + 2*pad_out,Cout] — and the backward undoes padding, activation and bias in one fused pass."""
-        x = dev(x.detach(), "x")
-        w = weight.detach()
-        Cin = x.shape[3]
-        if Cin % 32:                                    # thin inputs (discriminator stems: 8 / 11 channels): zero-pad K
-            x = _pad_last(x, 32)
-            w = torch.nn.functional.pad(w, (0, 0, 0, 0, 0, x.shape[3] - Cin))
-        y = conv2d_nhwc(x, w, bias.detach() if bias is not None else None, pad_y=pad_y, stride=stride, leaky=leaky,
-                        pad_out=pad_out, pad_mode=pad_mode, x_crop=x_crop)
-        if leaky != 1.0 or pad_out:
-            ctx.save_for_backward(x, w, y)
-        else:
-            ctx.save_for_backward(x, w)
-        ctx.cfg = (pad_y, stride, Cin, bias is not None, leaky, pad_out, pad_mode, x_crop)
-        return y
-
-    @staticmethod
-    def backward(ctx, gy):
-        pad_y, stride, Cin, has_bias, leaky, pad_out, pad_mode, x_crop = ctx.cfg
-        gb = None
-        want_gb = has_bias and ctx.needs_input_grad[2]
-        if pad_out:                       # padding + LeakyReLU + bias gradient in one pass over the padded gradient
-            x, w, y = ctx.saved_tensors
-            gy = dev(gy, "grad_output")
-            N, Ho, OW, Co = y.shape
-            masked = torch.empty(N, Ho, OW - 2 * pad_out, Co, device=gy.device, dtype=torch.float32)
-            gb = torch.zeros(Co, device=gy.device, dtype=torch.float32) if want_gb else None
-            check(lib.b3d_pad_leaky_bias_bwd(ptr(gy), ptr(y), ptr(masked), ptr(gb), N * Ho, OW - 2 * pad_out, Co, pad_out,
-                                             pad_mode, float(leaky), stream_ptr(gy)))
-            gy = masked
-        elif leaky != 1.0:                # LeakyReLU was fused into the epilogue: mask the incoming gradient by sign(y)
-            x, w, y = ctx.saved_tensors
-            gy = dev(gy, "grad_output")
-            masked = torch.empty_like(gy)
-            check(lib.b3d_leaky_bwd(ptr(gy), ptr(y), ptr(masked), gy.numel(), float(leaky), stream_ptr(gy)))
-            gy = masked
-        else:
-            x, w = ctx.saved_tensors
-        Cout, _, kh, kw = w.shape
-        gy = dev(gy, "grad_output")
-        if gb is None and want_gb:
-            gb = gy.sum(dim=(0, 1, 2))
-        gyp, wp = gy, w
-        if Cout % 32:                                   # heads with 1 / 3 output channels: zero-pad the reduction dim
-            gyp = _pad_last(gy, 32)
-            wp = torch.nn.functional.pad(w, (0, 0, 0, 0, 0, 0, 0, gyp.shape[3] - Cout))
-        gx = gw = None
-        if ctx.needs_input_grad[0]:
-            gx = conv2d_dgrad_nhwc(gyp, wp, (x.shape[1], x.shape[2]), pad_y=pad_y, stride=stride, x_crop=x_crop)[..., :Cin]
-        if ctx.needs_input_grad[1]:
-            gw = conv2d_wgrad_nhwc(gy if _thin(Cout, x.shape[3], kh, kw, stride) else gyp, x, kh, kw, pad_y=pad_y,
-                                   stride=stride, x_crop=x_crop)[:Cout, :Cin]
-        return gx, gw, gb, None, None, None, None, None, None
-
-
-def fold_kh_weight(weight, cpad=0):
-    """[Cout,Cin,kh,kw] -> [Cout, kh*Cin + cpad, 1, kw] matching fold_rows: channel r*Cin + c of the folded input is
-    row tap r of input channel c (pure torch; unit-tested on the CPU against the unfolded convolution)."""
-    Cout, Cin, kh, kw = weight.shape
-    w = weight.permute(0, 2, 1, 3).reshape(Cout, kh * Cin, 1, kw)
-    return torch.nn.functional.pad(w, (0, 0, 0, 0, 0, cpad)) if cpad else w
-
-
-def conv2d(x_nchw, weight, bias=None, pad_y=0, stride=1, leaky=1.0, pad_out=0, pad_mode=1, x_crop=0):
-    """Drop-in for F.conv2d(x, w, b, stride, padding=(pad_y, 0)) on logically-NCHW tensors: runs on the wgmma
-    kernels over the channels-last storage (a no-copy view when x is already channels_last) and returns a
-    logically-NCHW, channels-last tensor."""
-    x = x_nchw.permute(0, 2, 3, 1)
-    Cout, Cin, kh, kw = weight.shape
-    if stride == 1 and kh > 1 and Cin * kh <= 64:
-        # thin stems (discriminator conv1: 8 or 11 input channels, 5x5): fold the kh vertical taps into the channel
-        # dimension — X'[n,y,x, r*Cin + c] = X[n, y+r-pad_y, x, c] (zero rows = the y padding) — so the tensor cores see
-        # kw taps of kh*Cin real channels instead of kh*kw taps of Cin channels zero-padded to 32.  The remaining taps
-        # are horizontal: the weight-gradient kernel covers a whole row of taps per CTA (one pass over dY and X').
-        from .ew import fold_rows
-        cpad = (-kh * Cin) % 32                            # ... and round up to the 32-channel K slice in the same pass
-        x = fold_rows(x, kh, pad_y, kh * Cin + cpad)
-        weight = fold_kh_weight(weight, cpad)
-        pad_y = 0
-    y = _Conv2dNHWC.apply(x, weight, bias, int(pad_y), int(stride), float(leaky), int(pad_out), int(pad_mode), int(x_crop))
-    return y.permute(0, 3, 1, 2)
-
-
-# ------------------------------------------------------------------------------------------------------------------
-# Banked convolution: the weights arrive from b3d.bank.WeightBank already normalised and laid out for the kernels
-# (F [T'][Cout][Cin'] for fprop, D [T'][Cin'][Cout'] for the input gradient); the weight gradient is accumulated
-# straight into the bank's F-layout gradient sink.  No per-call permute / contiguous / zeros.
-# ------------------------------------------------------------------------------------------------------------------
-class _ConvOpts(ctypes.Structure):
-    """b3d_conv_opts (include/b3d.h)."""
-    _fields_ = [("mask", ctypes.c_void_p), ("mask_slope", ctypes.c_float), ("stats_sum_only", ctypes.c_int),
-                ("x_row_pitch", ctypes.c_int), ("nclass", ctypes.c_int), ("class_ooy", ctypes.c_int * 4), ("class_oox", ctypes.c_int * 4)]
-
-
 class ActLink:
     """Hand-over between two chained banked convolutions  conv_L -> bias -> LeakyReLU -> x padding -> conv_L+1  (the
     discriminators, models/gan.py:163-177,294-302) for the backward pass.  The producer (conv_L, `link_out`) records its
@@ -257,67 +231,40 @@ class ActLink:
         self.gb = None
 
 
-def _merge_parity_classes(classes):
-    """One launch for the four parity classes of a stride-2 input gradient when they have the same extent and tap count
-    (even H, W; 4x4 kernels); otherwise one launch per class."""
-    return len(classes) == 4 and all(c[2] for c in classes) and len({(len(c[2]), c[5], c[6]) for c in classes}) == 1
-
-
-class _ConvBanked(torch.autograd.Function):
+class _Conv(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, wf, bias, lw, pad_y, stride, leaky, pad_out, pad_mode, x_crop, stats=None, fold_raw=0, link_in=None,
+    def forward(ctx, x, w, bias, lw, pad_y, stride, leaky, pad_out, pad_mode, x_crop, stats=None, fold_raw=0, link_in=None,
                 link_out=None):
-        """fold_raw = kh > 0: x is the RAW 8-channel stem input [N,H,W,8]; the kernels fold the kh vertical taps into the K
+        """Runs on lw.wf (F [T'][Cout][Cin']); w is the tensor autograd differentiates: lw.wf itself (bank) or the module weight
+        lw.wf was laid out from.  Its gradient is accumulated into lw.df when the bank provides that sink, otherwise returned
+        as [Cout,Cin,kh,kw].  The input gradient runs on lw.wd, or on the per-tap transpose of lw.wf when there is none.
+        fold_raw = kh > 0: x is the RAW 8-channel stem input [N,H,W,8]; the kernels fold the kh vertical taps into the K
         dimension on the fly (TMA boxes of 4 rows x 8 channels) — the folded tensor never exists (pad_y = the fold's y padding)."""
         x = dev(x.detach(), "x")
-        N, H, W, Cx = x.shape
+        Cx = x.shape[3]
         fold_pad = 0
         if fold_raw:
             if not lw.fold or Cx != 8 or lw.Cin != 8 or stride != 1 or x_crop:
-                raise B3DError("banked conv: on-the-fly fold needs a folded 8-channel stride-1 stem")
+                raise B3DError("conv2d: on-the-fly fold needs a folded 8-channel stride-1 stem")
             fold_pad = pad_y
         elif Cx != lw.Cinp:
-            if lw.fold or Cx > lw.Cinp:
-                raise B3DError(f"banked conv: input has {Cx} channels, the layer expects {lw.Cinp}")
-            x = _pad_last(x, 32)                                      # thin un-folded inputs (512^2 stem): zero-pad K
+            if lw.fold or Cx != lw.Cin:
+                raise B3DError(f"conv2d: input has {Cx} channels, the layer expects {lw.Cinp if lw.fold else lw.Cin}")
+            x = _pad_last(x, 32)                                      # thin un-folded inputs (stems): zero-pad K
         kh, kw = (1, lw.kw) if lw.fold else (lw.kh, lw.kw)
         if lw.fold:
             pad_y = 0
-        Cout, Cin = lw.Cout, lw.Cinp
-        wt = dev(wf.detach(), "weight")
-        b = dev(bias.detach(), "bias") if bias is not None else None
-        Hout = (H + 2 * fold_pad - lw.kh + 1) if fold_raw else (H + 2 * pad_y - kh) // stride + 1
-        if x_crop and stride != 1:
-            raise B3DError("conv2d: x_crop needs stride 1")
-        Wout = (W - 2 * x_crop - kw) // stride + 1
-        OW = Wout + 2 * pad_out
-        if pad_out and Cout % 4:
-            raise B3DError("conv2d: pad_out needs Cout % 4 == 0")
-        out = torch.empty(N, Hout, OW, Cout, device=x.device, dtype=torch.float32)
-        optr = ctypes.c_void_p(out.data_ptr() + 4 * pad_out * Cout)
-        st = stream_ptr(x)
-        thin = _thin(Cout, Cin, kh, kw, stride)
-        if thin:
-            check(_conv_call(lib.b3d_conv2d_thin_fwd, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh, kw, pad_y,
-                             x_crop, OW, Cout, float(leaky), st))
-        else:
-            dy = [r - pad_y for r in range(kh) for _ in range(kw)]
-            dx = [s + x_crop for _ in range(kh) for s in range(kw)]
-            if stats is not None and (bias is not None or leaky != 1.0 or stride != 1):
-                raise B3DError("banked conv: output statistics are taken before bias / activation (plain stride-1 convs only)")
-            check(_conv_call(lib.b3d_conv2d_tf32, ptr(x), ptr(wt), ptr(b), optr, N, H, W, Cin, Hout, Wout, Cout, kh * kw,
-                             _ints(dy), _ints(dx), stride, stride, Hout, OW, Cout, 1, 1, 0, 0, float(leaky), None, 0, ptr(stats),
-                             fold_raw, fold_pad, None, st))
-        if pad_out:
-            check(lib.b3d_wrap_x_inplace(ptr(out), N * Hout, Wout, Cout, pad_out, pad_mode, st))
+        out = _fprop(x, dev(lw.wf.detach(), "weight"), bias.detach() if bias is not None else None, kh, kw, pad_y, stride,
+                     leaky, pad_out, pad_mode, x_crop, stats, fold_raw, fold_pad)
         ctx.save_for_backward(x, out if (leaky != 1.0 or pad_out) else None)
         ctx.lw = lw
-        ctx.cfg = (pad_y, stride, Cx, bias is not None, leaky, pad_out, pad_mode, x_crop, kh, kw, thin, fold_raw, fold_pad)
+        ctx.cfg = (pad_y, stride, Cx, bias is not None, leaky, pad_out, pad_mode, x_crop, kh, kw, fold_raw, fold_pad)
+        thin = _thin(lw.Cout, lw.Cinp, kh, kw, stride)
         # chained activation adjoint (ActLink): usable as a consumer when x is exactly the producer's padded output
         ctx.link_in = link_in if (link_in is not None and link_in.armed and link_in.ptr == x.data_ptr() and link_in.shape == tuple(x.shape)
-                                  and Cx == Cin and Cin % 32 == 0 and not fold_raw and not thin) else None
+                                  and Cx == lw.Cinp and lw.Cinp % 32 == 0 and not fold_raw and not thin) else None
         ctx.link_out = None
-        if link_out is not None and pad_out and leaky != 1.0 and Cout % 32 == 0 and not thin:
+        if link_out is not None and pad_out and leaky != 1.0 and lw.Cout % 32 == 0 and not thin:
             link_out.armed, link_out.slope, link_out.pad, link_out.mode = True, float(leaky), int(pad_out), int(pad_mode)
             link_out.ptr, link_out.shape, link_out.done = out.data_ptr(), tuple(out.shape), False
             link_out.want_gb = bias is not None and bool(ctx.needs_input_grad[2])     # frozen discriminator (generator step): no bias sums
@@ -328,119 +275,101 @@ class _ConvBanked(torch.autograd.Function):
     def backward(ctx, gy):
         x, y = ctx.saved_tensors
         lw = ctx.lw
-        pad_y, stride, Cx, has_bias, leaky, pad_out, pad_mode, x_crop, kh, kw, thin, fold_raw, fold_pad = ctx.cfg
+        pad_y, stride, Cx, has_bias, leaky, pad_out, pad_mode, x_crop, kh, kw, fold_raw, fold_pad = ctx.cfg
         Cout, Cin = lw.Cout, lw.Cinp
         N, H, W, _ = x.shape
         gy = dev(gy, "grad_output")
         st = stream_ptr(gy)
         gb = None
         want_gb = has_bias and ctx.needs_input_grad[2]
-        g_pitch, g_off = 0, 0                                          # gy as a window of wider rows (pixels): pitch, first column
+        g_pitch = 0                                                    # gy as a window of wider rows (pixels)
         link_out = ctx.link_out
         if link_out is not None and link_out.done:
             # the consumer's input-gradient epilogue already applied LeakyReLU', folded the pad columns and summed the bias
             # gradient: gy is the PADDED gradient [N,Ho,Wo + 2 pad,C]; its interior is read in place
             link_out.done = False
             if tuple(gy.shape) != tuple(y.shape):
-                raise B3DError("banked conv: chained gradient has the wrong shape")
-            g_pitch, g_off = y.shape[2], pad_out
+                raise B3DError("conv2d: chained gradient has the wrong shape")
+            g_pitch = y.shape[2]
             gb = link_out.gb if want_gb else None
             link_out.gb = None
             gy = gy[:, :, pad_out:y.shape[2] - pad_out]                # a view: shapes below are the interior's
-        elif pad_out:
+        elif pad_out:                     # padding + LeakyReLU + bias gradient in one pass over the padded gradient
             _, Ho, OW, _ = y.shape
             masked = torch.empty(N, Ho, OW - 2 * pad_out, Cout, device=gy.device, dtype=torch.float32)
             gb = torch.zeros(Cout, device=gy.device, dtype=torch.float32) if want_gb else None
             check(lib.b3d_pad_leaky_bias_bwd(ptr(gy), ptr(y), ptr(masked), ptr(gb), N * Ho, OW - 2 * pad_out, Cout, pad_out,
                                              pad_mode, float(leaky), st))
             gy = masked
-        elif leaky != 1.0:
+        elif leaky != 1.0:                # LeakyReLU was fused into the epilogue: mask the incoming gradient by sign(y)
             masked = torch.empty_like(gy)
             check(lib.b3d_leaky_bwd(ptr(gy), ptr(y), ptr(masked), gy.numel(), float(leaky), st))
             gy = masked
         if gb is None and want_gb:
             gb = gy.sum(dim=(0, 1, 2))
-        _, Hout, Wout, _ = gy.shape
         gx = gw = None
         if ctx.needs_input_grad[0]:
-            if lw.wd is None:
-                raise B3DError("banked conv: this layer was registered without an input gradient (no_dgrad)")
-            gyp = gy if g_pitch else _pad_last(gy, 32)                 # heads with 1 / 3 output channels: zero-pad K
-            gptr = ctypes.c_void_p(gy.data_ptr()) if g_pitch else ptr(gyp)     # (the view's data_ptr = first interior pixel)
-            Cop = lw.Coutp
-            Hraw = H
-            if fold_raw:
-                H = Hout                                               # gradient w.r.t. the (virtual) folded tensor [N, Hout, W, Cin]
-            gx = torch.empty(N, H, W, Cin, device=gy.device, dtype=torch.float32)
-            wd = lw.wd
-            link_in = ctx.link_in if (stride == 1 or (stride == 2 and not x_crop)) else None
-            opts, sums = None, None
-            classes = stride2_classes(kh, kw, pad_y, H, W) if (stride == 2 and not x_crop) else []
-            merged = _merge_parity_classes(classes)
-            if g_pitch or link_in is not None or merged:
-                opts = _ConvOpts(None, 1.0, 0, g_pitch, 0)
-                if link_in is not None:                                # LeakyReLU adjoint of the PRODUCER of x in this epilogue
-                    if link_in.want_gb:
-                        sums = torch.zeros(2 * Cin, device=gy.device, dtype=torch.float64)
-                    opts.mask, opts.mask_slope, opts.stats_sum_only = x.data_ptr(), link_in.slope, 1
-            optr_ = ctypes.cast(ctypes.pointer(opts), ctypes.c_void_p) if opts is not None else None
-            if stride == 1:
-                dy = [pad_y - r for r in range(kh) for _ in range(kw)]
-                dx = [-s - x_crop for _ in range(kh) for s in range(kw)]
-                check(_conv_call(lib.b3d_conv2d_tf32, gptr, ptr(wd), None, ptr(gx), N, Hout, Wout, Cop, H, W, Cin, kh * kw,
-                                 _ints(dy), _ints(dx), 1, 1, H, W, Cin, 1, 1, 0, 0, 1.0, None, 0, ptr(sums), 0, 0, optr_, st))
-            elif merged:
-                opts.nclass = 4
-                for i, c in enumerate(classes):
-                    opts.class_ooy[i], opts.class_oox[i] = c[0], c[1]
-                dy = [v for c in classes for v in c[3]]
-                dx = [v for c in classes for v in c[4]]
-                taps = [r * kw + s for c in classes for r, s in c[2]]   # rows of the tap-major D array: no gathered copy
-                check(_conv_call(lib.b3d_conv2d_tf32, gptr, ptr(wd), None, ptr(gx), N, Hout, Wout, Cop, classes[0][5], classes[0][6], Cin,
-                                 len(taps), _ints(dy), _ints(dx), 1, 1, H, W, Cin, 2, 2, 0, 0, 1.0, _ints(taps), kh * kw,
-                                 ptr(sums), 0, 0, optr_, st))
-            elif stride == 2 and not x_crop:
-                for cy, cx, rs, dy, dx, Ha, Wa in classes:
-                    if not rs:
-                        gx[:, cy::2, cx::2] = 0
-                        continue
-                    taps = [r * kw + s for r, s in rs]                  # rows of the tap-major D array: no gathered copy
-                    check(_conv_call(lib.b3d_conv2d_tf32, gptr, ptr(wd), None, ptr(gx), N, Hout, Wout, Cop, Ha, Wa, Cin,
-                                     len(rs), _ints(dy), _ints(dx), 1, 1, H, W, Cin, 2, 2, cy, cx, 1.0, _ints(taps), kh * kw,
-                                     ptr(sums), 0, 0, optr_, st))
-            else:
-                raise B3DError("conv2d_dgrad: stride must be 1 or 2 (x_crop: stride 1 only)")
+            link_in = ctx.link_in             # LeakyReLU adjoint of the PRODUCER of x in this epilogue
+            sums = torch.zeros(2 * Cin, device=gy.device, dtype=torch.float64) if link_in is not None and link_in.want_gb else None
+            gx = _dgrad(gy, lw.wd if lw.wd is not None else _d_layout(lw.wf.detach()), (gy.shape[1] if fold_raw else H, W), kh,
+                        kw, pad_y, stride, x_crop, g_pitch, x if link_in is not None else None,
+                        link_in.slope if link_in is not None else 1.0, sums)
             if link_in is not None:
                 # gx = LeakyReLU'(x) * d(padded input), pad columns included: fold them back, hand the bias gradient over
                 check(lib.b3d_wrap_x_bwd_inplace(ptr(gx), N * H, W - 2 * link_in.pad, Cin, link_in.pad, link_in.mode, st))
                 link_in.gb = sums[:Cin].float() if sums is not None else None
                 link_in.done = True
             if fold_raw:                                               # adjoint of the fold: back to the raw 8-channel layout
-                graw = torch.empty(N, Hraw, W, Cx, device=gy.device, dtype=torch.float32)
-                check(lib.b3d_fold_rows_bwd(ptr(gx), ptr(graw), N, Hraw, W, Cx, lw.kh, fold_pad, Cin, st))
-                gx, H = graw, Hraw
+                graw = torch.empty(N, H, W, Cx, device=gy.device, dtype=torch.float32)
+                check(lib.b3d_fold_rows_bwd(ptr(gx), ptr(graw), N, H, W, Cx, lw.kh, fold_pad, Cin, st))
+                gx = graw
             elif Cx != Cin:
                 gx = gx[..., :Cx]
         if ctx.needs_input_grad[1]:
-            gw = lw.df                                                 # the bank's gradient sink (zeroed by the bank)
-            if gw is None:
-                raise B3DError("banked conv: weight gradient requested but the bank was run without gradients")
-            if thin:
-                check(_conv_call(lib.b3d_conv2d_thin_wgrad, ptr(gy), ptr(x), ptr(gw), N, H, W, Cin, Hout, Wout, Cout, kh, kw, pad_y,
-                                 x_crop, 1, st))
-            else:
-                if Cout % 32:
-                    raise B3DError(f"banked conv: weight gradient needs Cout % 32 == 0 or a thin head (Cout={Cout})")
-                if fold_raw:
-                    raise B3DError("banked conv: the on-the-fly fold has no weight-gradient kernel (materialise the fold)")
-                check(_conv_call(lib.b3d_conv2d_wgrad_tf32, ctypes.c_void_p(gy.data_ptr()), ptr(x), ptr(gw), N, H, W, Cin, Hout, Wout,
-                                 Cout, kh, kw, pad_y, stride, x_crop, 1, 0, g_pitch, st))
+            if fold_raw:
+                raise B3DError("conv2d: the on-the-fly fold has no weight-gradient kernel (materialise the fold)")
+            gw = _wgrad(gy, x, kh, kw, pad_y, stride, x_crop, lw.df, g_pitch)
+            if lw.df is None:
+                gw = gw[:, :lw.Cin]                                    # the module weight: drop the zero-padded input channels
         return gx, gw, gb, None, None, None, None, None, None, None, None, None, None, None
 
 
+def fold_kh_weight(weight, cpad=0):
+    """[Cout,Cin,kh,kw] -> [Cout, kh*Cin + cpad, 1, kw] matching fold_rows: channel r*Cin + c of the folded input is
+    row tap r of input channel c (pure torch; unit-tested on the CPU against the unfolded convolution)."""
+    Cout, Cin, kh, kw = weight.shape
+    w = weight.permute(0, 2, 1, 3).reshape(Cout, kh * Cin, 1, kw)
+    return torch.nn.functional.pad(w, (0, 0, 0, 0, 0, cpad)) if cpad else w
+
+
+def conv2d(x_nchw, weight, bias=None, pad_y=0, stride=1, leaky=1.0, pad_out=0, pad_mode=1, x_crop=0):
+    """Drop-in for F.conv2d(x, w, b, stride, padding=(pad_y, 0)) on logically-NCHW tensors: runs on the wgmma
+    kernels over the channels-last storage (a no-copy view when x is already channels_last) and returns a
+    logically-NCHW, channels-last tensor.  The weight is laid out per call and used as stored (fp32, no tf32 rounding)."""
+    x = x_nchw.permute(0, 2, 3, 1)
+    Cout, Cin, kh, kw = weight.shape
+    if stride == 1 and kh > 1 and Cin * kh <= 64:
+        # thin stems (discriminator conv1: 8 or 11 input channels, 5x5): fold the kh vertical taps into the channel
+        # dimension — X'[n,y,x, r*Cin + c] = X[n, y+r-pad_y, x, c] (zero rows = the y padding) — so the tensor cores see
+        # kw taps of kh*Cin real channels instead of kh*kw taps of Cin channels zero-padded to 32.  The remaining taps
+        # are horizontal: the weight-gradient kernel covers a whole row of taps per CTA (one pass over dY and X').
+        from .ew import fold_rows
+        cpad = (-kh * Cin) % 32                            # ... and round up to the 32-channel K slice in the same pass
+        x = fold_rows(x, kh, pad_y, kh * Cin + cpad)
+        weight = fold_kh_weight(weight, cpad)
+        Cout, Cin, kh, kw = weight.shape
+        pad_y = 0
+    lw = LayerWeights(dict(Cout=Cout, Cin=Cin, kh=kh, kw=kw, fold=0, Cinp=-(-Cin // 32) * 32, Coutp=-(-Cout // 32) * 32,
+                           Tp=kh * kw))
+    lw.wf = _pad_last(taps_layout(weight.detach()), 32)
+    y = _Conv.apply(x, weight, bias, lw, int(pad_y), int(stride), float(leaky), int(pad_out), int(pad_mode), int(x_crop))
+    return y.permute(0, 3, 1, 2)
+
+
 def conv2d_banked(x_nchw, lw, pad_y=0, stride=1, leaky=1.0, pad_out=0, pad_mode=1, x_crop=0, stats=None, link_in=None, link_out=None):
-    """conv2d for a layer whose weights come from a WeightBank (`lw` = its LayerWeights).  Thin stems registered with
-    fold=True get their kh taps folded into the channels here (b3d.ew.fold_rows), as in conv2d().
+    """conv2d for a layer whose weights come from a WeightBank (`lw` = its LayerWeights: F and D normalised and laid out
+    for the kernels once per network forward, the weight gradient accumulated straight into the bank's F-layout sink).
+    Thin stems registered with fold=True get their kh taps folded into the channels here (b3d.ew.fold_rows), as in conv2d().
     stats: optional zeroed fp64 tensor [2*Cout]; the conv epilogue accumulates the output's per-channel sum / sum of
     squares into it (the following batch norm's statistics without another pass over the tensor)."""
     x = x_nchw.permute(0, 2, 3, 1)
@@ -456,6 +385,6 @@ def conv2d_banked(x_nchw, lw, pad_y=0, stride=1, leaky=1.0, pad_out=0, pad_mode=
         else:
             from .ew import fold_rows
             x = fold_rows(x, lw.kh, pad_y, lw.Cinp)
-    y = _ConvBanked.apply(x, lw.wf, lw.bias, lw, int(pad_y), int(stride), float(leaky), int(pad_out), int(pad_mode), int(x_crop), stats,
-                          fold_raw, link_in, link_out)
+    y = _Conv.apply(x, lw.wf, lw.bias, lw, int(pad_y), int(stride), float(leaky), int(pad_out), int(pad_mode), int(x_crop), stats,
+                    fold_raw, link_in, link_out)
     return y.permute(0, 3, 1, 2)

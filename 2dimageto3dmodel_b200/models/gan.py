@@ -69,12 +69,11 @@ def _conv_norm_act(conv, norm, x, pad_next=0, lw=None, link_in=None, link_out=No
     padded output / this layer's padded output has exactly one consumer, the next convolution — the backward pass then
     applies LeakyReLU', the padding's adjoint and the bias sum in the consumer's input-gradient epilogue."""
     if lw is not None:
-        run = lambda **kw: conv2d_banked(x, lw, pad_y=conv.padding[0], stride=conv.stride[0], link_in=link_in, **kw)
+        run = lambda **kw: conv2d_banked(x, lw, pad_y=conv.padding[0], stride=conv.stride[0], link_in=link_in,
+                                         link_out=link_out, **kw)
     else:
         run = lambda **kw: conv(x, **kw)
     if norm is None and conv.out_channels in (16, 32, 64, 128, 256, 512, 1024):
-        if lw is not None and pad_next:
-            return run(leaky=0.2, pad_out=pad_next, pad_mode=CIRCULAR, link_out=link_out)
         return run(leaky=0.2, pad_out=pad_next, pad_mode=CIRCULAR)
     y = run(leaky=0.2) if norm is None else F.leaky_relu(norm(run()), 0.2)
     return pad_x(y, pad_next, CIRCULAR) if pad_next else y

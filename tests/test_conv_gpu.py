@@ -115,6 +115,40 @@ def test_conv2d_autograd_matches_torch(N, Cin, H, W, Cout, k, pad_y, stride, bia
         assert float((a - r).abs().max()) <= TOL * float(r.abs().max()), (a.shape, float((a - r).abs().max()), float(r.abs().max()))
 
 
+@pytest.mark.parametrize("N,Cin,H,W,Cout,k,pad_y,stride", [
+    (2, 64, 16, 18, 128, 3, 1, 1),      # 3x3 stride 1
+    (2, 64, 16, 18, 128, 4, 1, 2),      # 4x4 stride 2 on an even-sized input: one launch over the four parity classes
+    (2, 256, 12, 16, 1, 5, 2, 1),       # 1-channel 5x5 head (CUDA-core thin kernels for fprop / wgrad)
+])
+def test_module_and_bank_entries_agree(N, Cin, H, W, Cout, k, pad_y, stride):
+    """One plain TCConv2d through conv2d (per-call layouts of the module weight) and through conv2d_banked (WeightBank
+    layouts without tf32 rounding): the same kernels on the same fp32 weights, so forward outputs, input and bias gradients
+    are bitwise equal; weight gradients differ only by the order of the split-K fp32 atomics."""
+    from b3d.bank import WeightBank
+    from b3d.conv import conv2d, conv2d_banked
+    from models.gan import TCConv2d
+    torch.manual_seed(Cin + Cout + k)
+    conv = TCConv2d(Cin, Cout, k, padding=(pad_y, 0), stride=stride).cuda()
+    x0 = torch.randn(N, Cin, H, W, device="cuda").contiguous(memory_format=torch.channels_last)
+    gy = None
+    res = []
+    for banked in (False, True):
+        conv.zero_grad()
+        x = x0.detach().clone().requires_grad_(True)
+        if banked:
+            y = conv2d_banked(x, WeightBank({"c": conv}, round_tf32=False).forward(True)["c"], pad_y=pad_y, stride=stride)
+        else:
+            y = conv2d(x, conv.weight, conv.bias, pad_y, stride)
+        if gy is None:
+            gy = torch.randn(y.shape, generator=torch.Generator().manual_seed(3)).cuda()
+        y.backward(gy)
+        res.append((y.detach(), x.grad, conv.bias.grad.clone(), conv.weight.grad.clone()))
+    torch.cuda.synchronize()
+    (ym, gxm, gbm, gwm), (yb, gxb, gbb, gwb) = res
+    assert torch.equal(ym, yb) and torch.equal(gxm, gxb) and torch.equal(gbm, gbb)
+    assert float((gwm - gwb).abs().max()) <= 1e-5 * float(gwm.abs().max())
+
+
 @pytest.mark.parametrize("mode", ["replicate", "circular"])
 @pytest.mark.parametrize("N,C,H,W,a", [(2, 8, 5, 7, 2), (3, 64, 16, 4, 1), (1, 12, 3, 9, 2)])
 def test_pad_x_matches_torch(mode, N, C, H, W, a):

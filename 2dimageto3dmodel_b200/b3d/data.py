@@ -2,7 +2,8 @@
 b3d_gather_fields: one launch that assembles a GAN batch from packed per-record stores (gather by index, fp16 -> fp32, UV
 mirroring).  The stores may sit in device memory or in pinned host memory (read over PCIe).
 b3d_image_batch: one launch that builds a reconstruction batch (crop, cv2-style resize, mirror, poses) from packed photo
-windows in device memory."""
+windows in device memory.
+b3d_pseudogt_pack: one launch that masks, transposes and rounds a batch of pseudo-ground-truth records to fp16."""
 import ctypes
 
 import torch
@@ -110,3 +111,32 @@ def image_batch(pixels, offsets, geometry, poses, idx, flip, images, scale, tran
     check(lib.b3d_image_batch(ptr(pixels), ptr(offsets), ptr(geometry), ptr(poses), n, ptr(idx), ptr(flip), B, len(res),
                               ctypes.cast(res_arr, ctypes.c_void_p), ctypes.cast(img_arr, ctypes.c_void_p), ptr(scale),
                               ptr(translation), ptr(rot), ptr(ind), stream_ptr(idx)))
+
+
+def pseudogt_pack(vis, tex, alpha, image, tex_out, alpha_out, image_out):
+    """b3d_pseudogt_pack: one launch turns a batch of inverse renders into pseudo-ground-truth planes.
+    vis uint8 [B,Th,Tw] (texel visibility), tex fp32 [B,R,R,C], alpha fp32 [B,R,R,1], image fp32 [B,Ci,h,w] -> tex_out fp16
+    [B,C,R,R], alpha_out fp16 [B,1,R,R], image_out fp16 [B,Ci,h,w]: visibility mask resized to R with F.interpolate's
+    bilinear taps (align_corners=False), texture and alpha masked, every plane rounded as .half() rounds.  All tensors
+    contiguous on the device."""
+    def need(t, dtype, name, dim):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dtype and t.is_contiguous() and t.dim() == dim):
+            raise B3DError(f"pseudogt_pack: {name} must be a contiguous {dtype} CUDA tensor with {dim} dimensions")
+    need(vis, torch.uint8, 'vis', 3)
+    need(tex, torch.float32, 'tex', 4)
+    need(alpha, torch.float32, 'alpha', 4)
+    need(image, torch.float32, 'image', 4)
+    B, Th, Tw = vis.shape
+    R, C = tex.shape[1], tex.shape[3]
+    Ci, h, w = image.shape[1:]
+    expect = {'tex': (tex, (B, R, R, C)), 'alpha': (alpha, (B, R, R, 1)), 'image': (image, (B, Ci, h, w))}
+    for name, (t, shape) in expect.items():
+        if tuple(t.shape) != shape:
+            raise B3DError(f"pseudogt_pack: {name} has shape {tuple(t.shape)}; expected {list(shape)}")
+    for name, t, shape in (('tex_out', tex_out, (B, C, R, R)), ('alpha_out', alpha_out, (B, 1, R, R)),
+                           ('image_out', image_out, (B, Ci, h, w))):
+        need(t, torch.float16, name, 4)
+        if tuple(t.shape) != shape:
+            raise B3DError(f"pseudogt_pack: {name} has shape {tuple(t.shape)}; expected {list(shape)}")
+    check(lib.b3d_pseudogt_pack(ptr(vis), Th, Tw, ptr(tex), ptr(alpha), B, R, C, ptr(image), Ci, h, w, ptr(tex_out),
+                                ptr(alpha_out), ptr(image_out), stream_ptr(vis)))

@@ -117,6 +117,61 @@ def render(verts, faces, uv, texture, ft=None, background=None, H=256, W=256):
     return _Render.apply(verts, uv, texture, faces, ft, background, int(H), int(W))
 
 
+@torch.no_grad()
+def render_indices(verts, faces, uv, ft, H, W, out=None):
+    """Unshaded forward render (no texture): -> (imidx [B,H,W] int32, imwei [B,H,W,3], fuv [B,F,6]), the inputs of
+    `texel_visibility`.  out: optional (imidx, imwei, imout, improb) buffers of at least B samples, reused across calls
+    (imout [B,H,W,3] and improb [B,H,W,1] are written but not returned)."""
+    fgeo, fuv, _ = face_setup(verts, faces, uv, ft, want_normals=False)
+    B, F = fgeo.shape[0], fgeo.shape[1]
+    d = fgeo.device
+    if out is None:
+        out = (torch.empty(B, H, W, device=d, dtype=torch.int32), torch.empty(B, H, W, 3, device=d),
+               torch.empty(B, H, W, 3, device=d), torch.empty(B, H, W, 1, device=d))
+    shapes = ((H, W), (H, W, 3), (H, W, 3), (H, W, 1))
+    dtypes = (torch.int32, torch.float32, torch.float32, torch.float32)
+    for t, s, dt in zip(out, shapes, dtypes):
+        if not (t.is_cuda and t.dtype == dt and t.is_contiguous() and t.shape[0] >= B and tuple(t.shape[1:]) == s):
+            raise B3DError(f"render_indices: buffer {tuple(t.shape)} {t.dtype} cannot hold [{B},{','.join(map(str, s))}] {dt}")
+    imidx, imwei, imout, improb = (t[:B] for t in out)
+    check(lib.b3d_mesh_render_fwd(ptr(fgeo), ptr(fuv), None, None, B, F, H, W, 0, 0, ptr(imidx), ptr(imwei), ptr(imout),
+                                  ptr(improb), stream_ptr(fgeo)))
+    return imidx, imwei, fuv
+
+
+def texel_visibility(imidx, imwei, fuv, Th, Tw, symmetric, out=None, words=None):
+    """Texels of the texture behind a forward render whose gradient d(render)/d(texture) with an all-ones upstream gradient
+    is > 0, computed from the render's index buffers (no adjoint, no float atomics).  Th x Tw: the padded texture the shader
+    samples (MeshTemplate.adjust_uv_and_texture); symmetric: circpad(., 1) seam (Tw - 2 columns out), else the appended
+    column 0 (Tw - 1 columns out).  -> uint8 [B, Th, Tw_out] of 0 / 1.  out / words: optional reusable buffers of at least B
+    samples (words: int32 [B, ceil(Th * Tw_out / 32)])."""
+    imidx = dev(imidx, "imidx", torch.int32)
+    imwei = dev(imwei, "imwei")
+    fuv = dev(fuv, "fuv")
+    B, H, W = imidx.shape
+    F = fuv.shape[1]
+    Tw_out = Tw - (2 if symmetric else 1)
+    if tuple(imwei.shape) != (B, H, W, 3) or fuv.dim() != 3 or tuple(fuv.shape) != (B, F, 6):
+        raise B3DError(f"texel_visibility: imidx {tuple(imidx.shape)}, imwei {tuple(imwei.shape)}, fuv {tuple(fuv.shape)}")
+    if Th < 2 or Tw_out < (2 if symmetric else 1):
+        raise B3DError(f"texel_visibility: bad padded texture size {Th} x {Tw}")
+    nwords = (Th * Tw_out + 31) // 32
+    if out is None:
+        out = torch.empty(B, Th, Tw_out, device=imidx.device, dtype=torch.uint8)
+    if words is None:
+        words = torch.empty(B, nwords, device=imidx.device, dtype=torch.int32)
+    if not (out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.shape[0] >= B
+            and tuple(out.shape[1:]) == (Th, Tw_out)):
+        raise B3DError(f"texel_visibility: out must be a contiguous uint8 CUDA tensor [>={B},{Th},{Tw_out}]")
+    if not (words.is_cuda and words.dtype == torch.int32 and words.is_contiguous() and words.shape[0] >= B
+            and tuple(words.shape[1:]) == (nwords,)):
+        raise B3DError(f"texel_visibility: words must be a contiguous int32 CUDA tensor [>={B},{nwords}]")
+    out = out[:B]
+    check(lib.b3d_texel_visibility(ptr(imidx), ptr(imwei), ptr(fuv), B, F, H, W, int(Th), int(Tw), int(bool(symmetric)),
+                                   ptr(words), ptr(out), stream_ptr(imidx)))
+    return out
+
+
 class _FaceNormals(torch.autograd.Function):
     @staticmethod
     def forward(ctx, verts, faces):

@@ -285,11 +285,67 @@ __global__ void __launch_bounds__(IMG_NT) image_batch_kernel(const __grid_consta
         image_rows<1>(tile, col_s0, col_w1, row_s0, row_w1, lut);
 }
 
-int check_device_ptr(const void* p, const char* what) {
+// ---------------------------------------------------------------------------------------------------------------------
+// Pseudo-ground-truth records (run_reconstruction.py:571-603): the texel-visibility mask resized to R, the inverse render
+// masked with it and moved to NCHW, every plane rounded to fp16 in one launch.
+
+constexpr int PACK_NT = 256;
+
+struct PackArgs {
+    const uint8_t* vis;      // [B, Th, Tw] 0 / 1
+    int Th, Tw;
+    float sy, sx;            // Th / R, Tw / R as F.interpolate(size=R) computes them
+    const float* tex;        // [B, R, R, C]
+    const float* alpha;      // [B, R, R, 1]
+    int R, C;
+    const float* image;      // [B, Ci, h, w]
+    long long pix_total, image_total;
+    int pix_blocks;
+    __half* tex_out;         // [B, C, R, R]
+    __half* alpha_out;       // [B, 1, R, R]
+    __half* image_out;       // [B, Ci, h, w]
+};
+
+// upsample_bilinear2d's source taps of output index d (align_corners=False): src = scale (d + 0.5) - 0.5 in fp32 with one
+// rounding, clamped at 0; the second tap is the next row / column unless d maps onto the last one, and takes part only
+// with a non-zero lambda
+__device__ __forceinline__ void mask_taps(int d, int in, float scale, int& i0, int& i1, bool& use1) {
+    float src = __fmaf_rn(scale, (float)d + 0.5f, -0.5f);
+    if (src < 0.f) src = 0.f;
+    i0 = (int)src;
+    i1 = i0 + (i0 < in - 1 ? 1 : 0);
+    use1 = src - (float)i0 > 0.f;
+}
+
+__global__ void __launch_bounds__(PACK_NT) pseudogt_pack_kernel(const __grid_constant__ PackArgs a) {
+    if ((int)blockIdx.x < a.pix_blocks) {
+        const long long t = (long long)blockIdx.x * PACK_NT + threadIdx.x;
+        if (t >= a.pix_total) return;
+        const long long plane = (long long)a.R * a.R;
+        const long long b = t / plane;
+        const int pos = (int)(t - b * plane), y = pos / a.R, x = pos - y * a.R;
+        int y0, y1, x0, x1;
+        bool uy, ux;
+        mask_taps(y, a.Th, a.sy, y0, y1, uy);
+        mask_taps(x, a.Tw, a.sx, x0, x1, ux);
+        const uint8_t* v = a.vis + b * a.Th * a.Tw;
+        const bool seen = v[y0 * a.Tw + x0] || (ux && v[y0 * a.Tw + x1]) ||
+                          (uy && (v[y1 * a.Tw + x0] || (ux && v[y1 * a.Tw + x1])));
+        const float m = seen ? 1.f : 0.f;
+        const float* src = a.tex + t * a.C;
+        for (int c = 0; c < a.C; ++c) a.tex_out[(b * a.C + c) * plane + pos] = __float2half_rn(__fmul_rn(src[c], m));
+        a.alpha_out[t] = __float2half_rn(__fmul_rn(a.alpha[t], m));
+    } else {
+        const long long t = (long long)(blockIdx.x - a.pix_blocks) * PACK_NT + threadIdx.x;
+        if (t < a.image_total) a.image_out[t] = __float2half_rn(a.image[t]);
+    }
+}
+
+int check_device_ptr(const void* p, const char* what, const char* fn = "b3d_image_batch") {
     cudaPointerAttributes at;
     B3D_CUDA_OK(cudaPointerGetAttributes(&at, p));
     B3D_REQUIRE(at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged, B3D_EINVAL,
-                "b3d_image_batch: %s is not device memory", what);
+                "%s: %s is not device memory", fn, what);
     return B3D_OK;
 }
 
@@ -381,6 +437,38 @@ int b3d_image_batch(const uint32_t* pixels, const int64_t* offsets, const int32_
         if (rc != B3D_OK) return rc;
     }
     image_batch_kernel<<<(unsigned)blocks, IMG_NT, 0, (cudaStream_t)stream>>>(a);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+int b3d_pseudogt_pack(const uint8_t* vis, int Th, int Tw, const float* tex, const float* alpha, int B, int R, int C,
+                      const float* image, int Ci, int h, int w, uint16_t* tex_out, uint16_t* alpha_out,
+                      uint16_t* image_out, void* stream) {
+    B3D_REQUIRE(B >= 0 && Th >= 1 && Tw >= 1 && R >= 1 && C >= 1 && Ci >= 1 && h >= 1 && w >= 1, B3D_EINVAL,
+                "b3d_pseudogt_pack: bad sizes (B %d, texture %d x %d, R %d, C %d, image %d x %d x %d)", B, Th, Tw, R, C,
+                Ci, h, w);
+    if (B == 0) return B3D_OK;
+    PackArgs a = {};
+    a.vis = vis, a.Th = Th, a.Tw = Tw;
+    a.sy = (float)Th / (float)R, a.sx = (float)Tw / (float)R;
+    a.tex = tex, a.alpha = alpha, a.R = R, a.C = C, a.image = image;
+    a.pix_total = (long long)B * R * R;
+    a.image_total = (long long)B * Ci * h * w;
+    a.tex_out = reinterpret_cast<__half*>(tex_out);
+    a.alpha_out = reinterpret_cast<__half*>(alpha_out);
+    a.image_out = reinterpret_cast<__half*>(image_out);
+    const long long pix_blocks = (a.pix_total + PACK_NT - 1) / PACK_NT;
+    const long long blocks = pix_blocks + (a.image_total + PACK_NT - 1) / PACK_NT;
+    B3D_REQUIRE(blocks < (1LL << 31), B3D_EINVAL, "b3d_pseudogt_pack: batch too large");
+    a.pix_blocks = (int)pix_blocks;
+    const void* ptrs[] = {vis, tex, alpha, image, tex_out, alpha_out, image_out};
+    const char* names[] = {"vis", "tex", "alpha", "image", "tex_out", "alpha_out", "image_out"};
+    for (int i = 0; i < 7; ++i) {
+        B3D_REQUIRE(ptrs[i], B3D_EINVAL, "b3d_pseudogt_pack: null %s", names[i]);
+        const int rc = check_device_ptr(ptrs[i], names[i], "b3d_pseudogt_pack");
+        if (rc != B3D_OK) return rc;
+    }
+    pseudogt_pack_kernel<<<(unsigned)blocks, PACK_NT, 0, (cudaStream_t)stream>>>(a);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }

@@ -180,6 +180,25 @@ __device__ __forceinline__ float tex_at(const float* __restrict__ t, int y, int 
     return (x >= 0 && x < Tw && y >= 0 && y < Th) ? __ldg(t + (size_t)y * Tw + x) : 0.f;
 }
 
+// interpolated (u, v) of a covered pixel and the interpolated constant-1 attribute (= hard mask) from the barycentrics
+// w0..w2 and the covering face's corner uvs a[6]; shared by the shader, its adjoint and the texel-visibility kernel so
+// that all three sample the texture at the same point
+struct ShadePoint {
+    float u, v, msum;
+};
+__device__ __forceinline__ ShadePoint shade_point(float w0, float w1, float w2, const float* a) {
+    return ShadePoint{w0 * a[0] + w1 * a[2] + w2 * a[4], w0 * a[1] + w1 * a[3] + w2 * a[5], w0 + w1 + w2};
+}
+
+// the texture adjoint's contribution g * wx * wy to the four taps (x0,y0), (x0+1,y0), (x0,y0+1), (x0+1,y0+1)
+struct TapWeights {
+    float w00, w01, w10, w11;
+};
+__device__ __forceinline__ TapWeights tap_weights(float g, const TexTap& tp) {
+    const float wx0 = 1.f - tp.wx1, wy0 = 1.f - tp.wy1;
+    return TapWeights{g * wx0 * wy0, g * tp.wx1 * wy0, g * wx0 * tp.wy1, g * tp.wx1 * tp.wy1};
+}
+
 template <bool SHADE>
 __global__ void __launch_bounds__(NT)
 mesh_raster_fwd_kernel(const float4* __restrict__ fgeo, const float* __restrict__ fuv, const float* __restrict__ tex,
@@ -268,10 +287,8 @@ mesh_raster_fwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
     improb[pix] = best >= 0 ? 1.f : 1.f - keep;
     float o0 = 0.f, o1 = 0.f, o2 = 0.f;
     if (best >= 0) {
-        const float* a = fuv + ((size_t)b * F + best) * 6;
-        const float u = bw0 * a[0] + bw1 * a[2] + bw2 * a[4];
-        const float v = bw0 * a[1] + bw1 * a[3] + bw2 * a[5];
-        const float msum = bw0 + bw1 + bw2;       // the interpolated constant-1 attribute = hard mask
+        const ShadePoint sp = shade_point(bw0, bw1, bw2, fuv + ((size_t)b * F + best) * 6);
+        const float u = sp.u, v = sp.v, msum = sp.msum;
         if (SHADE) {
             const TexTap tp = tex_tap(u, v, Th, Tw);
             const float wx0 = 1.f - tp.wx1, wy0 = 1.f - tp.wy1;
@@ -382,10 +399,9 @@ mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
         const float* a = fuv + ((size_t)b * F + fidx) * 6;
         float du, dv;
         if (SHADE) {
-            const float u = w0 * a[0] + w1 * a[2] + w2 * a[4];
-            const float v = w0 * a[1] + w1 * a[3] + w2 * a[5];
-            const float msum = w0 + w1 + w2;
-            const TexTap tp = tex_tap(u, v, Th, Tw);
+            const ShadePoint sp = shade_point(w0, w1, w2, a);
+            const float msum = sp.msum;
+            const TexTap tp = tex_tap(sp.u, sp.v, Th, Tw);
             const float wx0 = 1.f - tp.wx1, wy0 = 1.f - tp.wy1;
             const float g[3] = {g0 * msum, g1 * msum, g2 * msum};      // colour = tex * mask (or lerp)
             float sx = 0.f, sy = 0.f;
@@ -400,6 +416,7 @@ mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
                 if (g[c] != 0.f) {
                     const bool xa = tp.x0 >= 0 && tp.x0 < Tw, xb = tp.x0 + 1 >= 0 && tp.x0 + 1 < Tw;
                     const bool ya = tp.y0 >= 0 && tp.y0 < Th, yb = tp.y0 + 1 >= 0 && tp.y0 + 1 < Th;
+                    // the same products as tap_weights (texel_visibility_kernel marks the taps where they are > 0)
                     if (ya && xa) atomicAdd(dt + (size_t)tp.y0 * Tw + tp.x0, g[c] * wx0 * wy0);
                     if (ya && xb) atomicAdd(dt + (size_t)tp.y0 * Tw + tp.x0 + 1, g[c] * tp.wx1 * wy0);
                     if (yb && xa) atomicAdd(dt + (size_t)(tp.y0 + 1) * Tw + tp.x0, g[c] * wx0 * tp.wy1);
@@ -497,6 +514,66 @@ mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
     }
 }
 
+// Texel visibility of a forward render: the texels whose texture gradient under an all-ones upstream gradient is > 0,
+// i.e. the taps mesh_raster_bwd_kernel<true> would add a positive weight to, without running the adjoint.  A CTA covers
+// VIS_PIX * NT pixels of one sample and marks texels in a per-sample bit mask in shared memory (the padded columns folded
+// onto the texels they copy), then ORs its non-zero words into the global words once each.
+constexpr int VIS_PIX = 16;
+
+__device__ __forceinline__ void mark_texel(unsigned int* bits, int y, int x, float w, int Th, int Tw, int Tw_out,
+                                           int symmetric) {
+    if (!(w > 0.f) || x < 0 || x >= Tw || y < 0 || y >= Th) return;
+    // symmetric: circpad(tex, 1) put source column Tw_out-1 first and column 0 last; otherwise column 0 was appended
+    const int xs = symmetric ? (x == 0 ? Tw_out - 1 : (x == Tw - 1 ? 0 : x - 1)) : (x == Tw_out ? 0 : x);
+    const int bit = y * Tw_out + xs;
+    const unsigned int m = 1u << (bit & 31);
+    if (!(bits[bit >> 5] & m)) atomicOr(bits + (bit >> 5), m);
+}
+
+__global__ void __launch_bounds__(NT)
+texel_visibility_kernel(const int32_t* __restrict__ imidx, const float* __restrict__ imwei, const float* __restrict__ fuv,
+                        int F, long long HW, int Th, int Tw, int Tw_out, int symmetric, int nwords,
+                        unsigned int* __restrict__ words) {
+    extern __shared__ unsigned int bits[];
+    const int b = blockIdx.y;
+    for (int i = threadIdx.x; i < nwords; i += NT) bits[i] = 0u;
+    __syncthreads();
+    const long long p0 = (long long)blockIdx.x * NT * VIS_PIX + threadIdx.x;
+    for (int k = 0; k < VIS_PIX; ++k) {
+        const long long p = p0 + (long long)k * NT;
+        if (p >= HW) break;
+        const size_t pix = (size_t)b * HW + p;
+        const int fidx = imidx[pix] - 1;
+        if (fidx < 0) continue;
+        const ShadePoint sp = shade_point(imwei[3 * pix], imwei[3 * pix + 1], imwei[3 * pix + 2],
+                                          fuv + ((size_t)b * F + fidx) * 6);
+        const float g = 1.f * sp.msum;          // the adjoint's g[c] = d_imout * msum with d_imout = 1
+        if (g == 0.f) continue;
+        const TexTap tp = tex_tap(sp.u, sp.v, Th, Tw);
+        const TapWeights tw = tap_weights(g, tp);
+        mark_texel(bits, tp.y0, tp.x0, tw.w00, Th, Tw, Tw_out, symmetric);
+        mark_texel(bits, tp.y0, tp.x0 + 1, tw.w01, Th, Tw, Tw_out, symmetric);
+        mark_texel(bits, tp.y0 + 1, tp.x0, tw.w10, Th, Tw, Tw_out, symmetric);
+        mark_texel(bits, tp.y0 + 1, tp.x0 + 1, tw.w11, Th, Tw, Tw_out, symmetric);
+    }
+    __syncthreads();
+    unsigned int* dst = words + (size_t)b * nwords;
+    for (int i = threadIdx.x; i < nwords; i += NT) {
+        const unsigned int v = bits[i];
+        if (v) atomicOr(dst + i, v);
+    }
+}
+
+__global__ void __launch_bounds__(NT)
+visibility_bytes_kernel(const unsigned int* __restrict__ words, int nbits, int nwords, long long total,
+                        uint8_t* __restrict__ vis) {
+    const long long t = (long long)blockIdx.x * NT + threadIdx.x;
+    if (t >= total) return;
+    const long long b = t / nbits;
+    const int i = (int)(t - b * nbits);
+    vis[t] = (uint8_t)((words[b * nwords + (i >> 5)] >> (i & 31)) & 1u);
+}
+
 size_t fwd_smem(int F) { return sizeof(float4) * CHUNK * 3 + sizeof(int) * (size_t)F; }
 size_t bwd_smem(int F) { return sizeof(float4) * CHUNK * 3 + sizeof(float) * CAPN * 12 + 2 * sizeof(int) * (size_t)F; }
 
@@ -572,6 +649,35 @@ int b3d_mesh_render_bwd(const float* fgeo, const float* fuv, const float* tex, i
         mesh_raster_bwd_kernel<false><<<grid, NT, smem, st>>>((const float4*)fgeo, fuv, nullptr, 0, F, H, W, 0, 0, imidx,
                                                              imwei, d_imout, d_improb, dfp2d, dfuv, nullptr);
     }
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+int b3d_texel_visibility(const int32_t* imidx, const float* imwei, const float* fuv, int B, int F, int H, int W, int Th,
+                         int Tw, int symmetric, uint32_t* words, uint8_t* vis, void* stream) {
+    B3D_REQUIRE(B >= 0 && F > 0 && H > 0 && W > 0, B3D_EINVAL, "b3d_texel_visibility: bad sizes");
+    const int Tw_out = Tw - (symmetric ? 2 : 1);
+    B3D_REQUIRE(Th > 1 && Tw_out >= 1 && (!symmetric || Tw_out >= 2), B3D_EINVAL,
+                "b3d_texel_visibility: bad texture size %d x %d (symmetric %d)", Th, Tw, symmetric);
+    if (B == 0) return B3D_OK;
+    B3D_REQUIRE(imidx && imwei && fuv && words && vis, B3D_EINVAL, "b3d_texel_visibility: null pointer");
+    const long long nbits = (long long)Th * Tw_out;
+    const int nwords = (int)((nbits + 31) / 32);
+    const size_t smem = sizeof(unsigned int) * (size_t)nwords;
+    B3D_REQUIRE(smem <= 200 * 1024, B3D_EINVAL, "b3d_texel_visibility: texture %d x %d too large for the bit mask", Th,
+                Tw_out);
+    const long long HW = (long long)H * W;
+    const long long ctas = (HW + (long long)NT * VIS_PIX - 1) / ((long long)NT * VIS_PIX);
+    const long long total = (long long)B * nbits;
+    B3D_REQUIRE(B <= 65535 && ctas < (1LL << 31) && (total + NT - 1) / NT < (1LL << 31), B3D_EINVAL,
+                "b3d_texel_visibility: batch too large");
+    cudaStream_t st = (cudaStream_t)stream;
+    B3D_CUDA_OK(cudaMemsetAsync(words, 0, sizeof(uint32_t) * (size_t)B * nwords, st));
+    B3D_CUDA_OK(cudaFuncSetAttribute(texel_visibility_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    texel_visibility_kernel<<<dim3((unsigned)ctas, B), NT, smem, st>>>(imidx, imwei, fuv, F, HW, Th, Tw, Tw_out,
+                                                                       symmetric ? 1 : 0, nwords, words);
+    B3D_LAUNCH_OK();
+    visibility_bytes_kernel<<<(unsigned)((total + NT - 1) / NT), NT, 0, st>>>(words, (int)nbits, nwords, total, vis);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }

@@ -168,6 +168,18 @@ B3D_API int b3d_mesh_render_bwd(const float* fgeo, const float* fuv, const float
                                 const float* imwei, const float* d_imout, const float* d_improb,
                                 float* dfp2d, float* dfuv, float* dtex, void* stream);
 
+/* Texel visibility of a forward render          run_reconstruction.py:567-572, rendering/inverse_renderer.py texel_visibility
+ *   visibility_mask, = torch.autograd.grad(image_pred, pred_tex, torch.ones_like(image_pred))  ->  visibility_mask > 0
+ * imidx [B,H,W], imwei [B,H,W,3] of b3d_mesh_render_fwd (tex may be NULL there), fuv [B,F,6] of b3d_mesh_face_setup with the
+ * template's seam-adjusted uvs; Th x Tw the PADDED texture the shader would sample.  vis [B,Th,Tw_out] uint8 out: 1 exactly
+ * where b3d_mesh_render_bwd's dtex under d_imout = 1 is > 0 in some channel, summed back through the seam padding:
+ * symmetric = 1: circpad(tex, 1) (Tw_out = Tw - 2; padded column 0 is source column Tw_out - 1, column Tw - 1 is column 0);
+ * symmetric = 0: tex with column 0 appended (Tw_out = Tw - 1).  A covered pixel marks each in-bounds bilinear tap whose
+ * fp32 weight (msum * wx) * wy, evaluated as the adjoint evaluates it, is > 0; no float atomics.
+ * words [B, ceil(Th*Tw_out/32)] uint32 scratch (zeroed by the call).  Th*Tw_out <= 200 KiB * 8.                              */
+B3D_API int b3d_texel_visibility(const int32_t* imidx, const float* imwei, const float* fuv, int B, int F, int H, int W,
+                                 int Th, int Tw, int symmetric, uint32_t* words, uint8_t* vis, void* stream);
+
 /* MeshTemplate.compute_normals                  rendering/mesh_template.py:113-123
  * verts [B,V,3], faces [F,3] int32 -> normals [B,F,3] = normalize((v_b - v_a) x (v_c - v_a)) (F.normalize: n / max(|n|, 1e-12)).
  * bwd: gnormals [B,F,3] -> dverts [B,V,3] (zeroed by the call, accumulated with atomics).  Vertex ids must lie in [0, V). */
@@ -477,6 +489,20 @@ B3D_API int b3d_image_batch(const uint32_t* pixels, const int64_t* offsets, cons
                             int n, const int32_t* idx, const uint8_t* flip, int B, int nres, const int32_t* res,
                             float* const* images, float* scale, float* translation, float* rot, int64_t* ind,
                             void* stream);
+
+/* ---- Pseudo-ground-truth records (reference: run_reconstruction.py:573-603) ------------------------------------------
+ *   mask = F.interpolate(visibility_mask, R, mode='bilinear', align_corners=False).permute(0, 2, 3, 1)
+ *   mask = (mask > 0).any(dim=3, keepdim=True).float()
+ *   inverse_tex *= mask; inverse_alpha *= mask; .permute(0, 3, 1, 2).half(); inception_image.half()
+ * b3d_pseudogt_pack  vis [B,Th,Tw] uint8 (b3d_texel_visibility), tex [B,R,R,C] and alpha [B,R,R,1] fp32 (the inverse render
+ *                    and its hard mask), image [B,Ci,h,w] fp32 -> tex_out [B,C,R,R], alpha_out [B,1,R,R], image_out
+ *                    [B,Ci,h,w] fp16 (round to nearest even, as .half()).  The mask pixel is 1 iff a bilinear tap with a
+ *                    non-zero lambda is visible: upsample_bilinear2d's rule, src = (Th / R) (d + 0.5) - 0.5 in fp32 with one
+ *                    rounding, clamped at 0, the second tap the next row unless on the last row.  Masking multiplies by 1.0
+ *                    or 0.0 in fp32 (a negative value masked out stays -0.0).  Every pointer must be device memory.     */
+B3D_API int b3d_pseudogt_pack(const uint8_t* vis, int Th, int Tw, const float* tex, const float* alpha, int B, int R, int C,
+                              const float* image, int Ci, int h, int w, uint16_t* tex_out, uint16_t* alpha_out,
+                              uint16_t* image_out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -99,6 +99,38 @@ def pad_x(x_nchw, amount, mode):
 # ------------------------------------------------------------------------------------------------------------------
 # fused conditional-batch-norm -> LeakyReLU -> (+ residual) -> (LeakyReLU) -> x2 nearest upsample -> replicate pad
 # ------------------------------------------------------------------------------------------------------------------
+def identity_norm(x):
+    """The generator's norm_g='none' layer: the input unchanged (the reference's `lambda x: x`)."""
+    return x
+
+
+def norm_kind(norm):
+    """How the fused glue normalises for this layer: 'batch' (BatchNorm2d / SynchronizedBatchNorm2d), 'instance'
+    (InstanceNorm2d without running buffers, as the reference builds it: instance statistics in training and eval),
+    'none' (identity_norm), or None (anything else, which the fused glue does not run)."""
+    from torch.nn.modules.batchnorm import _BatchNorm
+    if isinstance(norm, _BatchNorm):
+        return 'batch'
+    if isinstance(norm, torch.nn.InstanceNorm2d) and not norm.track_running_stats:
+        return 'instance'
+    if norm is identity_norm:
+        return 'none'
+    return None
+
+
+def _check_glue(name, y, C_norm, up, pad, pad_mode):
+    """Shape checks of the fused glue's wrappers, before any CUDA call."""
+    if y.dim() != 4:
+        raise B3DError(f"{name}: expected a 4-D activation, got shape {tuple(y.shape)}")
+    C, W = y.shape[1], y.shape[3]
+    if C % 4 or 256 % (C // 4):
+        raise B3DError(f"{name}: C={C} must be 4 * a divisor of 256")
+    if C_norm is not None and C != C_norm:
+        raise B3DError(f"{name}: {C} channels, but the norm layer has {C_norm}")
+    if pad_mode not in (REPLICATE, CIRCULAR) or pad < 0 or (pad_mode == CIRCULAR and pad > up * W):
+        raise B3DError(f"{name}: pad {pad} in mode {pad_mode} does not fit {up * W} columns")
+
+
 def _f32(v):
     """v rounded to the nearest fp32 value, as a Python float."""
     return struct.unpack("f", struct.pack("f", float(v)))[0]
@@ -133,8 +165,9 @@ class CBNBatch:
         self.stats = torch.zeros(off, device=z.device, dtype=torch.float64) if z.is_cuda else None
 
     def stats_slot(self, cbn):
-        """The layer's zeroed statistics slot [2*C] (handed to the producing convolution), or None in eval mode."""
-        if self.stats is None or not cbn.norm.training:
+        """The layer's zeroed statistics slot [2*C] (handed to the producing convolution), or None in eval mode and for
+        instance / no normalisation (the epilogue sums over the whole batch)."""
+        if self.stats is None or norm_kind(cbn.norm) != 'batch' or not cbn.norm.training:
             return None
         goff, boff = self.offsets[id(cbn)]
         return self.stats[goff: goff + 2 * (boff - goff)]
@@ -164,12 +197,16 @@ class BNAffine(CBNBatch):
 class _CBNActPad(torch.autograd.Function):
     """y [N,H,W,C] (conv output, NHWC) -> out [N, up*H, up*W + 2*pad, C]; gb = CBNBatch.gb (gamma / beta of this layer at
     column offsets goff / boff).  `skip` (optional) [N,H,Ws,C] read at pixel offset skip_off.  Statistics, running buffers
-    and the per-sample affine come from one b3d_cbn_prepare launch (modes: 0 eval, 1 batch statistics, 2 SyncBN).
+    and the per-sample affine come from one b3d_cbn_prepare launch (modes: 0 eval, 1 batch statistics, 2 SyncBN,
+    3 instance statistics, 4 no normalisation; norm_kind(bn) picks the family).
     As in F.batch_norm, a norm without running buffers (track_running_stats=False) uses batch statistics in eval mode too,
-    and momentum=None makes the running buffers a cumulative average (factor 1 / num_batches_tracked)."""
+    and momentum=None makes the running buffers a cumulative average (factor 1 / num_batches_tracked).
+    Instance statistics come from one per-sample sums pass and, like no normalisation, give per-sample mean / inv_std rows
+    [N, C] and per-sample coupling terms in the backward: no cross-sample reduction and never SyncBN.  pad_mode: REPLICATE
+    or CIRCULAR x padding of the output (wrapped in upsampled coordinates)."""
 
     @staticmethod
-    def forward(ctx, y, gb, cb, key, bn, skip, skip_off, up, pad, post_leaky, sums_in=None, slope=0.2):
+    def forward(ctx, y, gb, cb, key, bn, skip, skip_off, up, pad, post_leaky, sums_in=None, slope=0.2, pad_mode=REPLICATE):
         y = dev(y.detach(), "y")
         N, H, W, C = y.shape
         gbd = dev(gb.detach(), "gamma/beta")
@@ -178,8 +215,17 @@ class _CBNActPad(torch.autograd.Function):
         goff, boff = cb.offsets[key]
         st = stream_ptr(y)
         mode, sums, count, sync, peers = 0, None, 1.0, False, None
+        kind = norm_kind(bn)
+        if kind is None:
+            raise B3DError(f"fused norm glue: unsupported norm layer {bn!r}")
+        if kind == 'instance':
+            sums = torch.empty(N, 2 * C, device=y.device, dtype=torch.float64)
+            check(lib.b3d_bn_sums_per_sample(ptr(y), N, H * W, C, ptr(sums), st))
+            mode, count = 3, float(H * W)
+        elif kind == 'none':
+            mode = 4
         # F.batch_norm normalises with the batch statistics in training, and in eval too when there are no running buffers
-        if bn.training or bn.running_mean is None:
+        elif bn.training or bn.running_mean is None:
             if sums_in is not None:                     # accumulated by the epilogue of the convolution that produced y
                 sums = sums_in
             else:
@@ -193,12 +239,15 @@ class _CBNActPad(torch.autograd.Function):
                 peers = peer_sync(y.device) if C <= 512 else None
                 if peers is None:
                     dist.all_reduce(sums)                   # NCCL fallback: one collective per layer, [sum x, sum x^2] in fp64
-        mean = torch.empty(C, device=y.device, dtype=torch.float32)
+        per_sample = mode >= 3
+        mean = torch.empty((N, C) if per_sample else C, device=y.device, dtype=torch.float32)
         invstd = torch.empty_like(mean)
         scale = torch.empty(N, C, device=y.device, dtype=torch.float32)
         shift, gt = torch.empty_like(scale), torch.empty_like(scale)
-        track = bn.training and bn.track_running_stats
-        momentum = -1.0 if bn.momentum is None else float(bn.momentum)    # < 0: cumulative average, as torch for None
+        track = kind == 'batch' and bn.training and bn.track_running_stats
+        # momentum < 0: cumulative average, as torch for None
+        momentum = -1.0 if kind != 'batch' or bn.momentum is None else float(bn.momentum)
+        eps = float(bn.eps) if kind != 'none' else 0.0
         if peers is not None:
             # statistics all-reduce over NVLink peer memory fused into the kernel that consumes them (csrc/ew_kernels.cu)
             check(lib.b3d_cbn_prepare_sync(peers.data, peers.flag, peers.rank, peers.world, ptr(peers.epoch), ptr(peers.err),
@@ -207,7 +256,7 @@ class _CBNActPad(torch.autograd.Function):
                                            ptr(bn.num_batches_tracked) if track else None,
                                            ptr(mean), ptr(invstd), ptr(scale), ptr(shift), ptr(gt), N, C, st))
         else:
-            check(lib.b3d_cbn_prepare(ptr(gbd), gp, goff, boff, ptr(sums), count, float(bn.eps), momentum, mode,
+            check(lib.b3d_cbn_prepare(ptr(gbd), gp, goff, boff, ptr(sums), count, eps, momentum, mode,
                                       ptr(bn.running_mean) if (track or mode == 0) else None,
                                       ptr(bn.running_var) if (track or mode == 0) else None,
                                       ptr(bn.num_batches_tracked) if track else None,
@@ -215,12 +264,12 @@ class _CBNActPad(torch.autograd.Function):
         sk = dev(skip.detach(), "skip") if skip is not None else None
         pitch = sk.shape[2] if sk is not None else 0
         out = torch.empty(N, up * H, up * W + 2 * pad, C, device=y.device, dtype=torch.float32)
-        check(lib.b3d_cbn_act_fwd(ptr(y), ptr(scale), ptr(shift), ptr(sk), pitch, skip_off, ptr(out), N, H, W, C, up, pad, float(slope),
-                                  int(post_leaky), st))
+        check(lib.b3d_cbn_act_fwd_ex(ptr(y), ptr(scale), ptr(shift), ptr(sk), pitch, skip_off, ptr(out), N, H, W, C, up, pad,
+                                     int(pad_mode), float(slope), int(post_leaky), st))
         ctx.save_for_backward(y, gt, scale, shift, mean, invstd, sk if sk is not None else torch.empty(0))
         ctx.cb, ctx.key = cb, key
-        ctx.cfg = (skip_off, up, pad, post_leaky, mode != 0, sync, count, sk is not None, skip.shape if skip is not None else None,
-                   P, goff, boff, float(slope))
+        ctx.cfg = (skip_off, up, pad, post_leaky, mode, sync, count, sk is not None, skip.shape if skip is not None else None,
+                   P, goff, boff, float(slope), int(pad_mode))
         ctx.peers = peers
         # mode 2's inv_std of a clamped channel, as the kernels round it: (float)(1 / sqrt((double)eps))
         ctx.clamp_lim = _f32(1.0 / math.sqrt(_f32(bn.eps))) if sync else None
@@ -229,7 +278,7 @@ class _CBNActPad(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gout):
         y, gt, scale, shift, mean, invstd, sk = ctx.saved_tensors
-        skip_off, up, pad, post_leaky, batch_stats, sync, count, has_skip, skip_shape, P, goff, boff, slope = ctx.cfg
+        skip_off, up, pad, post_leaky, mode, sync, count, has_skip, skip_shape, P, goff, boff, slope, pad_mode = ctx.cfg
         cb = ctx.cb
         N, H, W, C = y.shape
         gout = dev(gout, "grad")
@@ -243,11 +292,16 @@ class _CBNActPad(torch.autograd.Function):
         sink = cb.grad_sink(N) if want_gb else torch.empty(N, P, device=y.device)
         s1 = ctypes.c_void_p(sink.data_ptr() + 4 * boff)        # d beta  = sum ga
         s2 = ctypes.c_void_p(sink.data_ptr() + 4 * goff)        # d gamma = sum ga * xhat
-        check(lib.b3d_cbn_act_bwd1(ptr(gout), ptr(y), ptr(scale), ptr(shift), ptr(sk) if has_skip else None,
-                                   sk.shape[2] if has_skip else 0, skip_off, ptr(mean), ptr(invstd), ptr(ga), ptr(gskip), gpitch,
-                                   skip_off, s1, s2, P, N, H, W, C, up, pad, slope, int(post_leaky), st))
+        stat_pitch = C if mode >= 3 else 0                 # per-sample mean / inv_std rows (instance / no normalisation)
+        check(lib.b3d_cbn_act_bwd1_ex(ptr(gout), ptr(y), ptr(scale), ptr(shift), ptr(sk) if has_skip else None,
+                                      sk.shape[2] if has_skip else 0, skip_off, ptr(mean), ptr(invstd), stat_pitch, ptr(ga), ptr(gskip),
+                                      gpitch, skip_off, s1, s2, P, N, H, W, C, up, pad, pad_mode, slope, int(post_leaky), st))
         inv_m = 0.0
-        if batch_stats:
+        if mode >= 3:
+            # per-sample coupling terms inv_m * gamma_t * (S1, S2) read straight from the d(gamma, beta) rows
+            inv_m = 1.0 / count if mode == 3 else 0.0
+            check(lib.b3d_cbn_act_bwd2_ex(ptr(ga), ptr(y), ptr(gt), ptr(mean), ptr(invstd), C, s1, s2, P, inv_m, N, H, W, C, st))
+        elif mode != 0:
             red = torch.empty(2 * C, device=y.device, dtype=torch.float32)
             peers = ctx.peers
             if sync and peers is not None:
@@ -265,8 +319,9 @@ class _CBNActPad(torch.autograd.Function):
             inv_m = 1.0 / count
         else:
             red = torch.zeros(2 * C, device=y.device, dtype=torch.float32)
-        check(lib.b3d_cbn_act_bwd2(ptr(ga), ptr(y), ptr(gt), ptr(mean), ptr(invstd), ptr(red), ctypes.c_void_p(red.data_ptr() + 4 * C),
-                                   inv_m, N, H, W, C, st))
+        if mode < 3:
+            check(lib.b3d_cbn_act_bwd2(ptr(ga), ptr(y), ptr(gt), ptr(mean), ptr(invstd), ptr(red),
+                                       ctypes.c_void_p(red.data_ptr() + 4 * C), inv_m, N, H, W, C, st))
         ggb = None
         if want_gb:
             cb.done += 1
@@ -274,7 +329,7 @@ class _CBNActPad(torch.autograd.Function):
                 if cb.done != cb.n_layers:
                     raise RuntimeError(f"CBNBatch: {cb.done} of {cb.n_layers} layers ran their backward before the first layer's")
                 ggb = sink.sum(dim=0, keepdim=True) if cb.shared else sink
-        return ga, ggb, None, None, None, gskip, None, None, None, None, None, None
+        return ga, ggb, None, None, None, gskip, None, None, None, None, None, None, None
 
 
 def bn_act_pad(y_nchw, bn, skip_nchw=None, skip_off=0, up=1, pad=1, post_relu=False, slope=0.0):
@@ -290,17 +345,34 @@ def bn_act_pad(y_nchw, bn, skip_nchw=None, skip_off=0, up=1, pad=1, post_relu=Fa
     return out.permute(0, 3, 1, 2)
 
 
-def cbn_act_pad(y_nchw, cbn, z, skip_nchw=None, skip_off=0, up=1, pad=1, post_leaky=False, cb=None, sums=None):
-    """ConditionalBatchNorm2d(y, z) -> LeakyReLU(0.2) [-> + skip] [-> LeakyReLU] [-> x2 upsample] -> replicate pad, fused.
-    `cbn` is a models.gan.ConditionalBatchNorm2d whose .norm is a (Synchronized)BatchNorm2d without affine; statistics and
-    running buffers follow F.batch_norm (single process) or the reference's SyncBN formulas (torch.distributed).
-    cb: the forward's CBNBatch (gamma / beta of all layers from one GEMM); None = a one-layer batch built here."""
+def cbn_act_pad(y_nchw, cbn, z, skip_nchw=None, skip_off=0, up=1, pad=1, post_leaky=False, cb=None, sums=None,
+                pad_mode=REPLICATE):
+    """ConditionalBatchNorm2d(y, z) -> LeakyReLU(0.2) [-> + skip] [-> LeakyReLU] [-> x2 upsample] -> x pad, fused.
+    `cbn` is a models.gan.ConditionalBatchNorm2d whose .norm is a (Synchronized)BatchNorm2d without affine (statistics and
+    running buffers follow F.batch_norm in a single process, the reference's SyncBN formulas under torch.distributed), an
+    InstanceNorm2d without affine or running buffers (per-sample statistics), or identity_norm (no normalisation).
+    cb: the forward's CBNBatch (gamma / beta of all layers from one GEMM); None = a one-layer batch built here.
+    pad_mode: REPLICATE (symmetric generator) or CIRCULAR (asymmetric generator)."""
+    if norm_kind(cbn.norm) is None:
+        raise B3DError(f"cbn_act_pad: unsupported norm layer {cbn.norm!r}")
+    _check_glue("cbn_act_pad", y_nchw, cbn.fc_gamma.out_features, int(up), int(pad), int(pad_mode))
     if cb is None:
         cb = CBNBatch([cbn], z)
     y = y_nchw.permute(0, 2, 3, 1)
-    C = y.shape[3]
-    if C % 4 or 256 % (C // 4):
-        raise B3DError(f"cbn_act_pad: C={C} must be 4 * a divisor of 256")
     skip = skip_nchw.permute(0, 2, 3, 1) if skip_nchw is not None else None
-    out = _CBNActPad.apply(y, cb.gb, cb, id(cbn), cbn.norm, skip, int(skip_off), int(up), int(pad), bool(post_leaky), sums)
+    out = _CBNActPad.apply(y, cb.gb, cb, id(cbn), cbn.norm, skip, int(skip_off), int(up), int(pad), bool(post_leaky), sums, 0.2,
+                           int(pad_mode))
+    return out.permute(0, 3, 1, 2)
+
+
+def in_act_pad(y_nchw, norm, pad=0, pad_mode=CIRCULAR, slope=0.2):
+    """InstanceNorm2d(y) (affine, instance statistics in training and eval) -> LeakyReLU(slope) -> x pad in one pass: the
+    discriminators' norm_d='instance' layers (conv without bias -> norm -> LeakyReLU(0.2) -> the next layer's circular
+    padding).  The affine weight / bias are one row shared by all samples, as in bn_act_pad."""
+    if norm_kind(norm) != 'instance' or not norm.affine:
+        raise B3DError(f"in_act_pad: expected an affine InstanceNorm2d without running buffers, got {norm!r}")
+    _check_glue("in_act_pad", y_nchw, norm.num_features, 1, int(pad), int(pad_mode))
+    cb = BNAffine(norm)
+    out = _CBNActPad.apply(y_nchw.permute(0, 2, 3, 1), cb.gb, cb, id(norm), norm, None, 0, 1, int(pad), False, None,
+                           float(slope), int(pad_mode))
     return out.permute(0, 3, 1, 2)

@@ -445,11 +445,18 @@ int b3d_leaky_bwd(const float* gy, const float* y, float* out, long long n, floa
 // Per-channel fp64 sums and sums of squares of an NHWC activation for the (Sync)BatchNorm layers (models/gan.py:211-232 ->
 // F.batch_norm / sync_batchnorm/batchnorm.py:150) in one pass over the tensor.  Threads own a channel quad and stride over
 // the pixels (fp32 partial sums of ~50-100 values), a block folds its pixel lanes in shared memory and adds into fp64
-// accumulators.
+// accumulators.  PER_SAMPLE (InstanceNorm2d, models/gan.py:302 / :58): blockIdx.y is the sample, `rows` its pixel count,
+// and sample n's sums go to ws + n * 2C — the same pass with the sample index kept.  The pixel loop is bounded by `rows`,
+// so a sample smaller than one CTA's pixel range (blk1: 8 x 4 = 32 pixels) leaves the surplus lanes at zero.
 // ------------------------------------------------------------------------------------------------------------------
 namespace {
+template <bool PER_SAMPLE>
 __global__ void __launch_bounds__(NT)
 bn_sums_kernel(const float4* __restrict__ y, long long rows, int C4, double* __restrict__ ws) {
+    if (PER_SAMPLE) {
+        y += (long long)blockIdx.y * rows * C4;
+        ws += (long long)blockIdx.y * 8 * C4;
+    }
     __shared__ float4 rs[NT], rq[NT];
     const int c = threadIdx.x % C4, lane_p = threadIdx.x / C4, PPB = NT / C4;
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = s;
@@ -494,6 +501,9 @@ bn_sums_kernel(const float4* __restrict__ y, long long rows, int C4, double* __r
 // mode 0: eval (running statistics).  mode 1: batch statistics from fp64 sums [2][C] over `count` values per channel with
 // F.batch_norm's formulas (biased variance + eps under the root; running variance unbiased).  mode 2: the reference's
 // SyncBN formulas on the (all-reduced) sums: inv_std = clamp(var, eps)^-1/2 (sync_batchnorm/batchnorm.py:133-150).
+// mode 3: instance statistics (InstanceNorm2d without running buffers, so in eval mode too): mode 1's formulas on sample n's
+// sums [N][2][C] over `count` = H*W values.  mode 4: no normalisation (norm_g 'none'): mean 0, inv_std 1.  Modes 3 and 4
+// write mean / inv_std as [N, C] rows and never touch running buffers.
 // momentum < 0 selects torch's cumulative average (BatchNorm momentum=None): factor 1 / (num_batches_tracked + 1).
 __device__ __forceinline__ void cbn_batch_stats(const double* __restrict__ sums, double count, float eps, int mode, int C, int c,
                                                 float& mean, float& invstd, double& var_b) {
@@ -522,6 +532,11 @@ cbn_prepare_kernel(const float* __restrict__ gb, int gb_pitch, int gamma_off, in
         if (mode == 0) {
             mean = running_mean[c];
             invstd = rsqrtf(running_var[c] + eps);
+        } else if (mode == 3) {                              // instance statistics: sample n's sums, F.batch_norm's formulas
+            cbn_batch_stats(sums + (long long)n * 2 * C, count, eps, 1, C, c, mean, invstd, var_b);
+        } else if (mode == 4) {                              // no normalisation
+            mean = 0.f;
+            invstd = 1.f;
         } else {
             cbn_batch_stats(sums, count, eps, mode, C, c, mean, invstd, var_b);
         }
@@ -530,14 +545,17 @@ cbn_prepare_kernel(const float* __restrict__ gb, int gb_pitch, int gamma_off, in
         scale[i] = sc;
         shift[i] = gb[(long long)n * gb_pitch + beta_off + c] - mean * sc;
         gt[i] = g1;
-        if (n == 0) {
+        if (mode >= 3) {                                     // per-sample rows [N, C]
+            mean_out[i] = mean;
+            invstd_out[i] = invstd;
+        } else if (n == 0) {
             mean_out[c] = mean;
             invstd_out[c] = invstd;
         }
     }
     // Running buffers (modes 1, 2; mode 0 is the only one that reads them above): block 0 alone updates every channel, so
     // all its threads read num_batches_tracked (the momentum=None factor) before the barrier and thread 0 increments after it.
-    if (blockIdx.x == 0 && mode != 0 && running_mean != nullptr) {
+    if (blockIdx.x == 0 && (mode == 1 || mode == 2) && running_mean != nullptr) {
         const float f = cbn_momentum(momentum, nbt);
         for (int c = threadIdx.x; c < C; c += NT) {
             float mean, invstd;
@@ -700,6 +718,9 @@ struct CbnGeom {
 
 __device__ __forceinline__ float lk(float v, float s) { return v >= 0.f ? v : v * s; }
 
+// PM: x-padding mode of the output, 0 = replicate (symmetric generator), 1 = circular (asymmetric generator, discriminators;
+// the column is wrapped in upsampled coordinates, as circpad applied after F.interpolate).
+template <int PM>
 __global__ void __launch_bounds__(NT)
 cbn_act_fwd_kernel(const float4* __restrict__ y, const float4* __restrict__ scale, const float4* __restrict__ shift,
                    const float4* __restrict__ skip, float4* __restrict__ out, const CbnGeom g) {
@@ -712,8 +733,7 @@ cbn_act_fwd_kernel(const float4* __restrict__ y, const float4* __restrict__ scal
         t /= Wo;
         const int yo = (int)(t % Ho);
         const int n = (int)(t / Ho);
-        int xs = xo - g.pad;
-        xs = xs < 0 ? 0 : (xs >= g.up * g.W ? g.up * g.W - 1 : xs);
+        int xs = src_col(xo, g.pad, g.up * g.W, PM);
         const int ys = yo / g.up;
         xs /= g.up;
         const float4 v = __ldg(y + (((long long)n * g.H + ys) * g.W + xs) * g.C4 + c);
@@ -732,6 +752,7 @@ cbn_act_fwd_kernel(const float4* __restrict__ y, const float4* __restrict__ scal
 // Same pass with the index arithmetic hoisted: one block walks output rows (n, yo), a thread owns channel quad
 // c = tid % C4 for the pixels tid / C4, + NT / C4, ... (needs NT % C4 == 0) — no 64-bit divisions per element, the
 // per-sample scale / shift stay in registers along the row.
+template <int PM>
 __global__ void __launch_bounds__(NT)
 cbn_act_fwd_rows_kernel(const float4* __restrict__ y, const float4* __restrict__ scale, const float4* __restrict__ shift,
                         const float4* __restrict__ skip, float4* __restrict__ out, const CbnGeom g) {
@@ -751,8 +772,7 @@ cbn_act_fwd_rows_kernel(const float4* __restrict__ y, const float4* __restrict__
             for (int u = 0; u < U; ++u) {
                 const int xo = xb + u * PPB;
                 if (xo >= Wo) continue;
-                int xs = xo - g.pad;
-                xs = xs < 0 ? 0 : (xs >= Wu ? Wu - 1 : xs);
+                int xs = src_col(xo, g.pad, Wu, PM);
                 xs = g.up == 2 ? xs >> 1 : xs;
                 v[u] = __ldg(yrow + (long long)xs * g.C4);
                 if (srow) k[u] = __ldg(srow + (long long)xs * g.C4);
@@ -774,6 +794,9 @@ cbn_act_fwd_rows_kernel(const float4* __restrict__ y, const float4* __restrict__
 // Backward pass 1.  Per input pixel: gather the gradient of its up x up children (+ the replicate-pad columns), undo the
 // activations, write ga = d/d(pre-activation) and (optionally) gskip; accumulate S1[n,c] = sum ga, S2[n,c] = sum ga * xhat
 // with xhat = (y - mean) * inv_std.  One CTA walks `rows_per_cta` image rows of one sample, threads own channel quads.
+// PM: the forward's pad mode; with circular padding (1) every pad column is folded back onto the upsampled column it wraps
+// from (the order interior, right pad, left pad of b3d_pad_x_bwd).  PS: mean / inv_std are per-sample rows [N, C].
+template <int PM, bool PS>
 __global__ void __launch_bounds__(NT)
 cbn_act_bwd1_kernel(const float4* __restrict__ gout, const float4* __restrict__ y, const float4* __restrict__ scale,
                     const float4* __restrict__ shift, const float4* __restrict__ skip, const float4* __restrict__ mean,
@@ -781,22 +804,38 @@ cbn_act_bwd1_kernel(const float4* __restrict__ gout, const float4* __restrict__ 
                     int gskip_off, float* __restrict__ S1, float* __restrict__ S2, int s_pitch, const CbnGeom g, int rows_per_cta) {
     const int n = blockIdx.y;
     const int y0 = blockIdx.x * rows_per_cta, y1 = min(y0 + rows_per_cta, g.H);
-    const int Wo = g.up * g.W + 2 * g.pad;
+    const int Wu = g.up * g.W, Wo = Wu + 2 * g.pad;
     for (int c = threadIdx.x % g.C4, lane_px = threadIdx.x / g.C4, px_step = NT / g.C4; c < g.C4; c += g.C4) {
         const float4 sc = __ldg(scale + (long long)n * g.C4 + c), sh = __ldg(shift + (long long)n * g.C4 + c);
-        const float4 mu = __ldg(mean + c), is = __ldg(invstd + c);
+        const long long so = PS ? (long long)n * g.C4 + c : c;
+        const float4 mu = __ldg(mean + so), is = __ldg(invstd + so);
         float4 a1 = make_float4(0.f, 0.f, 0.f, 0.f), a2 = a1;
         for (int p = y0 * g.W + lane_px; p < y1 * g.W; p += px_step) {
             const int ys = p / g.W, xs = p % g.W;
             float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
             for (int i = 0; i < g.up; ++i) {
                 const float4* row = gout + (((long long)n * g.up * g.H + g.up * ys + i) * Wo) * g.C4 + c;
-                int lo = g.up * xs + g.pad, hi = lo + g.up;          // children columns [lo, hi)
-                if (xs == 0) lo = 0;                                  // left pad columns replicate column 0
-                if (xs == g.W - 1) hi = Wo;                           // right pad columns replicate the last column
-                for (int xo = lo; xo < hi; ++xo) {
-                    const float4 v = __ldg(row + (long long)xo * g.C4);
-                    s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+                if (PM == 0) {
+                    int lo = g.up * xs + g.pad, hi = lo + g.up;      // children columns [lo, hi)
+                    if (xs == 0) lo = 0;                              // left pad columns replicate column 0
+                    if (xs == g.W - 1) hi = Wo;                       // right pad columns replicate the last column
+                    for (int xo = lo; xo < hi; ++xo) {
+                        const float4 v = __ldg(row + (long long)xo * g.C4);
+                        s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+                    }
+                } else {
+                    for (int u = g.up * xs; u < g.up * xs + g.up; ++u) {   // upsampled column u: interior + its copies
+                        float4 v = __ldg(row + (long long)(u + g.pad) * g.C4);
+                        s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+                        if (u < g.pad) {                              // right pad column Wu + pad + u
+                            v = __ldg(row + (long long)(u + g.pad + Wu) * g.C4);
+                            s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+                        }
+                        if (u >= Wu - g.pad) {                        // left pad column u + pad - Wu
+                            v = __ldg(row + (long long)(u + g.pad - Wu) * g.C4);
+                            s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+                        }
+                    }
                 }
             }
             const long long idx = (((long long)n * g.H + ys) * g.W + xs) * g.C4 + c;
@@ -825,17 +864,26 @@ cbn_act_bwd1_kernel(const float4* __restrict__ gout, const float4* __restrict__ 
     }
 }
 
-// Backward pass 2 (in place on ga): dy = inv_std * (ga * gamma_t - m1 - xhat * m2), (m1, m2) = red[0 / 1] * inv_m
+// Backward pass 2 (in place on ga): dy = inv_std * (ga * gamma_t - m1 - xhat * m2), (m1, m2) = red[0 / 1] * inv_m.
+// PS (instance / no normalisation): mean / inv_std are rows [N, C], and the coupling terms are per sample,
+// (m1, m2)[n,c] = inv_m * gamma_t[n,c] * (S1, S2)[n,c] read from bwd1's sums at row pitch m4 (float4s) — no reduction
+// across samples is needed.  inv_m = 0 drops them (no normalisation).
+template <bool PS>
 __global__ void __launch_bounds__(NT)
 cbn_act_bwd2_kernel(float4* __restrict__ ga, const float4* __restrict__ y, const float4* __restrict__ gamma_t,
                     const float4* __restrict__ mean, const float4* __restrict__ invstd, const float4* __restrict__ m1,
-                    const float4* __restrict__ m2, float inv_m, long long per_n, int C4, long long total) {
+                    const float4* __restrict__ m2, int m4, float inv_m, long long per_n, int C4, long long total) {
     for (long long i = (long long)blockIdx.x * NT + threadIdx.x; i < total; i += (long long)gridDim.x * NT) {
         const int c = (int)(i % C4);
         const long long n = i / per_n;
         const float4 a = ga[i], v = __ldg(y + i), gt = __ldg(gamma_t + n * C4 + c);
-        const float4 mu = __ldg(mean + c), is = __ldg(invstd + c);
-        float4 q1 = __ldg(m1 + c), q2 = __ldg(m2 + c);
+        const long long so = PS ? n * C4 + c : c;
+        const float4 mu = __ldg(mean + so), is = __ldg(invstd + so);
+        float4 q1 = __ldg(m1 + (PS ? n * m4 + c : c)), q2 = __ldg(m2 + (PS ? n * m4 + c : c));
+        if (PS) {
+            q1.x *= gt.x; q1.y *= gt.y; q1.z *= gt.z; q1.w *= gt.w;
+            q2.x *= gt.x; q2.y *= gt.y; q2.z *= gt.z; q2.w *= gt.w;
+        }
         q1.x *= inv_m; q1.y *= inv_m; q1.z *= inv_m; q1.w *= inv_m;
         q2.x *= inv_m; q2.y *= inv_m; q2.z *= inv_m; q2.w *= inv_m;
         ga[i] = make_float4(is.x * (a.x * gt.x - q1.x - (v.x - mu.x) * is.x * q2.x), is.y * (a.y * gt.y - q1.y - (v.y - mu.y) * is.y * q2.y),
@@ -845,34 +893,54 @@ cbn_act_bwd2_kernel(float4* __restrict__ ga, const float4* __restrict__ y, const
 }  // namespace
 
 extern "C" {
-int b3d_cbn_act_fwd(const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch, int skip_off,
-                    float* out, int N, int H, int W, int C, int up, int pad, float slope, int post_leaky, void* stream) {
+int b3d_cbn_act_fwd_ex(const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch, int skip_off,
+                       float* out, int N, int H, int W, int C, int up, int pad, int pad_mode, float slope, int post_leaky,
+                       void* stream) {
     B3D_REQUIRE(N >= 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0 && (up == 1 || up == 2) && pad >= 0, B3D_EINVAL,
                 "b3d_cbn_act_fwd: bad arguments");
+    B3D_REQUIRE(pad_mode == 0 || (pad_mode == 1 && pad <= up * W), B3D_EINVAL, "b3d_cbn_act_fwd: pad mode %d with pad %d > %d columns",
+                pad_mode, pad, up * W);
     if (N == 0) return B3D_OK;
     B3D_REQUIRE(y && scale && shift && out && (skip != nullptr) == (skip_pitch != 0), B3D_EINVAL, "b3d_cbn_act_fwd: null pointer");
     CbnGeom g{N, H, W, C / 4, up, pad, skip_pitch, skip_off, slope, post_leaky};
     const long long total = (long long)N * up * H * (up * W + 2 * pad) * (C / 4);
+    cudaStream_t st = (cudaStream_t)stream;
     if (g.C4 <= NT && NT % g.C4 == 0 && (up == 1 || up == 2)) {
-        const int rows = N * up * H;
-        cbn_act_fwd_rows_kernel<<<rows < 132 * 16 ? rows : 132 * 16, NT, 0, (cudaStream_t)stream>>>(
-            (const float4*)y, (const float4*)scale, (const float4*)shift, (const float4*)skip, (float4*)out, g);
+        const int rows = N * up * H, grid = rows < 132 * 16 ? rows : 132 * 16;
+        if (pad_mode == 0)
+            cbn_act_fwd_rows_kernel<0><<<grid, NT, 0, st>>>((const float4*)y, (const float4*)scale, (const float4*)shift,
+                                                            (const float4*)skip, (float4*)out, g);
+        else
+            cbn_act_fwd_rows_kernel<1><<<grid, NT, 0, st>>>((const float4*)y, (const float4*)scale, (const float4*)shift,
+                                                            (const float4*)skip, (float4*)out, g);
+    } else if (pad_mode == 0) {
+        cbn_act_fwd_kernel<0><<<grid_for(total), NT, 0, st>>>((const float4*)y, (const float4*)scale, (const float4*)shift,
+                                                              (const float4*)skip, (float4*)out, g);
     } else {
-        cbn_act_fwd_kernel<<<grid_for(total), NT, 0, (cudaStream_t)stream>>>((const float4*)y, (const float4*)scale, (const float4*)shift,
-                                                                           (const float4*)skip, (float4*)out, g);
+        cbn_act_fwd_kernel<1><<<grid_for(total), NT, 0, st>>>((const float4*)y, (const float4*)scale, (const float4*)shift,
+                                                              (const float4*)skip, (float4*)out, g);
     }
     B3D_LAUNCH_OK();
     return B3D_OK;
 }
 
+int b3d_cbn_act_fwd(const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch, int skip_off,
+                    float* out, int N, int H, int W, int C, int up, int pad, float slope, int post_leaky, void* stream) {
+    return b3d_cbn_act_fwd_ex(y, scale, shift, skip, skip_pitch, skip_off, out, N, H, W, C, up, pad, 0, slope, post_leaky, stream);
+}
+
 // S1, S2 [N,C] are zeroed by the call; gskip (nullable) is written at pixel offset gskip_off with row pitch gskip_pitch
-// (its pad columns are NOT touched: the caller zeroes the buffer when gskip_pitch != W)
-int b3d_cbn_act_bwd1(const float* gout, const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch,
-                     int skip_off, const float* mean, const float* invstd, float* ga, float* gskip, int gskip_pitch, int gskip_off,
-                     float* S1, float* S2, int s_pitch, int N, int H, int W, int C, int up, int pad, float slope, int post_leaky,
-                     void* stream) {
+// (its pad columns are NOT touched: the caller zeroes the buffer when gskip_pitch != W).  stat_pitch: row pitch of mean /
+// inv_std, 0 = one row for all samples (batch statistics), C = per-sample rows (instance / no normalisation).
+int b3d_cbn_act_bwd1_ex(const float* gout, const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch,
+                        int skip_off, const float* mean, const float* invstd, int stat_pitch, float* ga, float* gskip, int gskip_pitch,
+                        int gskip_off, float* S1, float* S2, int s_pitch, int N, int H, int W, int C, int up, int pad, int pad_mode,
+                        float slope, int post_leaky, void* stream) {
     B3D_REQUIRE(N >= 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0 && C / 4 <= NT && NT % (C / 4) == 0 && (up == 1 || up == 2), B3D_EINVAL,
                 "b3d_cbn_act_bwd1: bad arguments (C/4 must divide %d)", NT);
+    B3D_REQUIRE(stat_pitch == 0 || stat_pitch == C, B3D_EINVAL, "b3d_cbn_act_bwd1: statistics pitch %d must be 0 or C=%d", stat_pitch, C);
+    B3D_REQUIRE(pad >= 0 && (pad_mode == 0 || (pad_mode == 1 && pad <= up * W)), B3D_EINVAL,
+                "b3d_cbn_act_bwd1: pad mode %d with pad %d > %d columns", pad_mode, pad, up * W);
     if (N == 0) return B3D_OK;
     B3D_REQUIRE(gout && y && scale && shift && mean && invstd && ga && S1 && S2, B3D_EINVAL, "b3d_cbn_act_bwd1: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
@@ -884,24 +952,44 @@ int b3d_cbn_act_bwd1(const float* gout, const float* y, const float* scale, cons
     int rows = (int)(((long long)N * H + 132 * 8 - 1) / (132 * 8));
     rows = rows < 1 ? 1 : rows;
     dim3 grid(b3d::ceil_div(H, rows), N);
-    cbn_act_bwd1_kernel<<<grid, NT, 0, st>>>((const float4*)gout, (const float4*)y, (const float4*)scale, (const float4*)shift,
-                                            (const float4*)skip, (const float4*)mean, (const float4*)invstd, (float4*)ga,
-                                            (float4*)gskip, gskip_pitch, gskip_off, S1, S2, s_pitch, g, rows);
+    auto kernel = pad_mode == 0 ? (stat_pitch ? cbn_act_bwd1_kernel<0, true> : cbn_act_bwd1_kernel<0, false>)
+                                : (stat_pitch ? cbn_act_bwd1_kernel<1, true> : cbn_act_bwd1_kernel<1, false>);
+    kernel<<<grid, NT, 0, st>>>((const float4*)gout, (const float4*)y, (const float4*)scale, (const float4*)shift, (const float4*)skip,
+                                (const float4*)mean, (const float4*)invstd, (float4*)ga, (float4*)gskip, gskip_pitch, gskip_off, S1, S2,
+                                s_pitch, g, rows);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+int b3d_cbn_act_bwd1(const float* gout, const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch,
+                     int skip_off, const float* mean, const float* invstd, float* ga, float* gskip, int gskip_pitch, int gskip_off,
+                     float* S1, float* S2, int s_pitch, int N, int H, int W, int C, int up, int pad, float slope, int post_leaky,
+                     void* stream) {
+    return b3d_cbn_act_bwd1_ex(gout, y, scale, shift, skip, skip_pitch, skip_off, mean, invstd, 0, ga, gskip, gskip_pitch, gskip_off,
+                               S1, S2, s_pitch, N, H, W, C, up, pad, 0, slope, post_leaky, stream);
+}
+
+// stat_pitch 0: mean / inv_std / m1 / m2 are [C] (batch statistics; m1, m2 = b3d_cbn_bwd_reduce's rows).  stat_pitch C:
+// mean / inv_std are [N, C] and m1, m2 are bwd1's per-sample sums S1, S2 at row pitch m_pitch (a multiple of 4).
+int b3d_cbn_act_bwd2_ex(float* ga, const float* y, const float* gamma_t, const float* mean, const float* invstd, int stat_pitch,
+                        const float* m1, const float* m2, int m_pitch, float inv_m, int N, int H, int W, int C, void* stream) {
+    B3D_REQUIRE(N >= 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, B3D_EINVAL, "b3d_cbn_act_bwd2: bad arguments");
+    B3D_REQUIRE(stat_pitch == 0 || (stat_pitch == C && m_pitch >= C && m_pitch % 4 == 0), B3D_EINVAL,
+                "b3d_cbn_act_bwd2: statistics pitch %d must be 0 or C=%d (sums pitch %d >= C, a multiple of 4)", stat_pitch, C, m_pitch);
+    if (N == 0) return B3D_OK;
+    B3D_REQUIRE(ga && y && gamma_t && mean && invstd && m1 && m2, B3D_EINVAL, "b3d_cbn_act_bwd2: null pointer");
+    const long long per_n = (long long)H * W * (C / 4), total = per_n * N;
+    auto kernel = stat_pitch ? cbn_act_bwd2_kernel<true> : cbn_act_bwd2_kernel<false>;
+    kernel<<<grid_for(total), NT, 0, (cudaStream_t)stream>>>((float4*)ga, (const float4*)y, (const float4*)gamma_t, (const float4*)mean,
+                                                             (const float4*)invstd, (const float4*)m1, (const float4*)m2, m_pitch / 4,
+                                                             inv_m, per_n, C / 4, total);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }
 
 int b3d_cbn_act_bwd2(float* ga, const float* y, const float* gamma_t, const float* mean, const float* invstd, const float* m1,
                      const float* m2, float inv_m, int N, int H, int W, int C, void* stream) {
-    B3D_REQUIRE(N >= 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, B3D_EINVAL, "b3d_cbn_act_bwd2: bad arguments");
-    if (N == 0) return B3D_OK;
-    B3D_REQUIRE(ga && y && gamma_t && mean && invstd && m1 && m2, B3D_EINVAL, "b3d_cbn_act_bwd2: null pointer");
-    const long long per_n = (long long)H * W * (C / 4), total = per_n * N;
-    cbn_act_bwd2_kernel<<<grid_for(total), NT, 0, (cudaStream_t)stream>>>((float4*)ga, (const float4*)y, (const float4*)gamma_t,
-                                                                         (const float4*)mean, (const float4*)invstd,
-                                                                         (const float4*)m1, (const float4*)m2, inv_m, per_n, C / 4, total);
-    B3D_LAUNCH_OK();
-    return B3D_OK;
+    return b3d_cbn_act_bwd2_ex(ga, y, gamma_t, mean, invstd, 0, m1, m2, 0, inv_m, N, H, W, C, stream);
 }
 
 // fp64 per-channel sums [2][C] (sum, sum of squares) of y [rows, C], for callers that all-reduce the sums across ranks
@@ -916,7 +1004,25 @@ int b3d_bn_sums(const float* y, long long rows, int C, double* sums, void* strea
     const int ppb = NT / (C / 4);
     long long blocks = (rows + ppb - 1) / ppb;
     if (blocks > 132 * 2) blocks = 132 * 2;                 // few blocks: every block ends with 2C same-address fp64 atomics
-    bn_sums_kernel<<<(int)blocks, NT, 0, st>>>((const float4*)y, rows, C / 4, sums);
+    bn_sums_kernel<false><<<(int)blocks, NT, 0, st>>>((const float4*)y, rows, C / 4, sums);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+// fp64 per-(sample, channel) sums [N][2][C] of y [N, HW, C] (InstanceNorm2d statistics, finished by b3d_cbn_prepare mode 3).
+// `sums` is zeroed here.  About 264 CTAs in all, split over the samples, at least one per sample.
+int b3d_bn_sums_per_sample(const float* y, int N, long long HW, int C, double* sums, void* stream) {
+    B3D_REQUIRE(N > 0 && N <= 65535 && HW > 0 && C >= 4 && C % 4 == 0 && C / 4 <= NT && NT % (C / 4) == 0, B3D_EINVAL,
+                "b3d_bn_sums_per_sample: N=%d (1..65535), C=%d must be 4 * a divisor of %d", N, C, NT);
+    B3D_REQUIRE(y && sums, B3D_EINVAL, "b3d_bn_sums_per_sample: null pointer");
+    B3D_CHECK_ALIGNED(y);
+    cudaStream_t st = (cudaStream_t)stream;
+    B3D_CUDA_OK(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * (size_t)C * N, st));
+    const int ppb = NT / (C / 4);
+    long long blocks = (HW + ppb - 1) / ppb;
+    const long long cap = (132 * 2 + N - 1) / N;
+    if (blocks > cap) blocks = cap;
+    bn_sums_kernel<true><<<dim3((unsigned)blocks, (unsigned)N), NT, 0, st>>>((const float4*)y, HW, C / 4, sums);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }
@@ -925,12 +1031,14 @@ int b3d_bn_sums(const float* y, long long rows, int C, double* sums, void* strea
 // gamma_off + c and beta at beta_off + c (the batched fc_gamma / fc_beta outputs of all layers).  mode 0 eval, 1 batch
 // statistics (F.batch_norm formulas), 2 the reference's SyncBN formulas; sums [2][C] fp64 (modes 1, 2), count = values per
 // channel over the (global) batch.  running_mean / running_var / num_batches_tracked (nullable) are updated in modes 1, 2.
-// Outputs: mean, invstd [C]; scale, shift, gt [N, C].
+// mode 3 instance statistics from sums [N][2][C] (b3d_bn_sums_per_sample), count = H*W; mode 4 no normalisation.
+// Outputs: mean, invstd [C] ([N, C] in modes 3, 4); scale, shift, gt [N, C].
 int b3d_cbn_prepare(const float* gb, int gb_pitch, int gamma_off, int beta_off, const double* sums, double count, float eps,
                     float momentum, int mode, float* running_mean, float* running_var, long long* num_batches_tracked,
                     float* mean, float* invstd, float* scale, float* shift, float* gt, int N, int C, void* stream) {
     B3D_REQUIRE(N > 0 && C > 0 && gb && mean && invstd && scale && shift && gt, B3D_EINVAL, "b3d_cbn_prepare: bad arguments");
-    B3D_REQUIRE(mode == 0 ? (running_mean && running_var) : (sums != nullptr && count > 0), B3D_EINVAL,
+    B3D_REQUIRE(mode >= 0 && mode <= 4, B3D_EINVAL, "b3d_cbn_prepare: unknown mode %d", mode);
+    B3D_REQUIRE(mode == 0 ? (running_mean && running_var) : (mode == 4 || (sums != nullptr && count > 0)), B3D_EINVAL,
                 "b3d_cbn_prepare: mode %d needs %s", mode, mode == 0 ? "running statistics" : "sums and a count");
     cbn_prepare_kernel<<<(N * C + NT - 1) / NT, NT, 0, (cudaStream_t)stream>>>(gb, gb_pitch, gamma_off, beta_off, sums, count, eps,
                                                                                 momentum, mode, running_mean, running_var,

@@ -7,8 +7,8 @@ Module tree, parameter and buffer names equal the reference's, so its checkpoint
 `emb_class.weight`, `fc.weight`, ... — SURVEY.md §8b).  Spectral normalisation is torch's own
 nn.utils.spectral_norm hook (parameter plumbing, one mat-vec per layer), as in the reference.
 Activations stay logically NCHW (the reference's interface) and physically channels-last, which is what the
-kernels read; x-padding (replicate for the symmetric generator, circular for the discriminators) is explicit
-as in the reference, y-padding is the convolution's zero padding (TMA out-of-bounds fill).
+kernels read; x-padding (replicate for the symmetric generator, circular for the asymmetric one and the discriminators)
+is explicit as in the reference, y-padding is the convolution's zero padding (TMA out-of-bounds fill).
 """
 import math
 
@@ -20,7 +20,7 @@ from b3d import B3DError
 from b3d.bank import WeightBank
 from b3d.conv import conv2d as _tc_conv2d
 from b3d.conv import ActLink, conv2d_banked
-from b3d.ew import CIRCULAR, REPLICATE, CBNBatch, cbn_act_pad, pad_x, stem_input
+from b3d.ew import CIRCULAR, REPLICATE, CBNBatch, cbn_act_pad, identity_norm, in_act_pad, norm_kind, pad_x, stem_input
 from rendering.utils import adjust_poles, symmetrize_texture
 
 
@@ -62,7 +62,9 @@ def _norm_and_bias(args):
 
 
 def _conv_norm_act(conv, norm, x, pad_next=0, lw=None, link_in=None, link_out=None):
-    """pad_x(LeakyReLU(0.2)(norm(conv(x))), pad_next, circular): one fused kernel when there is no norm layer.
+    """pad_x(LeakyReLU(0.2)(norm(conv(x))), pad_next, circular): one fused kernel when there is no norm layer; with an
+    instance norm (norm_d='instance'), the convolution, one per-sample statistics pass, and one pass for normalise + affine +
+    LeakyReLU + padding into the next layer's input buffer (b3d.ew.in_act_pad).
     lw: the layer's weights from the network's WeightBank (spectral norm + kernel layouts done for all layers at once);
     None = the module's own forward (torch's spectral-norm hook).
     link_in / link_out (b3d.conv.ActLink, banked layers only): this layer's input is the sole use of the previous layer's
@@ -75,6 +77,8 @@ def _conv_norm_act(conv, norm, x, pad_next=0, lw=None, link_in=None, link_out=No
         run = lambda **kw: conv(x, **kw)
     if norm is None and conv.out_channels in (16, 32, 64, 128, 256, 512, 1024):
         return run(leaky=0.2, pad_out=pad_next, pad_mode=CIRCULAR)
+    if norm_kind(norm) == 'instance' and norm.affine and conv.out_channels in (16, 32, 64, 128, 256, 512, 1024):
+        return in_act_pad(run(), norm, pad_next, CIRCULAR, 0.2)
     y = run(leaky=0.2) if norm is None else F.leaky_relu(norm(run()), 0.2)
     return pad_x(y, pad_next, CIRCULAR) if pad_next else y
 
@@ -302,7 +306,7 @@ class ConditionalBatchNorm2d(nn.Module):
         elif kind == 'instance':
             self.norm = nn.InstanceNorm2d(ch, affine=False)
         elif kind == 'none':
-            self.norm = lambda x: x
+            self.norm = identity_norm
         else:
             raise ValueError(f"norm_g={kind!r}")
         self.fc_gamma = nn.Linear(emb_dim, ch)
@@ -335,13 +339,14 @@ class ResBlockUp(nn.Module):
         return h + skip
 
     def fusable(self):
-        from torch.nn.modules.batchnorm import _BatchNorm
-        return isinstance(self.norm1.norm, _BatchNorm) and isinstance(self.norm2.norm, _BatchNorm)
+        """Every norm_g the reference offers (batch, syncbatch, instance, none) runs on the fused glue."""
+        return norm_kind(self.norm1.norm) is not None and norm_kind(self.norm2.norm) is not None
 
-    def forward_fused(self, xp, z, up, pad_next, post_leaky=False, W=None, prefix="", cb=None):
-        """Same block on an input that is ALREADY replicate-padded by 1 (xp = pad(x, 1)); returns the padded input of the
-        consumer: pad(up(out), pad_next) with out = [LeakyReLU](h + skip).  Every conv output goes through exactly one fused
-        elementwise kernel (b3d.ew.cbn_act_pad) instead of BN, affine, LeakyReLU, add, upsample and pad kernels."""
+    def forward_fused(self, xp, z, up, pad_next, post_leaky=False, W=None, prefix="", cb=None, pad_mode=REPLICATE):
+        """Same block on an input that is ALREADY x-padded by 1 (xp = pad(x, 1), replicate or circular = pad_mode); returns
+        the padded input of the consumer: pad(up(out), pad_next) with out = [LeakyReLU](h + skip).  Every conv output goes
+        through exactly one fused elementwise kernel (b3d.ew.cbn_act_pad) instead of norm, affine, LeakyReLU, add, upsample
+        and pad kernels."""
         s1 = s2 = None
         if W is not None:
             # the conv epilogues accumulate the batch-norm statistics of their output (no separate pass over y)
@@ -353,14 +358,14 @@ class ResBlockUp(nn.Module):
         else:
             c1, c2, sc = self.conv1, self.conv2, (lambda t: self.shortcut(t, x_crop=1))
         y1 = c1(xp)
-        a = cbn_act_pad(y1, self.norm1, z, up=1, pad=1, cb=cb, sums=s1)
+        a = cbn_act_pad(y1, self.norm1, z, up=1, pad=1, cb=cb, sums=s1, pad_mode=pad_mode)
         y2 = c2(a)
         if isinstance(self.shortcut, nn.Module):
             skip, off = sc(xp), 0                                    # 1x1 conv on the interior of the padded input
         else:
             skip, off = xp, 1                                        # identity: read the interior of the padded input
         return cbn_act_pad(y2, self.norm2, z, skip_nchw=skip, skip_off=off, up=up, pad=pad_next, post_leaky=post_leaky, cb=cb,
-                           sums=s2)
+                           sums=s2, pad_mode=pad_mode)
 
 
 class Generator(nn.Module):
@@ -419,7 +424,7 @@ class Generator(nn.Module):
 
         x = self.fc(z).view(z.shape[0], -1, self.height, self.width)
         x = x.contiguous(memory_format=torch.channels_last)
-        if self.symmetric and not a.conditional_text and self.blk1.fusable() and not getattr(self, 'disable_fusion', False):
+        if not a.conditional_text and self.blk1.fusable() and not getattr(self, 'disable_fusion', False):
             return self._forward_fused(x, z, return_attention)
         x = self.up(self.blk1(x, z))
         x = self.blk2(x, z)
@@ -472,17 +477,20 @@ class Generator(nn.Module):
         return bank.forward(self.training)
 
     def _forward_fused(self, x, z, return_attention):
-        """The same network with the inter-convolution glue fused (replicate-padded tensors flow between the blocks) and the
-        weights of all convolutions prepared by one WeightBank pass."""
+        """The same network with the inter-convolution glue fused (x-padded tensors flow between the blocks: replicate for the
+        symmetric half-width map, circular for the full-width one) and the weights of all convolutions prepared by one
+        WeightBank pass."""
         W = self._weights()
+        pm = REPLICATE if self.symmetric else CIRCULAR
         names = [n for n in ('blk1', 'blk2', 'blk3a', 'blk3b', 'blk3c', 'blk4', 'blk5', 'blk6') if hasattr(self, n)]
         if self.mesh_head:
             names.append('blk3_mesh')
         # gamma / beta of all conditional batch norms from one GEMM (blk1.norm1 first: it closes the gradient sink)
         cb = CBNBatch([m for n in names for m in (getattr(self, n).norm1, getattr(self, n).norm2)], z)
-        blk = lambda name, inp, **kw: getattr(self, name).forward_fused(inp, z, W=W, prefix=name, cb=cb, **kw)
+        blk = lambda name, inp, **kw: getattr(self, name).forward_fused(inp, z, W=W, prefix=name, cb=cb, pad_mode=pm, **kw)
         head = (lambda conv, name, inp: conv(inp)) if W is None else (lambda conv, name, inp: conv2d_banked(inp, W[name], pad_y=2))
-        p = pad_x(x, 1, REPLICATE)
+        sym = symmetrize_texture if self.symmetric else (lambda t: t)
+        p = pad_x(x, 1, pm)
         p = blk('blk1', p, up=2, pad_next=1)
         p = blk('blk2', p, up=2, pad_next=1)                          # blk2 -> up: shared by the texture and mesh branches
         t = p
@@ -492,11 +500,11 @@ class Generator(nn.Module):
         t = blk('blk4', t, up=2, pad_next=1)
         t = blk('blk5', t, up=2, pad_next=1)
         t = blk('blk6', t, up=1, pad_next=2, post_leaky=True)
-        x_tex = symmetrize_texture(torch.tanh(head(self.conv_final, "conv_final", t)))
+        x_tex = sym(torch.tanh(head(self.conv_final, "conv_final", t)))
         x_mesh = None
         if self.mesh_head:
             m = blk('blk3_mesh', p, up=1, pad_next=2, post_leaky=True)
-            x_mesh = symmetrize_texture(adjust_poles(head(self.conv_mesh, "conv_mesh", m)))
+            x_mesh = sym(adjust_poles(head(self.conv_mesh, "conv_mesh", m)))
         return (x_tex, x_mesh, None) if return_attention else (x_tex, x_mesh)
 
 

@@ -161,15 +161,22 @@ def _dgrad(gy, wd, in_hw, kh, kw, pad_y=0, stride=1, x_crop=0, g_pitch=0, mask=N
     return gx
 
 
-def _wgrad(gy, x, kh, kw, pad_y=0, stride=1, x_crop=0, sink=None, g_pitch=0):
+def _wgrad(gy, x, kh, kw, pad_y=0, stride=1, x_crop=0, sink=None, g_pitch=0, fold_kh=0, fold_cin=0):
     """Weight gradient from gy [N,Hout,Wout,Cout] and the (x-padded) input x [N,H,W,Cin].
     sink = None: returns a new [Cout,Cin,kh,kw] tensor (channel counts that are not multiples of 32 are zero-padded here);
     otherwise the gradient is accumulated into sink, the bank's tap-major [kh*kw][Cout][Cin] buffer.
-    g_pitch > 0: gy is the interior of a padded gradient whose rows are g_pitch pixels apart, read in place."""
+    g_pitch > 0: gy is the interior of a padded gradient whose rows are g_pitch pixels apart, read in place.
+    fold_kh > 0: x is the RAW 8-channel stem input whose fold_kh rows (y padding pad_y) fold into fold_cin channels; the
+    gradient is the folded layer's (kh = 1), computed from the raw input."""
     N, Hout, Wout, Cout = gy.shape
     _, H, W, Cin = x.shape
     tap_major = int(sink is not None)
     st = stream_ptr(gy)
+    if fold_kh:
+        dw = sink if tap_major else torch.zeros(Cout, fold_cin, 1, kw, device=gy.device, dtype=torch.float32)
+        check(_conv_call(lib.b3d_conv2d_wgrad_tf32, ctypes.c_void_p(gy.data_ptr()), ptr(x), ptr(dw), N, H, W, fold_cin, Hout,
+                         Wout, Cout, 1, kw, pad_y, 1, 0, tap_major, fold_kh, g_pitch, st))
+        return dw
     if _thin(Cout, Cin, kh, kw, stride):
         dw = sink if tap_major else torch.zeros(Cout, Cin, kh, kw, device=gy.device, dtype=torch.float32)
         check(_conv_call(lib.b3d_conv2d_thin_wgrad, ptr(gy), ptr(x), ptr(dw), N, H, W, Cin, Hout, Wout, Cout, kh, kw, pad_y,
@@ -234,12 +241,14 @@ class ActLink:
 class _Conv(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w, bias, lw, pad_y, stride, leaky, pad_out, pad_mode, x_crop, stats=None, fold_raw=0, link_in=None,
-                link_out=None):
+                link_out=None, fold_fwd=False):
         """Runs on lw.wf (F [T'][Cout][Cin']); w is the tensor autograd differentiates: lw.wf itself (bank) or the module weight
         lw.wf was laid out from.  Its gradient is accumulated into lw.df when the bank provides that sink, otherwise returned
         as [Cout,Cin,kh,kw].  The input gradient runs on lw.wd, or on the per-tap transpose of lw.wf when there is none.
         fold_raw = kh > 0: x is the RAW 8-channel stem input [N,H,W,8]; the kernels fold the kh vertical taps into the K
-        dimension on the fly (TMA boxes of 4 rows x 8 channels) — the folded tensor never exists (pad_y = the fold's y padding)."""
+        dimension on the fly (TMA boxes of 4 rows x 8 channels) — the folded tensor is not kept (pad_y = the fold's y padding).
+        fold_fwd: the forward alone runs on a folded copy of x (b3d.ew.fold_rows), freed when it returns; the backward still
+        reads the raw input."""
         x = dev(x.detach(), "x")
         Cx = x.shape[3]
         fold_pad = 0
@@ -254,8 +263,12 @@ class _Conv(torch.autograd.Function):
         kh, kw = (1, lw.kw) if lw.fold else (lw.kh, lw.kw)
         if lw.fold:
             pad_y = 0
-        out = _fprop(x, dev(lw.wf.detach(), "weight"), bias.detach() if bias is not None else None, kh, kw, pad_y, stride,
-                     leaky, pad_out, pad_mode, x_crop, stats, fold_raw, fold_pad)
+        wf, b = dev(lw.wf.detach(), "weight"), bias.detach() if bias is not None else None
+        if fold_raw and fold_fwd:
+            from .ew import fold_rows
+            out = _fprop(fold_rows(x, lw.kh, fold_pad, lw.Cinp), wf, b, kh, kw, 0, stride, leaky, pad_out, pad_mode, x_crop, stats)
+        else:
+            out = _fprop(x, wf, b, kh, kw, pad_y, stride, leaky, pad_out, pad_mode, x_crop, stats, fold_raw, fold_pad)
         ctx.save_for_backward(x, out if (leaky != 1.0 or pad_out) else None)
         ctx.lw = lw
         ctx.cfg = (pad_y, stride, Cx, bias is not None, leaky, pad_out, pad_mode, x_crop, kh, kw, fold_raw, fold_pad)
@@ -327,11 +340,12 @@ class _Conv(torch.autograd.Function):
                 gx = gx[..., :Cx]
         if ctx.needs_input_grad[1]:
             if fold_raw:
-                raise B3DError("conv2d: the on-the-fly fold has no weight-gradient kernel (materialise the fold)")
-            gw = _wgrad(gy, x, kh, kw, pad_y, stride, x_crop, lw.df, g_pitch)
+                gw = _wgrad(gy, x, kh, kw, fold_pad, stride, x_crop, lw.df, g_pitch, fold_raw, Cin)
+            else:
+                gw = _wgrad(gy, x, kh, kw, pad_y, stride, x_crop, lw.df, g_pitch)
             if lw.df is None:
                 gw = gw[:, :lw.Cin]                                    # the module weight: drop the zero-padded input channels
-        return gx, gw, gb, None, None, None, None, None, None, None, None, None, None, None
+        return gx, gw, gb, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 def fold_kh_weight(weight, cpad=0):
@@ -373,18 +387,21 @@ def conv2d_banked(x_nchw, lw, pad_y=0, stride=1, leaky=1.0, pad_out=0, pad_mode=
     stats: optional zeroed fp64 tensor [2*Cout]; the conv epilogue accumulates the output's per-channel sum / sum of
     squares into it (the following batch norm's statistics without another pass over the tensor)."""
     x = x_nchw.permute(0, 2, 3, 1)
-    fold_raw = 0
+    fold_raw, fold_fwd = 0, False
     if lw.fold:
         Wout = x.shape[2] - lw.kw + 1
-        need_wgrad = torch.is_grad_enabled() and lw.wf.requires_grad
-        if (lw.Cin == 8 and stride == 1 and not x_crop and Wout % 128 == 0 and x.shape[0] * x.shape[1] * (Wout // 128) >= 2 * torch.cuda.get_device_properties(x.device).multi_processor_count
-                and not need_wgrad):
-            # 8-channel stems of wide images when no weight gradient is taken (generator step: the discriminator is frozen):
-            # the forward kernel folds the kh rows on the fly (TMA boxes of 4 rows x 8 channels), no folded tensor is written.
+        if (lw.Cin == 8 and lw.kw == 5 and lw.Cinp == 64 and stride == 1 and not x_crop and Wout % 128 == 0
+                and x.shape[0] * x.shape[1] * (Wout // 128) >= 2 * torch.cuda.get_device_properties(x.device).multi_processor_count):
+            # 8-channel stems of wide images: the backward reads the raw input (the weight gradient folds the rows in shared
+            # memory), so no folded tensor is kept.  The forward folds the kh rows on the fly (TMA boxes of 4 rows x 8
+            # channels) when no weight gradient is taken (generator step); when one is (discriminator step), fold_rows plus the
+            # row-window kernel is faster at cfg3's shape (1.68 against 2.13 ms, H100 SXM at 700 W) and its folded copy is
+            # freed as the forward returns.
             fold_raw = lw.kh
+            fold_fwd = torch.is_grad_enabled() and lw.wf.requires_grad
         else:
             from .ew import fold_rows
             x = fold_rows(x, lw.kh, pad_y, lw.Cinp)
     y = _Conv.apply(x, lw.wf, lw.bias, lw, int(pad_y), int(stride), float(leaky), int(pad_out), int(pad_mode), int(x_crop), stats,
-                    fold_raw, link_in, link_out)
+                    fold_raw, link_in, link_out, fold_fwd)
     return y.permute(0, 3, 1, 2)

@@ -419,6 +419,183 @@ int launch_wgrad(const CUtensorMap& mdy, const CUtensorMap& mx, const WgradParam
     return B3D_OK;
 }
 
+// ----------------------------------------------------------------------------------------------
+// Stem wgrad from the RAW 8-channel input (fold_kh > 0): dW'[s][co][r*8 + ci] += sum dY[n,y,x,co] * X[n, y + r - pad_y, x + s, ci]
+// — the weight gradient of the kh-folded stem (kh = 1, kw = 5 taps, Cin' = 64 folded channels) without the folded tensor.
+// GEMM per tap s: M = 64 output channels, N = 64 folded channels (8 fold_kh real, the rest zero), K = output pixels in
+// 32-pixel row segments.  One TMA box {8 ch, 36 px, fold_kh rows} of the raw input per K slice (TMA's zero fill = the y
+// padding; the x padding is in the tensor) is expanded by the producer warpgroup into the five K-major B tiles of the
+// slice (tap s = the window shifted by s pixels), so dY and X are each read once for all taps.  dY is the register A
+// operand as in wgrad_wgmma_kernel (two 32-channel boxes).  The two consumer warpgroups take alternate K slices, each
+// with five 64 x 64 accumulators over the whole 64-channel tile; both are reduced into dW by fp32 atomics.
+// ----------------------------------------------------------------------------------------------
+constexpr int STEM_KW = 5, STEM_STAGES = 4, STEM_NRAW = 3;
+struct StemSmem {
+    static constexpr int DY_BYTES = 64 * BK * 4;
+    static constexpr int WPX = BK + STEM_KW - 1;                       // raw pixels per K slice: 32 + 4
+    static constexpr int RAW_X_MAX = 8 * WPX * 32;                     // fold_kh <= 8 rows of [36 px][8 ch]
+    static constexpr int RAW_BYTES = (DY_BYTES + RAW_X_MAX + 1023) / 1024 * 1024;
+    static constexpr int TILE_BYTES = 64 * BK * 4;                     // one tap's K-major [64 folded ch][32 px] tile
+    static constexpr int STAGE_BYTES = STEM_KW * TILE_BYTES;
+    static constexpr int TOTAL = STEM_STAGES * STAGE_BYTES + STEM_NRAW * RAW_BYTES + 1024 + 256;
+};
+
+__global__ void __launch_bounds__(NTHREADS, 1)
+wgrad_stem_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x,
+                  const WgradParams p, int fold_kh, float* __restrict__ dw) {
+    using S = StemSmem;
+    extern __shared__ unsigned char smem_raw[];
+    unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    unsigned char* raw = base + STEM_STAGES * S::STAGE_BYTES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(raw + STEM_NRAW * S::RAW_BYTES);
+    uint64_t* empty = full + STEM_STAGES;
+    uint64_t* rawfull = empty + STEM_STAGES;
+    uint64_t* rawempty = rawfull + STEM_NRAW;             // dY fragments loaded: one arrival per warp of the consumer
+
+    const int co0 = blockIdx.x * 64, split = blockIdx.y;
+    const int per_img = p.kx * p.ky;
+    const long long ktotal = (long long)p.N * per_img;
+    const long long k_lo = ktotal * split / p.splits, k_hi = ktotal * (split + 1) / p.splits;
+    const int KI = (int)(k_hi - k_lo);
+    const int creal = 8 * fold_kh;                        // folded channels that hold data
+    const int xbytes = fold_kh * S::WPX * 32;
+
+    if (threadIdx.x == 0) {
+        tc::tma_prefetch_desc(&tmap_dy);
+        tc::tma_prefetch_desc(&tmap_x);
+        for (int i = 0; i < STEM_STAGES; ++i) {
+            tc::mbar_init(full + i, 128);
+            tc::mbar_init(empty + i, 1);
+        }
+        for (int i = 0; i < STEM_NRAW; ++i) {
+            tc::mbar_init(rawfull + i, 1);
+            tc::mbar_init(rawempty + i, 4);
+        }
+        tc::fence_barrier_init();
+    }
+    __syncthreads();
+    const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
+
+    if (wg == 0) {
+        tc::setmaxnreg_dec<56>();
+        auto issue = [&](int j) {
+            if (tid != 0) return;
+            const long long k = k_lo + j;
+            const int n = (int)(k / per_img), rem = (int)(k % per_img);
+            const int x0 = (rem % p.kx) * BK, y0 = rem / p.kx;
+            const int rb = j % STEM_NRAW;
+            unsigned char* dst = raw + rb * S::RAW_BYTES;
+            tc::mbar_wait(rawempty + rb, ((j / STEM_NRAW) & 1) ^ 1);
+            tc::mbar_arrive_expect_tx(rawfull + rb, S::DY_BYTES + xbytes);
+            tc::tma_load_5d(dst, &tmap_dy, rawfull + rb, 0, x0, y0, n, co0 / 32);
+            tc::tma_load_4d(dst + S::DY_BYTES, &tmap_x, rawfull + rb, 0, x0, y0 - p.pad_y, n);
+        };
+        // the folded channels past creal are zero in every B tile: written once, never touched again
+        for (int i = tid; i < STEM_STAGES * STEM_KW * (64 - creal) * 8; i += 128) {
+            const int c = creal + (i >> 3) % (64 - creal), tile = (i >> 3) / (64 - creal);
+            *reinterpret_cast<float4*>(base + tile * S::TILE_BYTES + c * 128 + (i & 7) * 16) = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        for (int j = 0; j < STEM_NRAW - 1 && j < KI; ++j) issue(j);
+        const int ntask = fold_kh * 8 * STEM_KW * 8;
+        for (int it = 0; it < KI; ++it) {
+            if (it + STEM_NRAW - 1 < KI) issue(it + STEM_NRAW - 1);
+            const int rb = it % STEM_NRAW, st = it % STEM_STAGES;
+            tc::mbar_wait(rawfull + rb, (it / STEM_NRAW) & 1);
+            tc::mbar_wait(empty + st, ((it / STEM_STAGES) & 1) ^ 1);
+            const float* src = reinterpret_cast<const float*>(raw + rb * S::RAW_BYTES + S::DY_BYTES);    // [row][36 px][8 ch]
+            unsigned char* dst = base + st * S::STAGE_BYTES;
+            // task (r, q, s, ci), ci fastest: 16-byte chunk q (pixels 4q .. 4q + 3) of row c = 8r + ci of tap s's tile.  Eight
+            // lanes of a store phase write chunks q ^ ci of eight rows (conflict-free); the reads of a warp's four (s, q)
+            // groups start on pixels 4q + s, mostly different banks mod 4 pixels.
+            for (int i = tid; i < ntask; i += 128) {
+                const int ci = i & 7, u = i >> 3;
+                const int s = u % STEM_KW, q = (u / STEM_KW) & 7, r = u / (STEM_KW * 8);
+                const float* a = src + (r * S::WPX + 4 * q + s) * 8 + ci;
+                const int c = 8 * r + ci;
+                *reinterpret_cast<float4*>(dst + s * S::TILE_BYTES + c * 128 + ((q ^ ci) << 4)) = make_float4(a[0], a[8], a[16], a[24]);
+            }
+            tc::fence_proxy_async();
+            tc::mbar_arrive(full + st);
+            tc::named_sync(2, 128);                               // the raw X box is consumed before it is loaded again
+        }
+        return;
+    }
+    tc::setmaxnreg_inc<224>();
+
+    const int h = wg - 1, lane = tid & 31;
+    int aoff[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+        aoff[e] = dy_tile_offset(wgrad_row_co((tid >> 5) * 16 + (lane >> 2) + 8 * (e & 1)), (lane & 3) + 4 * (e >> 1));
+    float acc[STEM_KW][32];
+#pragma unroll
+    for (int t = 0; t < STEM_KW; ++t)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[t][i] = 0.f;
+    const uint32_t raw_s = tc::smem_u32(raw);
+    for (int it = h; it < KI; it += 2) {
+        const int st = it % STEM_STAGES, rb = it % STEM_NRAW;
+        tc::mbar_wait(rawfull + rb, (it / STEM_NRAW) & 1);
+        uint32_t frag[BK / MMA_K][4];
+#pragma unroll
+        for (int k = 0; k < BK / MMA_K; ++k)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) frag[k][e] = tc::lds_u32(raw_s + rb * S::RAW_BYTES + aoff[e] + k * 1024);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(rawempty + rb);
+        tc::mbar_wait(full + st, (it / STEM_STAGES) & 1);
+        const uint32_t b = tc::smem_u32(base + st * S::STAGE_BYTES);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int t = 0; t < STEM_KW; ++t)
+#pragma unroll
+            for (int k = 0; k < BK / MMA_K; ++k)
+                tc::Wgmma<64>::mma_rs(acc[t], frag[k], tc::desc_k128(b + t * S::TILE_BYTES + k * MMA_K * 4), 1u);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        if (tid == 0) tc::mbar_arrive(empty + st);
+    }
+    if (h >= KI) return;
+    const int m_a = (tid >> 5) * 16 + (lane >> 2);
+#pragma unroll
+    for (int t = 0; t < STEM_KW; ++t) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int co = co0 + wgrad_row_co(m_a + 8 * e);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int ci = 8 * j + 2 * (lane & 3);
+                if (ci >= creal) continue;                        // creal is even: ci + 1 < creal as well
+                const float v0 = acc[t][4 * j + 2 * e], v1 = acc[t][4 * j + 2 * e + 1];
+                if (p.tapmajor) {
+                    atomicAdd(reinterpret_cast<float2*>(dw + ((size_t)t * p.Cout + co) * p.Cin + ci), make_float2(v0, v1));
+                } else {
+                    atomicAdd(dw + ((size_t)co * p.Cin + ci) * STEM_KW + t, v0);
+                    atomicAdd(dw + ((size_t)co * p.Cin + ci + 1) * STEM_KW + t, v1);
+                }
+            }
+        }
+    }
+}
+
+// K splits of a weight-gradient grid of base_ctas CTAs per split (one CTA per SM): the count that minimises the modelled
+// time  waves(s) * (ceil(K / s) + FIXED)  — a CTA's time is its share of the K slices plus a fixed cost (pipeline
+// fill, the atomic epilogue), taken as 16 K slices; a partial last wave costs as much as a full one.  At least 8 K
+// slices per CTA; ties go to the smaller count (fewer atomics).
+int wgrad_splits(int base_ctas, long long ktotal) {
+    constexpr long long FIXED = 16;
+    const long long sms = tc::num_sms();
+    long long smax = ktotal / 8;
+    if (smax > 8 * sms) smax = 8 * sms;
+    int best = 1;
+    long long best_cost = -1;
+    for (long long s = 1; s <= smax; ++s) {
+        const long long cost = (base_ctas * s + sms - 1) / sms * ((ktotal + s - 1) / s + FIXED);
+        if (best_cost < 0 || cost < best_cost) { best = (int)s; best_cost = cost; }
+    }
+    return best;
+}
+
 template <int BN, int STAGES, int KW = 1>
 int launch_conv(const CUtensorMap& mx, const CUtensorMap& mw, const ConvParams& p, const float* bias, float* out, int tiles,
                 cudaStream_t st) {
@@ -604,11 +781,42 @@ int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, int N, int
     B3D_CHECK_ALIGNED(dy);
     B3D_CHECK_ALIGNED(x);
     b3d::clear_variant();
-    B3D_REQUIRE(fold_kh == 0, B3D_EINVAL,
-                "b3d_conv2d_wgrad_tf32: the on-the-fly fold is not available for the weight gradient: pass the materialised fold");
     if (tap_major) B3D_CHECK_ALIGNED(dw);
     WgradParams p{};
     p.N = N; p.Hout = Hout; p.Wout = Wout; p.Cout = Cout; p.Cin = Cin;
+    const uint64_t dpitch = dy_row_pitch > 0 ? dy_row_pitch : Wout;            // pixels per row of dy in memory
+    B3D_REQUIRE(dpitch >= (uint64_t)Wout, B3D_EINVAL, "b3d_conv2d_wgrad_tf32: dy_row_pitch=%d must be >= Wout=%d", dy_row_pitch, Wout);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (fold_kh > 0) {
+        // raw 8-channel stem input: 32-pixel row segments of the output are the K slices
+        B3D_REQUIRE(fold_kh > 4 && fold_kh <= 8 && Cin == 64 && kh == 1 && kw == STEM_KW && stride == 1 && x_off == 0 &&
+                        Cout % 64 == 0 && W == Wout + STEM_KW - 1 && Hout == H + 2 * pad_y - fold_kh + 1,
+                    B3D_EINVAL, "b3d_conv2d_wgrad_tf32: the raw-input stem weight gradient needs 4 < fold_kh <= 8 rows folded into "
+                    "64 channels, a 1x5 stride-1 filter, Cout %% 64 == 0 and the x padding in the input");
+        p.BWk = BK; p.BHk = 1;
+        p.kx = b3d::ceil_div(Wout, BK);
+        p.ky = Hout;
+        p.kh = 1; p.kw = kw; p.pad_y = pad_y; p.st = 1; p.tapmajor = tap_major ? 1 : 0;
+        p.splits = wgrad_splits(Cout / 64, (long long)N * p.kx * p.ky);
+        CUtensorMap mdy, mx;
+        {
+            const uint64_t dims[5] = {32, (uint64_t)Wout, (uint64_t)Hout, (uint64_t)N, (uint64_t)Cout / 32};
+            const uint64_t strides[4] = {(uint64_t)Cout * 4, dpitch * Cout * 4, (uint64_t)Hout * dpitch * Cout * 4, 128};
+            const uint32_t box[5] = {32, (uint32_t)BK, 1, 1, 2};
+            if (int rc = tc::make_tmap_f32(&mdy, dy, 5, dims, strides, box)) return rc;    // 128-byte swizzle: dy_tile_offset
+        }
+        {
+            const uint64_t dims[4] = {8, (uint64_t)W, (uint64_t)H, (uint64_t)N};          // the raw NHWC tensor
+            const uint64_t strides[3] = {32, (uint64_t)W * 32, (uint64_t)H * W * 32};
+            const uint32_t box[4] = {8, (uint32_t)StemSmem::WPX, (uint32_t)fold_kh, 1};
+            if (int rc = tc::make_tmap_f32(&mx, x, 4, dims, strides, box, nullptr, CU_TENSOR_MAP_SWIZZLE_NONE)) return rc;
+        }
+        B3D_CUDA_OK(cudaFuncSetAttribute(wgrad_stem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, StemSmem::TOTAL));
+        wgrad_stem_kernel<<<dim3(Cout / 64, p.splits), NTHREADS, StemSmem::TOTAL, st>>>(mdy, mx, p, fold_kh, dw);
+        B3D_LAUNCH_OK();
+        b3d::add_variant("wgrad_stem<%d,%d,%d>", STEM_KW, STEM_STAGES, STEM_NRAW);
+        return B3D_OK;
+    }
     p.BWk = pow2_floor(Wout < BK ? Wout : BK);
     p.BHk = BK / p.BWk;
     p.kx = b3d::ceil_div(Wout, p.BWk);
@@ -626,16 +834,12 @@ int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, int N, int
     }
     const int base_ctas = b3d::ceil_div(Cout, BM) * b3d::ceil_div(Cin, BN) * kh * (kw / T);
     const long long ktotal = (long long)N * p.kx * p.ky;
-    int splits = (2 * tc::num_sms() + base_ctas - 1) / base_ctas;    // ~2 waves of CTAs
-    if (splits > ktotal / 8) splits = (int)(ktotal / 8);           // at least 8 K slices per CTA
-    if (splits < 1) splits = 1;
+    const int splits = wgrad_splits(base_ctas, ktotal);
     p.splits = splits;
 
     CUtensorMap mdy, mx;
     {   // dims: (32 channels, W, H, N, channel block) — the block dim is outermost so that a box of BM/32 blocks is contiguous
         const uint64_t dims[5] = {32, (uint64_t)Wout, (uint64_t)Hout, (uint64_t)N, (uint64_t)Cout / 32};
-        const uint64_t dpitch = dy_row_pitch > 0 ? dy_row_pitch : Wout;            // pixels per row of dy in memory
-        B3D_REQUIRE(dpitch >= (uint64_t)Wout, B3D_EINVAL, "b3d_conv2d_wgrad_tf32: dy_row_pitch=%d must be >= Wout=%d", dy_row_pitch, Wout);
         const uint64_t strides[4] = {(uint64_t)Cout * 4, dpitch * Cout * 4, (uint64_t)Hout * dpitch * Cout * 4, 128};
         const uint32_t box[5] = {32, (uint32_t)p.BWk, (uint32_t)p.BHk, 1, (uint32_t)(BM / 32)};
         if (int rc = tc::make_tmap_f32(&mdy, dy, 5, dims, strides, box)) return rc;    // 128-byte swizzle: dy_tile_offset
@@ -648,7 +852,6 @@ int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, int N, int
         const uint32_t es[5] = {1, (uint32_t)stride, (uint32_t)stride, 1, 1};
         if (int rc = tc::make_tmap_f32(&mx, x, 5, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_NONE)) return rc;
     }
-    cudaStream_t st = (cudaStream_t)stream;
     dim3 grid(b3d::ceil_div(Cout, BM), b3d::ceil_div(Cin, BN), kh * (kw / T) * splits);
     if (T == 3) return launch_wgrad<64, 3, 3, 3>(mdy, mx, p, dw, grid, st);
     if (T == 2) return BN == 128 ? launch_wgrad<128, 2, 3, 2>(mdy, mx, p, dw, grid, st) : launch_wgrad<64, 3, 3, 2>(mdy, mx, p, dw, grid, st);

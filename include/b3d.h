@@ -285,7 +285,9 @@ B3D_API int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, in
  * buffer, read in place); 0 = dense [N,Hout,Wout,Cout].                                                                   */
 /* tap_major != 0: dw is the tap-major array [kh*kw][Cout][Cin] (the layout b3d_conv2d_tf32 reads, 16-byte vector
  * reductions) instead of [Cout][Cin][kh][kw].  fold_kh > 0: x is the raw 8-channel stem input, folded on the fly as in
- * b3d_conv2d_tf32 (kh = 1, kw = the horizontal taps, Cin = folded channel count, pad_y = the fold's y padding).              */
+ * b3d_conv2d_tf32 (kh = 1, kw = the horizontal taps, Cin = folded channel count, pad_y = the fold's y padding); supported
+ * for kw = 5, 5 <= fold_kh <= 8 (Cin = 64), stride 1, x_off = 0, Cout % 64 == 0 and W = Wout + 4.  Folded channels past
+ * 8 fold_kh receive nothing.                                                                                             */
 
 /* Thin heads: 5x5 / stride-1 convolutions with 1..4 output channels (generator conv_final, models/gan.py:359;
  * discriminator heads :177, :302) on the fp32 CUDA cores, channels across the lanes of a warp.  Cin % 64 == 0.

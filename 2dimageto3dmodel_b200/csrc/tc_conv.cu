@@ -14,9 +14,10 @@
 //     TMA zero fill, and strided (4x4 / stride 2) dgrad runs as 4 parity classes with a strided epilogue,
 //   * strided fprop (element strides in the tensor map).
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one thread issues), warpgroups 1-2 = wgmma on pixel rows 0-63 /
-// 64-127 of the tile and the epilogue straight from the accumulator registers (bias / LeakyReLU / BN statistics /
-// fused activation adjoint -> global).  Persistent: a CTA per SM walks the work items; the STAGES-deep mbarrier ring
-// keeps the producer loading the next item while the consumers run the epilogue of the current one.
+// 64-127 of the tile (BN = 64: on alternate work items, the whole tile each, weights as the M operand) and the epilogue
+// straight from the accumulator registers (bias / LeakyReLU / BN statistics / fused activation adjoint -> global).
+// Persistent: a CTA per SM walks the work items; the STAGES-deep mbarrier ring keeps the producer loading the next item
+// while the consumers run the epilogue of the current one.
 #include "tc_common.cuh"
 
 namespace {
@@ -64,25 +65,49 @@ struct CSmem {
     static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * BN * 4 /*BN statistics*/;
 };
 
-// The K loop of one work item for one consumer warpgroup: rows [64 h, 64 h + 64) of the 128 x BN accumulator.  A stage
-// is handed back to the producer once the wgmma group that read it has retired (one arrival per warpgroup).
+// BN == 64 swaps the operands: the 64 x 32 weight tile is the M operand and the whole 128-pixel tile the N operand of one
+// m64n128k8 per K step (6 KB of shared memory read per 65 536 MACs instead of 4 KB per 32 768), and each consumer
+// warpgroup owns whole work items (item k of the CTA goes to warpgroup k % 2), so one warpgroup's epilogue overlaps the
+// other's main loop.
+template <int BN>
+constexpr bool kSwap = BN == 64;
+template <int BN>
+constexpr int kAcc = kSwap<BN> ? BM / 2 : BN / 2;      // accumulator registers per consumer thread
+
+// The K loop of one work item for one consumer warpgroup: rows [64 h, 64 h + 64) of the 128 x BN accumulator, or with
+// kSwap the whole 64 x 128 (channel x pixel) transposed one.  With kSwap, `full` is the warpgroup's own row of full
+// barriers and `phase` holds the parity of its next wait on each of them: a warpgroup that skips the other's stages
+// cannot derive it from git, and on a shared barrier it could wait for a phase before the previous one completed.  A stage is handed back to the producer once the wgmma group that read it has retired (one arrival per warpgroup
+// that reads it).
 template <int BN, int STAGES, int KW, bool FOLD>
-__device__ __forceinline__ void mainloop(float (&acc)[BN / 2], unsigned char* base, uint64_t* full, uint64_t* empty, int KI,
-                                         uint32_t& git, int h, bool leader, const int* shift) {
+__device__ __forceinline__ void mainloop(float (&acc)[kAcc<BN>], unsigned char* base, uint64_t* full, uint64_t* empty, int KI,
+                                         uint32_t& git, uint32_t& phase, int h, bool leader, const int* shift) {
     constexpr int A_BYTES = CSmem<BN, STAGES, KW>::A_BYTES, STAGE = CSmem<BN, STAGES, KW>::STAGE_BYTES;
     for (int it = 0; it < KI; ++it, ++git) {
         const int s = git % STAGES;
-        tc::mbar_wait(full + s, (git / STAGES) & 1);
+        if constexpr (kSwap<BN>) {
+            tc::mbar_wait(full + s, (phase >> s) & 1);
+            phase ^= 1u << s;
+        } else {
+            tc::mbar_wait(full + s, (git / STAGES) & 1);
+        }
         const uint32_t a = tc::smem_u32(base + s * STAGE), b = a + A_BYTES;
         tc::wgmma_fence();
 #pragma unroll
         for (int t = 0; t < KW; ++t) {
-            const uint32_t at = a + h * (64 * 128) + (KW > 1 ? shift[t] * 128 : 0);
+            const uint32_t shifted = a + (KW > 1 ? shift[t] * 128 : 0);
 #pragma unroll
             for (int k = 0; k < BK / MMA_K; ++k) {
-                // on-the-fly fold: K step k = image row k of the 4-row box, a [128 px][32 B] tile of its own (32-byte swizzle)
-                const uint64_t da = FOLD ? tc::desc_k32(a + k * (BM * 32) + h * (64 * 32)) : tc::desc_k128(at + k * MMA_K * 4);
-                tc::Wgmma<BN>::mma(acc, da, tc::desc_k128(b + t * (BN * 128) + k * MMA_K * 4), (it | t | k) ? 1u : 0u);
+                const uint32_t acc_flag = (it | t | k) ? 1u : 0u;
+                if constexpr (kSwap<BN>) {
+                    // on-the-fly fold: K step k = image row k of the 4-row box, a [128 px][32 B] tile of its own (32-byte swizzle)
+                    const uint64_t dp = FOLD ? tc::desc_k32(a + k * (BM * 32)) : tc::desc_k128(shifted + k * MMA_K * 4);
+                    tc::Wgmma<BM>::mma(acc, tc::desc_k128(b + t * (BN * 128) + k * MMA_K * 4), dp, acc_flag);
+                } else {
+                    const uint64_t da = FOLD ? tc::desc_k32(a + k * (BM * 32) + h * (64 * 32))
+                                             : tc::desc_k128(shifted + h * (64 * 128) + k * MMA_K * 4);
+                    tc::Wgmma<BN>::mma(acc, da, tc::desc_k128(b + t * (BN * 128) + k * MMA_K * 4), acc_flag);
+                }
             }
         }
         tc::wgmma_commit();
@@ -98,18 +123,21 @@ __global__ void __launch_bounds__(NTHREADS, 1)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w, const ConvParams p,
                   const float* __restrict__ bias, float* __restrict__ out, int tiles, int work_items) {
     using S = CSmem<BN, STAGES, KW>;
+    constexpr bool SWAP = kSwap<BN>;
+    constexpr int OWNERS = SWAP ? 2 : 1;               // rows of full barriers: one per warpgroup that owns items
     extern __shared__ unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * S::STAGE_BYTES);
-    uint64_t* empty = full + STAGES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * S::STAGE_BYTES);     // [OWNERS][STAGES]
+    uint64_t* empty = full + OWNERS * STAGES;
+    static_assert((OWNERS + 1) * STAGES * 8 <= 256, "barriers do not fit their area");
     float* sm_stats = reinterpret_cast<float*>(base + STAGES * S::STAGE_BYTES + 256);
     for (int i = threadIdx.x; i < 2 * BN; i += blockDim.x) sm_stats[i] = 0.f;
     if (threadIdx.x == 0) {
         tc::tma_prefetch_desc(&tmap_x);
         tc::tma_prefetch_desc(&tmap_w);
         for (int s = 0; s < STAGES; ++s) {
-            tc::mbar_init(full + s, 1);
-            tc::mbar_init(empty + s, 2);
+            for (int o = 0; o < OWNERS; ++o) tc::mbar_init(full + o * STAGES + s, 1);
+            tc::mbar_init(empty + s, SWAP ? 1 : 2);
         }
         tc::fence_barrier_init();
     }
@@ -120,7 +148,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     if (wg == 0) {
         if (threadIdx.x == 0) {
             uint32_t git = 0;
-            for (int w = blockIdx.x; w < work_items; w += gridDim.x) {
+            for (int w = blockIdx.x, k = 0; w < work_items; w += gridDim.x, ++k) {
+                uint64_t* fb = full + (SWAP ? (k & 1) * STAGES : 0);     // the owner's full barriers
                 // classes are the fastest index: the CTAs that work on the same pixel tiles at the same time share them in L2
                 const int cls = w % p.ncls, wq = w / p.ncls, tb = cls * p.ntaps;
                 int t = wq % tiles;
@@ -133,14 +162,14 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                     tc::mbar_wait(empty + s, ((git / STAGES) & 1) ^ 1);
                     const int tap = it / p.kslices * KW, ks = it % p.kslices;        // KW > 1: first tap of the filter row
                     unsigned char* a = base + s * S::STAGE_BYTES;
-                    tc::mbar_arrive_expect_tx(full + s, S::TX_BYTES);
+                    tc::mbar_arrive_expect_tx(fb + s, S::TX_BYTES);
                     if (KW > 1)     // window of 128 + KW - 1 pixels of the row; one box with the row's KW weight tiles
-                        tc::tma_load_4d(a, &tmap_x, full + s, ks * BK, x0 + p.dx0, y0 + p.dy[tb + tap], n0);
+                        tc::tma_load_4d(a, &tmap_x, fb + s, ks * BK, x0 + p.dx0, y0 + p.dy[tb + tap], n0);
                     else if (p.fold)     // box {8 ch, BW px, 4 rows}: lands as [row][pixel][8 floats] = four 32-byte-swizzled K-step tiles
-                        tc::tma_load_4d(a, &tmap_x, full + s, 0, x0 + p.dx[tb + tap], y0 + p.fold_y0 + 4 * ks, n0);
+                        tc::tma_load_4d(a, &tmap_x, fb + s, 0, x0 + p.dx[tb + tap], y0 + p.fold_y0 + 4 * ks, n0);
                     else
-                        tc::tma_load_4d(a, &tmap_x, full + s, ks * BK, p.sx * x0 + p.dx[tb + tap], p.sy * y0 + p.dy[tb + tap], n0);
-                    tc::tma_load_3d(a + S::A_BYTES, &tmap_w, full + s, ks * BK, c0, p.wtap[tb + tap]);
+                        tc::tma_load_4d(a, &tmap_x, fb + s, ks * BK, p.sx * x0 + p.dx[tb + tap], p.sy * y0 + p.dy[tb + tap], n0);
+                    tc::tma_load_3d(a + S::A_BYTES, &tmap_w, fb + s, ks * BK, c0, p.wtap[tb + tap]);
                 }
             }
         }
@@ -148,6 +177,76 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     }
 
     const int h = wg - 1, tid = threadIdx.x & 127, lane = tid & 31;
+    float acc[kAcc<BN>];
+#pragma unroll
+    for (int i = 0; i < kAcc<BN>; ++i) acc[i] = 0.f;
+    uint32_t git = 0, phase = 0;
+
+    if constexpr (SWAP) {
+        // this thread holds D[co][px] for the channels c0 + cw, c0 + cw + 8 and the pixels 8 j + 2 (lane % 4) + {0, 1}
+        uint64_t* fb = full + h * STAGES;
+        const int cw = (tid >> 5) * 16 + (lane >> 2);
+        const int lbw = __ffs(p.BW) - 1, lbwh = lbw + __ffs(p.BH) - 1;      // BW, BH are powers of two
+        for (int k = h;; k += 2) {
+            const int w = blockIdx.x + k * gridDim.x;
+            if (w >= work_items) break;
+            git = (uint32_t)k * KI;                                            // skip the other warpgroup's items
+            const int cls = w % p.ncls, wq = w / p.ncls;
+            const int tile = wq % tiles, c0 = (wq / tiles) * BN;
+            if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, fb, empty, KI, git, phase, h, tid == 0, p.shift);
+            else mainloop<BN, STAGES, KW, false>(acc, base, fb, empty, KI, git, phase, h, tid == 0, p.shift);
+
+            const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, tn = tile / (p.tiles_x * p.tiles_y);
+            bool cok[2];
+            float bv[2], sum[2] = {0.f, 0.f}, sq[2] = {0.f, 0.f};
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                cok[e] = c0 + cw + 8 * e < p.Cout;
+                bv[e] = bias && cok[e] ? __ldg(bias + c0 + cw + 8 * e) : 0.f;
+            }
+#pragma unroll
+            for (int j = 0; j < BM / 8; ++j) {
+#pragma unroll
+                for (int e1 = 0; e1 < 2; ++e1) {
+                    const int px = 8 * j + 2 * (lane & 3) + e1;
+                    const int n = tn * p.BI + (px >> lbwh), y = ty * p.BH + ((px >> lbw) & (p.BH - 1)),
+                              x = p.xbase + tx * p.BW + (px & (p.BW - 1));
+                    const bool valid = n < p.N && y < p.Hout && x < p.Wout;
+                    const size_t off = valid ? (((size_t)n * p.OH + (size_t)(p.osy * y + p.cooy[cls])) * p.OW +
+                                                (size_t)(p.osx * x + p.coox[cls])) * p.OC + c0 + cw : 0;
+#pragma unroll
+                    for (int e2 = 0; e2 < 2; ++e2) {
+                        float t = acc[4 * j + 2 * e2 + e1];
+                        const bool ok = valid && cok[e2];
+                        if (p.mask && ok && !(__ldg(p.mask + off + 8 * e2) >= 0.f)) t *= p.mslope;   // as pad_leaky_bias_bwd_kernel
+                        const float v = valid ? t : 0.f;
+                        sum[e2] += v;
+                        sq[e2] += v * v;
+                        if (ok) {
+                            const float o = v + bv[e2];
+                            out[off + 8 * e2] = o >= 0.f ? o : o * p.leaky;
+                        }
+                    }
+                }
+            }
+            if (p.stats) {
+                // the four lanes of a quad hold the channel's 128 pixels; warp w alone holds channels 16 w .. 16 w + 15
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 1);
+                    sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 2);
+                    sq[e] += __shfl_xor_sync(0xffffffffu, sq[e], 1);
+                    sq[e] += __shfl_xor_sync(0xffffffffu, sq[e], 2);
+                    if ((lane & 3) == 0 && cok[e]) {
+                        atomicAdd(p.stats + c0 + cw + 8 * e, (double)sum[e]);
+                        if (!p.stats_sum) atomicAdd(p.stats + p.Cout + c0 + cw + 8 * e, (double)sq[e]);
+                    }
+                }
+            }
+        }
+        return;
+    }
+
     const int row_a = h * 64 + (tid >> 5) * 16 + (lane >> 2);          // this thread's two accumulator rows: row_a, row_a + 8
     int bx[2], by[2], bi[2];
 #pragma unroll
@@ -157,15 +256,11 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         by[e] = (r / p.BW) % p.BH;
         bi[e] = r / (p.BW * p.BH);
     }
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    uint32_t git = 0;
     for (int w = blockIdx.x; w < work_items; w += gridDim.x) {
         const int cls = w % p.ncls, wq = w / p.ncls;
         const int tile = wq % tiles, c0 = (wq / tiles) * BN;
-        if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, full, empty, KI, git, h, tid == 0, p.shift);
-        else mainloop<BN, STAGES, KW, false>(acc, base, full, empty, KI, git, h, tid == 0, p.shift);
+        if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, full, empty, KI, git, phase, h, tid == 0, p.shift);
+        else mainloop<BN, STAGES, KW, false>(acc, base, full, empty, KI, git, phase, h, tid == 0, p.shift);
 
         const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, tn = tile / (p.tiles_x * p.tiles_y);
         bool valid[2];

@@ -74,6 +74,23 @@ __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* m, ui
         : "memory");
 }
 
+// the 128-byte line that holds p is brought into L2 (no register, no wait): for data a later plain load will want
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+
+// Plain global loads.  The scheduler moves ld.global.nc (__ldg) freely and sinks each load of a batch next to its use;
+// these keep their place relative to the stores around them, which holds a batch of independent loads together ahead of
+// the code that consumes it.
+__device__ __forceinline__ float ld_global(const float* p) {
+    float v;
+    asm volatile("ld.global.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ float2 ld_global2(const float* p) {          // p 8-byte aligned
+    float2 v;
+    asm volatile("ld.global.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p) : "memory");
+    return v;
+}
+
 // ---------------------------------------------------------------------------------------------- wgmma
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

@@ -48,6 +48,7 @@ struct ConvParams {
     int stats_sum;                    // statistics: sums only (the bias gradient of the fused adjoint)
     int ncls;                         // >= 1 output classes in ONE launch (the stride-2 input gradient's parity classes): class c uses taps
     int cooy[4], coox[4];             //      [c * ntaps, (c + 1) * ntaps) of dy / dx / wtap and the output offset (cooy[c], coox[c])
+    uint32_t esn, esy, esx;           // element strides of the output between pixels of a tile one step apart along n / y / x
     int dx0, shift[5];                // row window (KW > 1): window starts at column x + dx0; tap t of a filter row reads it shift[t] rows in
 };
 
@@ -118,6 +119,176 @@ __device__ __forceinline__ void mainloop(float (&acc)[kAcc<BN>], unsigned char* 
     if (KI > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES);
 }
 
+// Where a work item's 128-pixel tile lies in the output tensor (and in the mask, which has the output's geometry): pixel
+// px = (bi, by, bx) of the BI x BH x BW box is output pixel (n0 + bi, y0 + by, x0 + bx) of the launch's logical extent, and
+// its channel 0 is element  base + bi esn + by esy + bx esx  (the part after base fits 32 bits: checked by the host).
+struct TileAt {
+    int n0, y0, x0;
+    size_t base;
+    int lbw, lbwh;                    // log2 BW, log2 (BW * BH): both are powers of two
+};
+__device__ __forceinline__ void tile_origin(const ConvParams& p, TileAt& t, int tile, int cls) {
+    t.x0 = p.xbase + (tile % p.tiles_x) * p.BW;
+    t.y0 = (tile / p.tiles_x) % p.tiles_y * p.BH;
+    t.n0 = tile / (p.tiles_x * p.tiles_y) * p.BI;
+    t.base = (((size_t)t.n0 * p.OH + (size_t)(p.osy * t.y0 + p.cooy[cls])) * p.OW + (size_t)(p.osx * t.x0 + p.coox[cls])) * p.OC;
+}
+// false when pixel px (0 .. 127) of the tile lies outside the launch's extent (`rel` is then not to be used)
+__device__ __forceinline__ bool tile_pixel(const ConvParams& p, const TileAt& t, int px, uint32_t& rel) {
+    const int bi = px >> t.lbwh, by = (px >> t.lbw) & (p.BH - 1), bx = px & (p.BW - 1);
+    rel = bi * p.esn + by * p.esy + bx * p.esx;
+    return t.n0 + bi < p.N && t.y0 + by < p.Hout && t.x0 + bx < p.Wout;
+}
+
+// The fused LeakyReLU adjoint reads the mask once per accumulator value, and the mask (the producer layer's activation) is
+// in DRAM.  The `nthr` threads that will run the item's epilogue request its mask tile (128 pixels x BN channels, BN / 32
+// lines of 128 bytes per pixel) into L2 before the item's main loop, so the fetch runs under the main loop.
+template <int BN>
+__device__ __forceinline__ void prefetch_mask_tile(const ConvParams& p, const TileAt& t, int c0, int et, int nthr) {
+    constexpr int LPP = BN / 32;
+    for (int i = et; i < BM * LPP; i += nthr) {
+        const int c = c0 + (i % LPP) * 32;
+        uint32_t rel;
+        if (tile_pixel(p, t, i / LPP, rel) && c < p.Cout) tc::prefetch_l2(p.mask + t.base + rel + c);
+    }
+}
+
+// Epilogue of a BN == 64 item: this thread holds D[co][px] for the channels c0 + cw, c0 + cw + 8 and the pixels
+// 8 j + 2 (lane % 4) + {0, 1}.  MASKED: the mask values of SWAP_MASK_BLOCKS 8-pixel blocks are loaded before the first of
+// them is used (32 loads in flight per thread instead of one), and the slope is applied with a select:
+// t * (m >= 0 ? 1 : slope)  is pad_leaky_bias_bwd_kernel's  !(m >= 0) -> slope  rule, NaN included.
+constexpr int SWAP_MASK_BLOCKS = 8;
+template <bool MASKED>
+__device__ __forceinline__ void epilogue_swapped(const float (&acc)[BM / 2], const ConvParams& p, const TileAt& t, const float* bias,
+                                                 float* out, int c0, int cw, int lane) {
+    bool cok[2];
+    float bv[2], sum[2] = {0.f, 0.f}, sq[2] = {0.f, 0.f};
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+        cok[e] = c0 + cw + 8 * e < p.Cout;
+        bv[e] = bias && cok[e] ? __ldg(bias + c0 + cw + 8 * e) : 0.f;
+    }
+    const float* mask0 = p.mask + t.base + c0 + cw;
+    float* out0 = out + t.base + c0 + cw;
+    // A zero the compiler cannot see through: the pixels' box coordinates and relative offsets do not depend on the item, and
+    // hoisted out of the item loop they cost more registers than the kernel has.
+    int q;
+    asm volatile("mov.u32 %0, 0;" : "=r"(q));
+    q += 2 * (lane & 3);
+#pragma unroll
+    for (int j0 = 0; j0 < BM / 8; j0 += SWAP_MASK_BLOCKS) {
+        uint32_t rel[2 * SWAP_MASK_BLOCKS];
+        bool valid[2 * SWAP_MASK_BLOCKS];
+        float m[MASKED ? 4 * SWAP_MASK_BLOCKS : 1];
+#pragma unroll
+        for (int i = 0; i < 2 * SWAP_MASK_BLOCKS; ++i) {                 // pixel 8 j + 2 (lane % 4) + e1 of block j = j0 + i / 2, e1 = i % 2
+            valid[i] = tile_pixel(p, t, 8 * (j0 + (i >> 1)) + q + (i & 1), rel[i]);
+            if constexpr (MASKED) {
+#pragma unroll
+                for (int e2 = 0; e2 < 2; ++e2) m[2 * i + e2] = valid[i] && cok[e2] ? tc::ld_global(mask0 + rel[i] + 8 * e2) : 0.f;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 2 * SWAP_MASK_BLOCKS; ++i) {
+#pragma unroll
+            for (int e2 = 0; e2 < 2; ++e2) {
+                float v = acc[4 * (j0 + (i >> 1)) + 2 * e2 + (i & 1)];
+                if constexpr (MASKED) v *= m[2 * i + e2] >= 0.f ? 1.f : p.mslope;
+                v = valid[i] ? v : 0.f;
+                sum[e2] += v;
+                sq[e2] += v * v;
+                if (valid[i] && cok[e2]) {
+                    const float o = v + bv[e2];
+                    out0[rel[i] + 8 * e2] = o >= 0.f ? o : o * p.leaky;
+                }
+            }
+        }
+    }
+    if (p.stats) {
+        // the four lanes of a quad hold the channel's 128 pixels; warp w alone holds channels 16 w .. 16 w + 15
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 1);
+            sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 2);
+            sq[e] += __shfl_xor_sync(0xffffffffu, sq[e], 1);
+            sq[e] += __shfl_xor_sync(0xffffffffu, sq[e], 2);
+            if ((lane & 3) == 0 && cok[e]) {
+                atomicAdd(p.stats + c0 + cw + 8 * e, (double)sum[e]);
+                if (!p.stats_sum) atomicAdd(p.stats + p.Cout + c0 + cw + 8 * e, (double)sq[e]);
+            }
+        }
+    }
+}
+
+// Epilogue of a BN >= 128 item: this thread holds two pixel rows (validity and offsets in valid[] / off[]) x the channel pairs
+// c0 + 2 (lane % 4) + 8 j + {0, 1}.  One 8-wide column block at a time, without writing the accumulators (they stay
+// wgmma-only registers).  MASKED: the mask values of MASK_BLOCKS column blocks are loaded, a channel pair per load where the
+// tensor allows it, before the first of them is used (as many blocks as fit in registers next to the accumulators).
+template <int BN, bool MASKED>
+__device__ __forceinline__ void epilogue_rows(const float (&acc)[BN / 2], const ConvParams& p, const bool (&valid)[2],
+                                              const size_t (&off)[2], const float* bias, float* out, float* sm_stats, int c0, int lane) {
+    const int cq = c0 + 2 * (lane & 3);                           // first channel of this thread's column pair in block j: cq + 8 j
+    const bool vec = (p.OC & 1) == 0;
+    constexpr int MASK_BLOCKS = BN == 256 ? 8 : 16;
+#pragma unroll
+    for (int j0 = 0; j0 < BN / 8; j0 += MASK_BLOCKS) {
+        float2 mk[MASKED ? MASK_BLOCKS : 1][2];                   // [column block][row a / b]
+        if constexpr (MASKED) {
+#pragma unroll
+            for (int jj = 0; jj < MASK_BLOCKS; ++jj) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int co = cq + 8 * (j0 + jj);
+                    const float* a = p.mask + off[e] + co;
+                    const bool ok0 = valid[e] && co < p.Cout, ok1 = valid[e] && co + 1 < p.Cout, pair = vec && ok1;
+                    const float2 m2 = pair ? tc::ld_global2(a) : make_float2(0.f, 0.f);
+                    const float m0 = ok0 && !pair ? tc::ld_global(a) : m2.x, m1 = ok1 && !pair ? tc::ld_global(a + 1) : m2.y;
+                    mk[jj][e] = make_float2(m0, m1);
+                }
+            }
+        }
+#pragma unroll
+        for (int jj = 0; jj < MASK_BLOCKS; ++jj) {
+            const int j = j0 + jj;
+            float v[2][2];                                            // [row a / b][column pair]
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int e = i >> 1;
+                float t = acc[4 * j + i];
+                if constexpr (MASKED) t *= ((i & 1) ? mk[jj][e].y : mk[jj][e].x) >= 0.f ? 1.f : p.mslope;
+                v[e][i & 1] = valid[e] ? t : 0.f;
+            }
+            if (p.stats) tc::stats_accumulate8(v[0], v[1], sm_stats, BN, 8 * j, p.stats_sum != 0);
+            const int co = cq + 8 * j;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                if (!valid[e]) continue;
+                float* dst = out + off[e];
+                float o0 = v[e][0], o1 = v[e][1];
+                if (vec && co + 1 < p.Cout) {
+                    if (bias) { o0 += __ldg(bias + co); o1 += __ldg(bias + co + 1); }
+                    o0 = o0 >= 0.f ? o0 : o0 * p.leaky;
+                    o1 = o1 >= 0.f ? o1 : o1 * p.leaky;
+                    *reinterpret_cast<float2*>(dst + co) = make_float2(o0, o1);
+                } else {
+                    if (co < p.Cout) {
+                        o0 += bias ? __ldg(bias + co) : 0.f;
+                        dst[co] = o0 >= 0.f ? o0 : o0 * p.leaky;
+                    }
+                    if (co + 1 < p.Cout) {
+                        o1 += bias ? __ldg(bias + co + 1) : 0.f;
+                        dst[co + 1] = o1 >= 0.f ? o1 : o1 * p.leaky;
+                    }
+                }
+            }
+        }
+    }
+}
+
+// registers move from the producer warpgroup (one thread issues TMA) to the consumers, whose masked epilogues hold a batch of
+// mask values next to the accumulators: 128 * (168 - 40) == 256 * (232 - 168)
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+
 template <int BN, int STAGES, int KW>
 __global__ void __launch_bounds__(NTHREADS, 1)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w, const ConvParams p,
@@ -146,6 +317,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     const int wg = threadIdx.x >> 7;
 
     if (wg == 0) {
+        tc::setmaxnreg_dec<PRODUCER_REGS>();
         if (threadIdx.x == 0) {
             uint32_t git = 0;
             for (int w = blockIdx.x, k = 0; w < work_items; w += gridDim.x, ++k) {
@@ -175,140 +347,53 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         }
         return;
     }
+    tc::setmaxnreg_inc<CONSUMER_REGS>();
 
     const int h = wg - 1, tid = threadIdx.x & 127, lane = tid & 31;
     float acc[kAcc<BN>];
 #pragma unroll
     for (int i = 0; i < kAcc<BN>; ++i) acc[i] = 0.f;
     uint32_t git = 0, phase = 0;
+    TileAt at;
+    at.lbw = __ffs(p.BW) - 1;
+    at.lbwh = at.lbw + __ffs(p.BH) - 1;
 
     if constexpr (SWAP) {
-        // this thread holds D[co][px] for the channels c0 + cw, c0 + cw + 8 and the pixels 8 j + 2 (lane % 4) + {0, 1}
         uint64_t* fb = full + h * STAGES;
         const int cw = (tid >> 5) * 16 + (lane >> 2);
-        const int lbw = __ffs(p.BW) - 1, lbwh = lbw + __ffs(p.BH) - 1;      // BW, BH are powers of two
         for (int k = h;; k += 2) {
             const int w = blockIdx.x + k * gridDim.x;
             if (w >= work_items) break;
             git = (uint32_t)k * KI;                                            // skip the other warpgroup's items
-            const int cls = w % p.ncls, wq = w / p.ncls;
-            const int tile = wq % tiles, c0 = (wq / tiles) * BN;
+            const int wq = w / p.ncls, tile = wq % tiles, c0 = (wq / tiles) * BN;
+            tile_origin(p, at, tile, w % p.ncls);
+            if (p.mask) prefetch_mask_tile<BN>(p, at, c0, tid, 128);
             if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, fb, empty, KI, git, phase, h, tid == 0, p.shift);
             else mainloop<BN, STAGES, KW, false>(acc, base, fb, empty, KI, git, phase, h, tid == 0, p.shift);
+            if (p.mask) epilogue_swapped<true>(acc, p, at, bias, out, c0, cw, lane);
+            else epilogue_swapped<false>(acc, p, at, bias, out, c0, cw, lane);
+        }
+    } else {
+        const int row_a = h * 64 + (tid >> 5) * 16 + (lane >> 2);          // this thread's two accumulator rows: row_a, row_a + 8
+        for (int w = blockIdx.x; w < work_items; w += gridDim.x) {
+            const int wq = w / p.ncls, tile = wq % tiles, c0 = (wq / tiles) * BN;
+            tile_origin(p, at, tile, w % p.ncls);
+            if (p.mask) prefetch_mask_tile<BN>(p, at, c0, threadIdx.x - 128, 256);
+            if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, full, empty, KI, git, phase, h, tid == 0, p.shift);
+            else mainloop<BN, STAGES, KW, false>(acc, base, full, empty, KI, git, phase, h, tid == 0, p.shift);
 
-            const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, tn = tile / (p.tiles_x * p.tiles_y);
-            bool cok[2];
-            float bv[2], sum[2] = {0.f, 0.f}, sq[2] = {0.f, 0.f};
-#pragma unroll
+            bool valid[2];
+            size_t off[2];
+    #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                cok[e] = c0 + cw + 8 * e < p.Cout;
-                bv[e] = bias && cok[e] ? __ldg(bias + c0 + cw + 8 * e) : 0.f;
+                uint32_t rel;
+                valid[e] = tile_pixel(p, at, row_a + 8 * e, rel);
+                off[e] = at.base + rel;
             }
-#pragma unroll
-            for (int j = 0; j < BM / 8; ++j) {
-#pragma unroll
-                for (int e1 = 0; e1 < 2; ++e1) {
-                    const int px = 8 * j + 2 * (lane & 3) + e1;
-                    const int n = tn * p.BI + (px >> lbwh), y = ty * p.BH + ((px >> lbw) & (p.BH - 1)),
-                              x = p.xbase + tx * p.BW + (px & (p.BW - 1));
-                    const bool valid = n < p.N && y < p.Hout && x < p.Wout;
-                    const size_t off = valid ? (((size_t)n * p.OH + (size_t)(p.osy * y + p.cooy[cls])) * p.OW +
-                                                (size_t)(p.osx * x + p.coox[cls])) * p.OC + c0 + cw : 0;
-#pragma unroll
-                    for (int e2 = 0; e2 < 2; ++e2) {
-                        float t = acc[4 * j + 2 * e2 + e1];
-                        const bool ok = valid && cok[e2];
-                        if (p.mask && ok && !(__ldg(p.mask + off + 8 * e2) >= 0.f)) t *= p.mslope;   // as pad_leaky_bias_bwd_kernel
-                        const float v = valid ? t : 0.f;
-                        sum[e2] += v;
-                        sq[e2] += v * v;
-                        if (ok) {
-                            const float o = v + bv[e2];
-                            out[off + 8 * e2] = o >= 0.f ? o : o * p.leaky;
-                        }
-                    }
-                }
-            }
-            if (p.stats) {
-                // the four lanes of a quad hold the channel's 128 pixels; warp w alone holds channels 16 w .. 16 w + 15
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 1);
-                    sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 2);
-                    sq[e] += __shfl_xor_sync(0xffffffffu, sq[e], 1);
-                    sq[e] += __shfl_xor_sync(0xffffffffu, sq[e], 2);
-                    if ((lane & 3) == 0 && cok[e]) {
-                        atomicAdd(p.stats + c0 + cw + 8 * e, (double)sum[e]);
-                        if (!p.stats_sum) atomicAdd(p.stats + p.Cout + c0 + cw + 8 * e, (double)sq[e]);
-                    }
-                }
-            }
+            if (p.mask) epilogue_rows<BN, true>(acc, p, valid, off, bias, out, sm_stats, c0, lane);
+            else epilogue_rows<BN, false>(acc, p, valid, off, bias, out, sm_stats, c0, lane);
+            if (p.stats) tc::stats_flush(sm_stats, BN, p.stats, p.Cout, c0, threadIdx.x - 128, 256);
         }
-        return;
-    }
-
-    const int row_a = h * 64 + (tid >> 5) * 16 + (lane >> 2);          // this thread's two accumulator rows: row_a, row_a + 8
-    int bx[2], by[2], bi[2];
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-        const int r = row_a + 8 * e;
-        bx[e] = r % p.BW;
-        by[e] = (r / p.BW) % p.BH;
-        bi[e] = r / (p.BW * p.BH);
-    }
-    for (int w = blockIdx.x; w < work_items; w += gridDim.x) {
-        const int cls = w % p.ncls, wq = w / p.ncls;
-        const int tile = wq % tiles, c0 = (wq / tiles) * BN;
-        if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, full, empty, KI, git, phase, h, tid == 0, p.shift);
-        else mainloop<BN, STAGES, KW, false>(acc, base, full, empty, KI, git, phase, h, tid == 0, p.shift);
-
-        const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, tn = tile / (p.tiles_x * p.tiles_y);
-        bool valid[2];
-        size_t off[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            const int n = tn * p.BI + bi[e], y = ty * p.BH + by[e], x = p.xbase + tx * p.BW + bx[e];
-            valid[e] = n < p.N && y < p.Hout && x < p.Wout;
-            off[e] = valid[e] ? (((size_t)n * p.OH + (size_t)(p.osy * y + p.cooy[cls])) * p.OW + (size_t)(p.osx * x + p.coox[cls])) * p.OC : 0;
-        }
-        // one 8-wide column block at a time, without writing the accumulators (they stay wgmma-only registers)
-        const int cq = c0 + 2 * (lane & 3);                           // first channel of this thread's column pair in block j: cq + 8 j
-        const bool vec = (p.OC & 1) == 0;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-            float v[2][2];                                            // [row a / b][column pair]
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int e = i >> 1, co = cq + 8 * j + (i & 1);
-                float t = acc[4 * j + i];
-                if (p.mask && valid[e] && co < p.Cout && !(__ldg(p.mask + off[e] + co) >= 0.f)) t *= p.mslope;   // as pad_leaky_bias_bwd_kernel
-                v[e][i & 1] = valid[e] ? t : 0.f;
-            }
-            if (p.stats) tc::stats_accumulate8(v[0], v[1], sm_stats, BN, 8 * j, p.stats_sum != 0);
-            const int co = cq + 8 * j;
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                if (!valid[e]) continue;
-                float* dst = out + off[e];
-                float o0 = v[e][0], o1 = v[e][1];
-                if (vec && co + 1 < p.Cout) {
-                    if (bias) { o0 += __ldg(bias + co); o1 += __ldg(bias + co + 1); }
-                    o0 = o0 >= 0.f ? o0 : o0 * p.leaky;
-                    o1 = o1 >= 0.f ? o1 : o1 * p.leaky;
-                    *reinterpret_cast<float2*>(dst + co) = make_float2(o0, o1);
-                } else {
-                    if (co < p.Cout) {
-                        o0 += bias ? __ldg(bias + co) : 0.f;
-                        dst[co] = o0 >= 0.f ? o0 : o0 * p.leaky;
-                    }
-                    if (co + 1 < p.Cout) {
-                        o1 += bias ? __ldg(bias + co + 1) : 0.f;
-                        dst[co + 1] = o1 >= 0.f ? o1 : o1 * p.leaky;
-                    }
-                }
-            }
-        }
-        if (p.stats) tc::stats_flush(sm_stats, BN, p.stats, p.Cout, c0, threadIdx.x - 128, 256);
     }
 }
 
@@ -817,6 +902,13 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
         p.stats = stats;
         p.mask = mask; p.mslope = mslope; p.stats_sum = stats_sum;
         p.fold = fold_kh; p.fold_y0 = -fold_pad;
+        {   // the epilogue addresses a tile's pixels relative to its first one in 32 bits
+            const unsigned long long esn = p.BI > 1 ? (unsigned long long)OH * OW * OC : 0, esy = p.BH > 1 ? (unsigned long long)osy * OW * OC : 0,
+                                     esx = (unsigned long long)osx * OC;
+            B3D_REQUIRE((p.BI - 1) * esn + (p.BH - 1) * esy + (p.BW - 1) * esx + OC < (1ull << 32), B3D_EINVAL,
+                        "b3d_conv2d_tf32: a %d x %d x %d pixel tile spans more than 2^32 elements of the output", p.BI, p.BH, p.BW);
+            p.esn = (uint32_t)esn; p.esy = (uint32_t)esy; p.esx = (uint32_t)esx;
+        }
         CUtensorMap mx;
         if (g_kw && wspan >= BM) {
             // row window: tiles are 128-pixel row segments (BW = 128, BH = BI = 1); one A box = 128 + kw - 1 pixels of a row,

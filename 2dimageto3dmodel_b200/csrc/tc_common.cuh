@@ -28,6 +28,10 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// `count` arrivals at once (one thread standing for several readers of a stage)
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar, uint32_t count) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     asm volatile(
         "{\n"
@@ -74,23 +78,6 @@ __device__ __forceinline__ void tma_load_5d(void* smem, const CUtensorMap* m, ui
         : "memory");
 }
 
-// the 128-byte line that holds p is brought into L2 (no register, no wait): for data a later plain load will want
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-
-// Plain global loads.  The scheduler moves ld.global.nc (__ldg) freely and sinks each load of a batch next to its use;
-// these keep their place relative to the stores around them, which holds a batch of independent loads together ahead of
-// the code that consumes it.
-__device__ __forceinline__ float ld_global(const float* p) {
-    float v;
-    asm volatile("ld.global.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ float2 ld_global2(const float* p) {          // p 8-byte aligned
-    float2 v;
-    asm volatile("ld.global.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p) : "memory");
-    return v;
-}
-
 // ---------------------------------------------------------------------------------------------- wgmma
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -99,6 +86,16 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 __device__ __forceinline__ uint32_t lds_u32(uint32_t smem_addr) {
     uint32_t v;
     asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(smem_addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ float lds_f32(uint32_t smem_addr) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(smem_addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ float2 lds_f32x2(uint32_t smem_addr) {       // 8-byte aligned
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(smem_addr) : "memory");
     return v;
 }
 // per-thread register budget of the executing warpgroup (warp-specialized kernels move registers from producer to consumers)

@@ -17,7 +17,9 @@
 // 64-127 of the tile (BN = 64: on alternate work items, the whole tile each, weights as the M operand) and the epilogue
 // straight from the accumulator registers (bias / LeakyReLU / BN statistics / fused activation adjoint -> global).
 // Persistent: a CTA per SM walks the work items; the STAGES-deep mbarrier ring keeps the producer loading the next item
-// while the consumers run the epilogue of the current one.
+// while the consumers run the epilogue of the current one.  The fused activation adjoint's mask travels through the same
+// ring: after an item's K steps the producer loads its mask tile as BN / 32 more stages (one 128-pixel x 32-channel TMA box
+// of the mask, which has the output's geometry, each), and the epilogue reads the mask from shared memory.
 #include "tc_common.cuh"
 
 namespace {
@@ -43,8 +45,8 @@ struct ConvParams {
     double* stats;                    // nullable: [2][Cout] fp64 sum / sum of squares of the (pre-bias) output, accumulated
     int fold;                         // > 0: the A operand is folded on the fly from a raw [N,H,W,8] tensor (thin stems): K slice ks
     int fold_y0;                      //      = image rows y + fold_y0 + 4 ks .. + 3 of the 8 channels (tensor map dims c, x, row, n)
-    const float* mask;                // nullable: tensor of the output's geometry; acc *= (mask >= 0 ? 1 : mslope) before statistics / bias
-    float mslope;                     //           (LeakyReLU adjoint fused into the input-gradient epilogue)
+    int mask;                         // 1: acc *= (mask >= 0 ? 1 : mslope) before statistics / bias, the mask (a tensor of the output's
+    float mslope;                     //    geometry) read through the third tensor map (LeakyReLU adjoint fused into the input gradient)
     int stats_sum;                    // statistics: sums only (the bias gradient of the fused adjoint)
     int ncls;                         // >= 1 output classes in ONE launch (the stride-2 input gradient's parity classes): class c uses taps
     int cooy[4], coox[4];             //      [c * ntaps, (c + 1) * ntaps) of dy / dx / wtap and the output offset (cooy[c], coox[c])
@@ -56,6 +58,8 @@ struct ConvParams {
 // 128 + KW - 1 input pixels of a filter row and the KW weight tiles of that row; the consumers feed tap t as the window
 // shifted by whole 128-byte rows (the 128-byte swizzle is a function of the absolute shared-memory address, so TMA's write
 // pattern and the shifted descriptor agree), i.e. the A operand is loaded once per filter row instead of once per tap.
+// A mask stage holds one 32-channel chunk of the item's mask tile in the A region, 128-byte swizzled: see mask_offset.
+constexpr int MASK_BYTES = BM * BK * 4;
 template <int BN, int STAGES, int KW>
 struct CSmem {
     static constexpr int WIN_BYTES = (BM + KW - 1) * BK * 4;                 // what the A box delivers
@@ -64,7 +68,12 @@ struct CSmem {
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int TX_BYTES = WIN_BYTES + B_BYTES;
     static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * BN * 4 /*BN statistics*/;
+    static_assert(A_BYTES >= MASK_BYTES, "a mask chunk does not fit the A region of a stage");
 };
+
+// Byte offset of mask element (pixel px of the tile, channel ch of the 32-channel chunk) in a mask stage: TMA writes the
+// box's 128-byte pixel rows with the 128-byte swizzle (16-byte chunk index XOR px % 8; stages are 1024-byte aligned).
+__device__ __forceinline__ uint32_t mask_offset(int px, int ch) { return px * 128 + ((((ch >> 2) ^ px) & 7) << 4) + (ch & 3) * 4; }
 
 // BN == 64 swaps the operands: the 64 x 32 weight tile is the M operand and the whole 128-pixel tile the N operand of one
 // m64n128k8 per K step (6 KB of shared memory read per 65 536 MACs instead of 4 KB per 32 768), and each consumer
@@ -74,12 +83,17 @@ template <int BN>
 constexpr bool kSwap = BN == 64;
 template <int BN>
 constexpr int kAcc = kSwap<BN> ? BM / 2 : BN / 2;      // accumulator registers per consumer thread
+// Arrivals that hand a stage back to the producer.  A mask stage is read with shared-memory loads, and each warp that read
+// it arrives once (all 8 consumer warps with BN >= 128; with kSwap the 2 warps of the owner whose 32 channels it holds).
+// An operand stage, read by wgmma, gets the same total from the leader of each warpgroup that read it.
+template <int BN>
+constexpr int kEmptyArrivals = kSwap<BN> ? 2 : 8;
 
 // The K loop of one work item for one consumer warpgroup: rows [64 h, 64 h + 64) of the 128 x BN accumulator, or with
 // kSwap the whole 64 x 128 (channel x pixel) transposed one.  With kSwap, `full` is the warpgroup's own row of full
 // barriers and `phase` holds the parity of its next wait on each of them: a warpgroup that skips the other's stages
-// cannot derive it from git, and on a shared barrier it could wait for a phase before the previous one completed.  A stage is handed back to the producer once the wgmma group that read it has retired (one arrival per warpgroup
-// that reads it).
+// cannot derive it from git, and on a shared barrier it could wait for a phase before the previous one completed.  A stage is handed back to the producer once the wgmma group that read it has retired (by the leader
+// of each warpgroup that reads it, see kEmptyArrivals).
 template <int BN, int STAGES, int KW, bool FOLD>
 __device__ __forceinline__ void mainloop(float (&acc)[kAcc<BN>], unsigned char* base, uint64_t* full, uint64_t* empty, int KI,
                                          uint32_t& git, uint32_t& phase, int h, bool leader, const int* shift) {
@@ -113,10 +127,10 @@ __device__ __forceinline__ void mainloop(float (&acc)[kAcc<BN>], unsigned char* 
         }
         tc::wgmma_commit();
         tc::wgmma_wait<1>();
-        if (it > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES);
+        if (it > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES, kEmptyArrivals<BN> / (kSwap<BN> ? 1 : 2));
     }
     tc::wgmma_wait<0>();
-    if (KI > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES);
+    if (KI > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES, kEmptyArrivals<BN> / (kSwap<BN> ? 1 : 2));
 }
 
 // Where a work item's 128-pixel tile lies in the output tensor (and in the mask, which has the output's geometry): pixel
@@ -140,27 +154,14 @@ __device__ __forceinline__ bool tile_pixel(const ConvParams& p, const TileAt& t,
     return t.n0 + bi < p.N && t.y0 + by < p.Hout && t.x0 + bx < p.Wout;
 }
 
-// The fused LeakyReLU adjoint reads the mask once per accumulator value, and the mask (the producer layer's activation) is
-// in DRAM.  The `nthr` threads that will run the item's epilogue request its mask tile (128 pixels x BN channels, BN / 32
-// lines of 128 bytes per pixel) into L2 before the item's main loop, so the fetch runs under the main loop.
-template <int BN>
-__device__ __forceinline__ void prefetch_mask_tile(const ConvParams& p, const TileAt& t, int c0, int et, int nthr) {
-    constexpr int LPP = BN / 32;
-    for (int i = et; i < BM * LPP; i += nthr) {
-        const int c = c0 + (i % LPP) * 32;
-        uint32_t rel;
-        if (tile_pixel(p, t, i / LPP, rel) && c < p.Cout) tc::prefetch_l2(p.mask + t.base + rel + c);
-    }
-}
-
 // Epilogue of a BN == 64 item: this thread holds D[co][px] for the channels c0 + cw, c0 + cw + 8 and the pixels
-// 8 j + 2 (lane % 4) + {0, 1}.  MASKED: the mask values of SWAP_MASK_BLOCKS 8-pixel blocks are loaded before the first of
-// them is used (32 loads in flight per thread instead of one), and the slope is applied with a select:
-// t * (m >= 0 ? 1 : slope)  is pad_leaky_bias_bwd_kernel's  !(m >= 0) -> slope  rule, NaN included.
-constexpr int SWAP_MASK_BLOCKS = 8;
+// 8 j + 2 (lane % 4) + {0, 1}.  MASKED: the warp's 16 channels lie in one 32-channel chunk, whose mask stage starts at
+// shared address `mstage`; the warp loads its 32 mask values per thread from it, hands the stage back (`mempty`) and
+// applies the slope with a select: t * (m >= 0 ? 1 : slope)  is pad_leaky_bias_bwd_kernel's  !(m >= 0) -> slope  rule,
+// NaN included.  Across the warp the loads of one (j, e1, e2) cover 8 chunk indices x 4 words: conflict-free.
 template <bool MASKED>
 __device__ __forceinline__ void epilogue_swapped(const float (&acc)[BM / 2], const ConvParams& p, const TileAt& t, const float* bias,
-                                                 float* out, int c0, int cw, int lane) {
+                                                 float* out, int c0, int cw, int lane, uint32_t mstage, uint64_t* mempty) {
     bool cok[2];
     float bv[2], sum[2] = {0.f, 0.f}, sq[2] = {0.f, 0.f};
 #pragma unroll
@@ -168,38 +169,38 @@ __device__ __forceinline__ void epilogue_swapped(const float (&acc)[BM / 2], con
         cok[e] = c0 + cw + 8 * e < p.Cout;
         bv[e] = bias && cok[e] ? __ldg(bias + c0 + cw + 8 * e) : 0.f;
     }
-    const float* mask0 = p.mask + t.base + c0 + cw;
     float* out0 = out + t.base + c0 + cw;
     // A zero the compiler cannot see through: the pixels' box coordinates and relative offsets do not depend on the item, and
     // hoisted out of the item loop they cost more registers than the kernel has.
     int q;
     asm volatile("mov.u32 %0, 0;" : "=r"(q));
     q += 2 * (lane & 3);
+    float m[MASKED ? BM / 2 : 1];                                         // [block j][e2][e1], as acc
+    if constexpr (MASKED) {
 #pragma unroll
-    for (int j0 = 0; j0 < BM / 8; j0 += SWAP_MASK_BLOCKS) {
-        uint32_t rel[2 * SWAP_MASK_BLOCKS];
-        bool valid[2 * SWAP_MASK_BLOCKS];
-        float m[MASKED ? 4 * SWAP_MASK_BLOCKS : 1];
+        for (int j = 0; j < BM / 8; ++j)
 #pragma unroll
-        for (int i = 0; i < 2 * SWAP_MASK_BLOCKS; ++i) {                 // pixel 8 j + 2 (lane % 4) + e1 of block j = j0 + i / 2, e1 = i % 2
-            valid[i] = tile_pixel(p, t, 8 * (j0 + (i >> 1)) + q + (i & 1), rel[i]);
-            if constexpr (MASKED) {
+            for (int i = 0; i < 4; ++i)                                   // pixel 8 j + q + e1 (px % 8 == q + e1), chunk channel (cw + 8 e2) % 32
+                m[4 * j + i] = tc::lds_f32(mstage + mask_offset(8 * j + q + (i & 1), (cw + 8 * (i >> 1)) & 31));
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(mempty);
+    }
 #pragma unroll
-                for (int e2 = 0; e2 < 2; ++e2) m[2 * i + e2] = valid[i] && cok[e2] ? tc::ld_global(mask0 + rel[i] + 8 * e2) : 0.f;
-            }
-        }
+    for (int j = 0; j < BM / 8; ++j) {
 #pragma unroll
-        for (int i = 0; i < 2 * SWAP_MASK_BLOCKS; ++i) {
+        for (int e1 = 0; e1 < 2; ++e1) {
+            uint32_t rel;
+            const bool valid = tile_pixel(p, t, 8 * j + q + e1, rel);
 #pragma unroll
             for (int e2 = 0; e2 < 2; ++e2) {
-                float v = acc[4 * (j0 + (i >> 1)) + 2 * e2 + (i & 1)];
-                if constexpr (MASKED) v *= m[2 * i + e2] >= 0.f ? 1.f : p.mslope;
-                v = valid[i] ? v : 0.f;
+                float v = acc[4 * j + 2 * e2 + e1];
+                if constexpr (MASKED) v *= m[4 * j + 2 * e2 + e1] >= 0.f ? 1.f : p.mslope;
+                v = valid ? v : 0.f;
                 sum[e2] += v;
                 sq[e2] += v * v;
-                if (valid[i] && cok[e2]) {
+                if (valid && cok[e2]) {
                     const float o = v + bv[e2];
-                    out0[rel[i] + 8 * e2] = o >= 0.f ? o : o * p.leaky;
+                    out0[rel + 8 * e2] = o >= 0.f ? o : o * p.leaky;
                 }
             }
         }
@@ -222,34 +223,32 @@ __device__ __forceinline__ void epilogue_swapped(const float (&acc)[BM / 2], con
 
 // Epilogue of a BN >= 128 item: this thread holds two pixel rows (validity and offsets in valid[] / off[]) x the channel pairs
 // c0 + 2 (lane % 4) + 8 j + {0, 1}.  One 8-wide column block at a time, without writing the accumulators (they stay
-// wgmma-only registers).  MASKED: the mask values of MASK_BLOCKS column blocks are loaded, a channel pair per load where the
-// tensor allows it, before the first of them is used (as many blocks as fit in registers next to the accumulators).
-template <int BN, bool MASKED>
+// wgmma-only registers).  MASKED: chunk m of the item's mask (channels c0 + 32 m ..) is in ring stage git + m; before column
+// block 4 m each thread waits for it, loads its 4 blocks x 2 rows as channel pairs and its warp hands the stage back.  A
+// stage is consumed in chunk order, so the BN / 32 chunks may outnumber the stages of the ring.  Across the warp one load
+// covers 8 pixel rows (px % 8 == lane / 4) x 2 chunk indices x 2 pairs: two wavefronts of 32 banks, the least 256 bytes take.
+template <int BN, int STAGES, int STAGE_BYTES, bool MASKED>
 __device__ __forceinline__ void epilogue_rows(const float (&acc)[BN / 2], const ConvParams& p, const bool (&valid)[2],
-                                              const size_t (&off)[2], const float* bias, float* out, float* sm_stats, int c0, int lane) {
+                                              const size_t (&off)[2], const float* bias, float* out, float* sm_stats, int c0, int lane,
+                                              int row_a, uint32_t ring, uint64_t* full, uint64_t* empty, uint32_t git) {
     const int cq = c0 + 2 * (lane & 3);                           // first channel of this thread's column pair in block j: cq + 8 j
     const bool vec = (p.OC & 1) == 0;
-    constexpr int MASK_BLOCKS = BN == 256 ? 8 : 16;
 #pragma unroll
-    for (int j0 = 0; j0 < BN / 8; j0 += MASK_BLOCKS) {
-        float2 mk[MASKED ? MASK_BLOCKS : 1][2];                   // [column block][row a / b]
+    for (int m = 0; m < BN / 32; ++m) {
+        float2 mk[MASKED ? 4 : 1][2];                             // [column block][row a / b]
         if constexpr (MASKED) {
+            const uint32_t g = git + m, s = g % STAGES;
+            tc::mbar_wait(full + s, (g / STAGES) & 1);
 #pragma unroll
-            for (int jj = 0; jj < MASK_BLOCKS; ++jj) {
+            for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int co = cq + 8 * (j0 + jj);
-                    const float* a = p.mask + off[e] + co;
-                    const bool ok0 = valid[e] && co < p.Cout, ok1 = valid[e] && co + 1 < p.Cout, pair = vec && ok1;
-                    const float2 m2 = pair ? tc::ld_global2(a) : make_float2(0.f, 0.f);
-                    const float m0 = ok0 && !pair ? tc::ld_global(a) : m2.x, m1 = ok1 && !pair ? tc::ld_global(a + 1) : m2.y;
-                    mk[jj][e] = make_float2(m0, m1);
-                }
-            }
+                for (int e = 0; e < 2; ++e) mk[jj][e] = tc::lds_f32x2(ring + s * STAGE_BYTES + mask_offset(row_a + 8 * e, 8 * jj + 2 * (lane & 3)));
+            __syncwarp();
+            if (lane == 0) tc::mbar_arrive(empty + s);
         }
 #pragma unroll
-        for (int jj = 0; jj < MASK_BLOCKS; ++jj) {
-            const int j = j0 + jj;
+        for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * m + jj;
             float v[2][2];                                            // [row a / b][column pair]
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
@@ -285,14 +284,18 @@ __device__ __forceinline__ void epilogue_rows(const float (&acc)[BN / 2], const 
     }
 }
 
-// registers move from the producer warpgroup (one thread issues TMA) to the consumers, whose masked epilogues hold a batch of
-// mask values next to the accumulators: 128 * (168 - 40) == 256 * (232 - 168)
+// registers move from the producer warpgroup (one thread issues TMA) to the consumers: at an even 168 per thread the 64- and
+// 256-wide instantiations spill (the 64-wide masked epilogue holds its 32 mask values next to the accumulators);
+// 128 * (168 - 40) == 256 * (232 - 168)
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
+// tmap_m: the mask (masked launches only), dims {OC, OW, OH, N}, box {32, osx (BW - 1) + 1, osy (BH - 1) + 1, BI} with
+// element strides {1, osx, osy, 1}: pixel px of the box lands as row px of the tile, zero-filled outside the tensor
 template <int BN, int STAGES, int KW>
 __global__ void __launch_bounds__(NTHREADS, 1)
-conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w, const ConvParams p,
-                  const float* __restrict__ bias, float* __restrict__ out, int tiles, int work_items) {
+conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
+                  const __grid_constant__ CUtensorMap tmap_m, const ConvParams p, const float* __restrict__ bias,
+                  float* __restrict__ out, int tiles, int work_items) {
     using S = CSmem<BN, STAGES, KW>;
     constexpr bool SWAP = kSwap<BN>;
     constexpr int OWNERS = SWAP ? 2 : 1;               // rows of full barriers: one per warpgroup that owns items
@@ -306,14 +309,16 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     if (threadIdx.x == 0) {
         tc::tma_prefetch_desc(&tmap_x);
         tc::tma_prefetch_desc(&tmap_w);
+        if (p.mask) tc::tma_prefetch_desc(&tmap_m);
         for (int s = 0; s < STAGES; ++s) {
             for (int o = 0; o < OWNERS; ++o) tc::mbar_init(full + o * STAGES + s, 1);
-            tc::mbar_init(empty + s, SWAP ? 1 : 2);
+            tc::mbar_init(empty + s, kEmptyArrivals<BN>);
         }
         tc::fence_barrier_init();
     }
     __syncthreads();
     const int KI = p.ntaps / KW * p.kslices;           // K steps: (taps or filter rows) x channel slices
+    const int MS = p.mask ? BN / 32 : 0;               // mask stages per item
     const int wg = threadIdx.x >> 7;
 
     if (wg == 0) {
@@ -343,6 +348,13 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                         tc::tma_load_4d(a, &tmap_x, fb + s, ks * BK, p.sx * x0 + p.dx[tb + tap], p.sy * y0 + p.dy[tb + tap], n0);
                     tc::tma_load_3d(a + S::A_BYTES, &tmap_w, fb + s, ks * BK, c0, p.wtap[tb + tap]);
                 }
+                const int mx = p.osx * x0 + p.coox[cls], my = p.osy * y0 + p.cooy[cls];
+                for (int m = 0; m < MS; ++m, ++git) {
+                    const int s = git % STAGES;
+                    tc::mbar_wait(empty + s, ((git / STAGES) & 1) ^ 1);
+                    tc::mbar_arrive_expect_tx(fb + s, MASK_BYTES);
+                    tc::tma_load_4d(base + s * S::STAGE_BYTES, &tmap_m, fb + s, c0 + 32 * m, mx, my, n0);
+                }
             }
         }
         return;
@@ -354,6 +366,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
 #pragma unroll
     for (int i = 0; i < kAcc<BN>; ++i) acc[i] = 0.f;
     uint32_t git = 0, phase = 0;
+    const uint32_t ring = tc::smem_u32(base);
     TileAt at;
     at.lbw = __ffs(p.BW) - 1;
     at.lbwh = at.lbw + __ffs(p.BH) - 1;
@@ -364,21 +377,33 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         for (int k = h;; k += 2) {
             const int w = blockIdx.x + k * gridDim.x;
             if (w >= work_items) break;
-            git = (uint32_t)k * KI;                                            // skip the other warpgroup's items
+            git = (uint32_t)k * (KI + MS);                                     // skip the other warpgroup's items
             const int wq = w / p.ncls, tile = wq % tiles, c0 = (wq / tiles) * BN;
             tile_origin(p, at, tile, w % p.ncls);
-            if (p.mask) prefetch_mask_tile<BN>(p, at, c0, tid, 128);
             if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, fb, empty, KI, git, phase, h, tid == 0, p.shift);
             else mainloop<BN, STAGES, KW, false>(acc, base, fb, empty, KI, git, phase, h, tid == 0, p.shift);
-            if (p.mask) epilogue_swapped<true>(acc, p, at, bias, out, c0, cw, lane);
-            else epilogue_swapped<false>(acc, p, at, bias, out, c0, cw, lane);
+            if (p.mask) {
+                // every warp waits for both mask stages, so that its phase bits stay those of the barriers; warp w reads
+                // chunk w / 2 (its channels 16 w .. 16 w + 15)
+                uint32_t mstage = 0;
+                uint64_t* mempty = empty;
+#pragma unroll
+                for (int m = 0; m < BN / 32; ++m, ++git) {
+                    const int s = git % STAGES;
+                    tc::mbar_wait(fb + s, (phase >> s) & 1);
+                    phase ^= 1u << s;
+                    if (m == (tid >> 6)) { mstage = ring + s * S::STAGE_BYTES; mempty = empty + s; }
+                }
+                epilogue_swapped<true>(acc, p, at, bias, out, c0, cw, lane, mstage, mempty);
+            } else {
+                epilogue_swapped<false>(acc, p, at, bias, out, c0, cw, lane, 0, nullptr);
+            }
         }
     } else {
         const int row_a = h * 64 + (tid >> 5) * 16 + (lane >> 2);          // this thread's two accumulator rows: row_a, row_a + 8
         for (int w = blockIdx.x; w < work_items; w += gridDim.x) {
             const int wq = w / p.ncls, tile = wq % tiles, c0 = (wq / tiles) * BN;
             tile_origin(p, at, tile, w % p.ncls);
-            if (p.mask) prefetch_mask_tile<BN>(p, at, c0, threadIdx.x - 128, 256);
             if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, full, empty, KI, git, phase, h, tid == 0, p.shift);
             else mainloop<BN, STAGES, KW, false>(acc, base, full, empty, KI, git, phase, h, tid == 0, p.shift);
 
@@ -390,8 +415,12 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                 valid[e] = tile_pixel(p, at, row_a + 8 * e, rel);
                 off[e] = at.base + rel;
             }
-            if (p.mask) epilogue_rows<BN, true>(acc, p, valid, off, bias, out, sm_stats, c0, lane);
-            else epilogue_rows<BN, false>(acc, p, valid, off, bias, out, sm_stats, c0, lane);
+            if (p.mask) {
+                epilogue_rows<BN, STAGES, S::STAGE_BYTES, true>(acc, p, valid, off, bias, out, sm_stats, c0, lane, row_a, ring, full, empty, git);
+                git += MS;
+            } else {
+                epilogue_rows<BN, STAGES, S::STAGE_BYTES, false>(acc, p, valid, off, bias, out, sm_stats, c0, lane, row_a, ring, full, empty, git);
+            }
             if (p.stats) tc::stats_flush(sm_stats, BN, p.stats, p.Cout, c0, threadIdx.x - 128, 256);
         }
     }
@@ -777,14 +806,14 @@ int wgrad_splits(int base_ctas, long long ktotal) {
 }
 
 template <int BN, int STAGES, int KW = 1>
-int launch_conv(const CUtensorMap& mx, const CUtensorMap& mw, const ConvParams& p, const float* bias, float* out, int tiles,
-                cudaStream_t st) {
+int launch_conv(const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mm, const ConvParams& p, const float* bias, float* out,
+                int tiles, cudaStream_t st) {
     using S = CSmem<BN, STAGES, KW>;
     static_assert(S::TOTAL <= 227 * 1024, "conv pipeline does not fit shared memory");
     B3D_CUDA_OK(cudaFuncSetAttribute(conv_wgmma_kernel<BN, STAGES, KW>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
     const int work = tiles * b3d::ceil_div(p.Cout, BN) * p.ncls;
     const int sms = tc::num_sms();
-    conv_wgmma_kernel<BN, STAGES, KW><<<work < sms ? work : sms, NTHREADS, S::TOTAL, st>>>(mx, mw, p, bias, out, tiles, work);
+    conv_wgmma_kernel<BN, STAGES, KW><<<work < sms ? work : sms, NTHREADS, S::TOTAL, st>>>(mx, mw, mm, p, bias, out, tiles, work);
     B3D_LAUNCH_OK();
     if (KW > 1) b3d::add_variant("conv_wgmma_rowwin<%d,%d,%d>", BN, KW, STAGES);
     else b3d::add_variant("conv_wgmma<%d,%d>", BN, STAGES);
@@ -793,11 +822,11 @@ int launch_conv(const CUtensorMap& mx, const CUtensorMap& mw, const ConvParams& 
 
 // row-window launch of a filter grid of rows of kw horizontally consecutive taps (stages: as many as fit ~200 KB)
 template <int BN>
-int launch_rowwin(int kw, const CUtensorMap& mx, const CUtensorMap& mw, const ConvParams& p, const float* bias, float* out, int tiles,
-                  cudaStream_t st) {
-    if (kw == 2) return launch_conv<BN, BN == 64 ? 5 : 4, 2>(mx, mw, p, bias, out, tiles, st);
-    if (kw == 3) return launch_conv<BN, BN == 64 ? 4 : 3, 3>(mx, mw, p, bias, out, tiles, st);
-    return launch_conv<BN, BN == 64 ? 3 : 2, 5>(mx, mw, p, bias, out, tiles, st);
+int launch_rowwin(int kw, const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mm, const ConvParams& p, const float* bias,
+                  float* out, int tiles, cudaStream_t st) {
+    if (kw == 2) return launch_conv<BN, BN == 64 ? 5 : 4, 2>(mx, mw, mm, p, bias, out, tiles, st);
+    if (kw == 3) return launch_conv<BN, BN == 64 ? 4 : 3, 3>(mx, mw, mm, p, bias, out, tiles, st);
+    return launch_conv<BN, BN == 64 ? 3 : 2, 5>(mx, mw, mm, p, bias, out, tiles, st);
 }
 
 int pow2_floor(int v) {
@@ -832,6 +861,9 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
 
     const float* mask = opts ? opts->mask : nullptr;
     const float mslope = opts ? opts->mask_slope : 1.f;
+    // the mask is read through a tensor map of the output's geometry: a 16-byte aligned base and 16-byte pixel strides
+    B3D_REQUIRE(!mask || (reinterpret_cast<uintptr_t>(mask) % 16 == 0 && OC % 4 == 0), B3D_EINVAL,
+                "b3d_conv2d_tf32: the mask needs a 16-byte aligned base and OC %% 4 == 0 (OC=%d)", OC);
     const int stats_sum = (opts && opts->stats_sum_only) ? 1 : 0;
     const int xpitch = (opts && opts->x_row_pitch) ? opts->x_row_pitch : W;
     // nclass > 1: the tap lists hold nclass groups of ntaps / nclass taps; class c writes at (class_ooy[c], class_oox[c])
@@ -900,7 +932,7 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
         p.OH = OH; p.OW = OW; p.OC = OC; p.osy = osy; p.osx = osx;
         p.leaky = leaky;
         p.stats = stats;
-        p.mask = mask; p.mslope = mslope; p.stats_sum = stats_sum;
+        p.mask = mask != nullptr; p.mslope = mslope; p.stats_sum = stats_sum;
         p.fold = fold_kh; p.fold_y0 = -fold_pad;
         {   // the epilogue addresses a tile's pixels relative to its first one in 32 bits
             const unsigned long long esn = p.BI > 1 ? (unsigned long long)OH * OW * OC : 0, esy = p.BH > 1 ? (unsigned long long)osy * OW * OC : 0,
@@ -908,6 +940,14 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
             B3D_REQUIRE((p.BI - 1) * esn + (p.BH - 1) * esy + (p.BW - 1) * esx + OC < (1ull << 32), B3D_EINVAL,
                         "b3d_conv2d_tf32: a %d x %d x %d pixel tile spans more than 2^32 elements of the output", p.BI, p.BH, p.BW);
             p.esn = (uint32_t)esn; p.esy = (uint32_t)esy; p.esx = (uint32_t)esx;
+        }
+        CUtensorMap mm{};                                      // the mask, with the output's geometry: one 32-channel chunk of a tile per box
+        if (mask) {
+            const uint64_t dims[4] = {(uint64_t)OC, (uint64_t)OW, (uint64_t)OH, (uint64_t)N};
+            const uint64_t strides[3] = {(uint64_t)OC * 4, (uint64_t)OW * OC * 4, (uint64_t)OH * OW * OC * 4};
+            const uint32_t box[4] = {(uint32_t)BK, (uint32_t)(osx * (p.BW - 1) + 1), (uint32_t)(osy * (p.BH - 1) + 1), (uint32_t)p.BI};
+            const uint32_t es[4] = {1, (uint32_t)osx, (uint32_t)osy, 1};
+            if (int rc = tc::make_tmap_f32(&mm, mask, 4, dims, strides, box, es)) return rc;
         }
         CUtensorMap mx;
         if (g_kw && wspan >= BM) {
@@ -925,7 +965,8 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
             const uint32_t wbox[3] = {(uint32_t)BK, (uint32_t)BN, (uint32_t)((g_kw - 1) * g_wstep + 1)};
             const uint32_t wes[3] = {1, 1, (uint32_t)g_wstep};
             if (int rc = tc::make_tmap_f32(&mwr, wt, 3, wdims, wstrides, wbox, wes)) return rc;
-            return BN == 128 ? launch_rowwin<128>(g_kw, mx, mwr, p, bias, out, tiles, st) : launch_rowwin<64>(g_kw, mx, mwr, p, bias, out, tiles, st);
+            return BN == 128 ? launch_rowwin<128>(g_kw, mx, mwr, mm, p, bias, out, tiles, st)
+                             : launch_rowwin<64>(g_kw, mx, mwr, mm, p, bias, out, tiles, st);
         }
         if (fold_kh > 0) {
             B3D_REQUIRE(p.BH == 1 && p.BI == 1, B3D_EINVAL, "b3d_conv2d_tf32: on-the-fly fold needs one-row tiles");
@@ -941,9 +982,9 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
             if (int rc = tc::make_tmap_f32(&mx, x, 4, dims, strides, box, es)) return rc;
         }
         // ring depth: as many stages as fit next to the statistics / barrier area (~192 KB of operands)
-        if (BN == 256) return launch_conv<256, 4>(mx, mw, p, bias, out, tiles, st);
-        if (BN == 128) return launch_conv<128, 6>(mx, mw, p, bias, out, tiles, st);
-        return launch_conv<64, 8>(mx, mw, p, bias, out, tiles, st);
+        if (BN == 256) return launch_conv<256, 4>(mx, mw, mm, p, bias, out, tiles, st);
+        if (BN == 128) return launch_conv<128, 6>(mx, mw, mm, p, bias, out, tiles, st);
+        return launch_conv<64, 8>(mx, mw, mm, p, bias, out, tiles, st);
     };
     const int bw_full = pow2_floor(Wout < BM ? Wout : BM);
     const int rem = Wout % bw_full;

@@ -1,7 +1,8 @@
 """Timing of the input-gradient launches of a cfg3 step that carry the fused LeakyReLU adjoint (b3d_conv_opts.mask: the
 discriminators' backward chain, b3d.conv.ActLink), each WITH and WITHOUT the mask on the same operands: the stride-2 4x4
 layers of the texture discriminator (d1.conv2 / conv3 / conv4: 64-, 128- and 256-wide tiles) and of the mesh discriminator
-(d2.conv2 / conv3), at batch 32 (generator step, no bias sums) and 64 (discriminator step, with them).
+(d2.conv2 / conv3), at batch 32 (generator step, no bias sums) and 64 (discriminator step, with them; at batch 64 the
+masked launch is also timed without the bias sums, which the unmasked launch does not compute).
 
     python tools/time_dgrad_mask.py [--ref-lib OTHER/libb3d.so] [--reps 7] [--n 20]
 
@@ -65,16 +66,19 @@ def main():
             mask = torch.randn(N, H, W, Cin, device=dev, generator=g)
             sums = torch.zeros(2 * Cin, device=dev, dtype=torch.float64) if N == 2 * B else None
 
-            def call(lib, m):
+            def call(lib, m, s=True):
                 def run():
                     C.lib = lib
                     try:
-                        return C._dgrad(gy, wd, (H, W), 4, 4, 1, 2, mask=mask if m else None, slope=0.2, sums=sums if m else None)
+                        return C._dgrad(gy, wd, (H, W), 4, 4, 1, 2, mask=mask if m else None, slope=0.2,
+                                        sums=sums if m and s else None)
                     finally:
                         C.lib = b3d.lib
                 return run
 
             fns = [(f"{'masked' if m else 'plain'}_{ln}", call(lib, m)) for m in (True, False) for ln, lib in libs]
+            if sums is not None:        # the mask without the bias sums: what the mask alone costs over the plain launch
+                fns.append(("masked_nosums_this", call(b3d.lib, True, False)))
             row = {"launch": f"{name}.dgrad", "N": N, "gflop": round(2.0 * N * Hout * Wout * Cin * Cout * 16 / 1e9, 1)}
             if a.ref_lib:
                 outs = [f() for k, f in fns if k.startswith("masked")]
@@ -85,6 +89,8 @@ def main():
                 row[f"ms_{k}"] = round(m, 4)
                 tot[k] = tot.get(k, 0.0) + m
             row["masked_over_plain_this"] = round(row["ms_masked_this"] / row["ms_plain_this"], 3)
+            if sums is not None:
+                row["masked_nosums_over_plain_this"] = round(row["ms_masked_nosums_this"] / row["ms_plain_this"], 3)
             print(json.dumps(row), flush=True)
             del gy, wd, mask, sums
     print(json.dumps({"total_ms": {k: round(v, 3) for k, v in tot.items()}}))

@@ -42,10 +42,14 @@ _sz = ctypes.c_size_t
 _ll = ctypes.c_longlong
 
 
+_signed = []          # every entry point _sig declared, in order (prof_enable wraps them)
+
+
 def _sig(name, *argtypes):
     fn = getattr(lib, name)
     fn.argtypes = list(argtypes)
     fn.restype = ctypes.c_int
+    _signed.append(name)
     return fn
 
 
@@ -88,17 +92,14 @@ _sig("b3d_vox_termination_bwd", _vp, _vp, _i, _i, _i, _vp, _vp)
 _sig("b3d_vox_splat_sorted", _vp, _vp, _i, _i, _i, _i, _vp, _vp)
 _sig("b3d_vox_clamp01", _vp, ctypes.c_longlong, _vp)
 _sig("b3d_vox_gather", _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp)
-_sig("b3d_cbn_act_fwd", _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _f, _i, _vp)
-_sig("b3d_cbn_act_bwd1", _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _i, _vp)
-_sig("b3d_cbn_act_bwd2", _vp, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i, _i, _i, _i, _vp)
+_sig("b3d_cbn_act_fwd", _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _i, _vp)
+_sig("b3d_cbn_act_bwd1", _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i,
+     _f, _i, _vp)
+_sig("b3d_cbn_act_bwd2", _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _f, _i, _i, _i, _i, _vp)
 _sig("b3d_bn_sums", _vp, _ll, _i, _vp, _vp)
 _sig("b3d_cbn_prepare", _vp, _i, _i, _i, _vp, ctypes.c_double, _f, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp)
 _sig("b3d_cbn_bwd_reduce", _vp, _vp, _i, _vp, _vp, _i, _i, _vp)
 _sig("b3d_bn_sums_per_sample", _vp, _i, _ll, _i, _vp, _vp)
-_sig("b3d_cbn_act_fwd_ex", _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _i, _vp)
-_sig("b3d_cbn_act_bwd1_ex", _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i,
-     _f, _i, _vp)
-_sig("b3d_cbn_act_bwd2_ex", _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _f, _i, _i, _i, _i, _vp)
 _sig("b3d_cbn_prepare_sync", _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, ctypes.c_double, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
      _vp, _i, _i, _vp)
 _sig("b3d_cbn_bwd_reduce_sync", _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp)
@@ -181,7 +182,7 @@ def prof_enable():
     if _prof_records is not None:
         return
     _prof_records = []
-    for name in [n for n in dir(lib) if n.startswith("b3d_")] + list(_TIMED):
+    for name in _signed + [n for n in dir(lib) if n.startswith("b3d_")]:
         fn = getattr(lib, name)
         if name in _prof_saved or not hasattr(fn, "argtypes") or name in ("b3d_last_error", "b3d_launch_count",
                                                                           "b3d_version", "b3d_last_variant"):
@@ -216,12 +217,3 @@ def prof_disable():
     _prof_saved.clear()
     _prof_records = None
     return out
-
-
-_TIMED = ("b3d_pc_project", "b3d_pc_silhouette_fwd_hosttaps", "b3d_pc_silhouette_bwd_hosttaps", "b3d_pc_project_bwd",
-          "b3d_pc_splat_grid", "b3d_mesh_face_setup", "b3d_mesh_render_fwd", "b3d_mesh_render_bwd", "b3d_face_normals_fwd", "b3d_face_normals_bwd", "b3d_flat_loss_fwd",
-          "b3d_flat_loss_bwd", "b3d_rgba_mse_iou_fwd", "b3d_rgba_mse_bwd", "b3d_rgba_l1_iou_fwd", "b3d_rgba_l1_bwd", "b3d_chamfer_nn", "b3d_chamfer_bwd", "b3d_conv2d_tf32", "b3d_conv2d_wgrad_tf32", "b3d_conv2d_thin_fwd", "b3d_conv2d_thin_wgrad", "b3d_pad_x_fwd", "b3d_pad_x_bwd", "b3d_stem_input_fwd", "b3d_stem_input_bwd",
-          "b3d_leaky_bwd", "b3d_wrap_x_inplace", "b3d_wrap_x_bwd_inplace", "b3d_pad_leaky_bias_bwd", "b3d_fold_rows_fwd", "b3d_fold_rows_bwd", "b3d_cbn_act_fwd", "b3d_cbn_act_bwd1", "b3d_cbn_act_bwd2", "b3d_bn_sums", "b3d_cbn_prepare", "b3d_cbn_bwd_reduce",
-          "b3d_bn_sums_per_sample", "b3d_cbn_act_fwd_ex", "b3d_cbn_act_bwd1_ex", "b3d_cbn_act_bwd2_ex",
-          "b3d_bank_forward", "b3d_bank_backward", "b3d_vertex_pipeline_fwd", "b3d_vertex_pipeline_bwd", "b3d_gather_fields", "b3d_image_batch",
-          "b3d_texel_visibility", "b3d_pseudogt_pack")

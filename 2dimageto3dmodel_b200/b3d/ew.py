@@ -264,8 +264,8 @@ class _CBNActPad(torch.autograd.Function):
         sk = dev(skip.detach(), "skip") if skip is not None else None
         pitch = sk.shape[2] if sk is not None else 0
         out = torch.empty(N, up * H, up * W + 2 * pad, C, device=y.device, dtype=torch.float32)
-        check(lib.b3d_cbn_act_fwd_ex(ptr(y), ptr(scale), ptr(shift), ptr(sk), pitch, skip_off, ptr(out), N, H, W, C, up, pad,
-                                     int(pad_mode), float(slope), int(post_leaky), st))
+        check(lib.b3d_cbn_act_fwd(ptr(y), ptr(scale), ptr(shift), ptr(sk), pitch, skip_off, ptr(out), N, H, W, C, up, pad,
+                                  int(pad_mode), float(slope), int(post_leaky), st))
         ctx.save_for_backward(y, gt, scale, shift, mean, invstd, sk if sk is not None else torch.empty(0))
         ctx.cb, ctx.key = cb, key
         ctx.cfg = (skip_off, up, pad, post_leaky, mode, sync, count, sk is not None, skip.shape if skip is not None else None,
@@ -293,14 +293,14 @@ class _CBNActPad(torch.autograd.Function):
         s1 = ctypes.c_void_p(sink.data_ptr() + 4 * boff)        # d beta  = sum ga
         s2 = ctypes.c_void_p(sink.data_ptr() + 4 * goff)        # d gamma = sum ga * xhat
         stat_pitch = C if mode >= 3 else 0                 # per-sample mean / inv_std rows (instance / no normalisation)
-        check(lib.b3d_cbn_act_bwd1_ex(ptr(gout), ptr(y), ptr(scale), ptr(shift), ptr(sk) if has_skip else None,
-                                      sk.shape[2] if has_skip else 0, skip_off, ptr(mean), ptr(invstd), stat_pitch, ptr(ga), ptr(gskip),
-                                      gpitch, skip_off, s1, s2, P, N, H, W, C, up, pad, pad_mode, slope, int(post_leaky), st))
+        check(lib.b3d_cbn_act_bwd1(ptr(gout), ptr(y), ptr(scale), ptr(shift), ptr(sk) if has_skip else None,
+                                   sk.shape[2] if has_skip else 0, skip_off, ptr(mean), ptr(invstd), stat_pitch, ptr(ga), ptr(gskip),
+                                   gpitch, skip_off, s1, s2, P, N, H, W, C, up, pad, pad_mode, slope, int(post_leaky), st))
         inv_m = 0.0
         if mode >= 3:
             # per-sample coupling terms inv_m * gamma_t * (S1, S2) read straight from the d(gamma, beta) rows
             inv_m = 1.0 / count if mode == 3 else 0.0
-            check(lib.b3d_cbn_act_bwd2_ex(ptr(ga), ptr(y), ptr(gt), ptr(mean), ptr(invstd), C, s1, s2, P, inv_m, N, H, W, C, st))
+            check(lib.b3d_cbn_act_bwd2(ptr(ga), ptr(y), ptr(gt), ptr(mean), ptr(invstd), C, s1, s2, P, inv_m, N, H, W, C, st))
         elif mode != 0:
             red = torch.empty(2 * C, device=y.device, dtype=torch.float32)
             peers = ctx.peers
@@ -320,8 +320,8 @@ class _CBNActPad(torch.autograd.Function):
         else:
             red = torch.zeros(2 * C, device=y.device, dtype=torch.float32)
         if mode < 3:
-            check(lib.b3d_cbn_act_bwd2(ptr(ga), ptr(y), ptr(gt), ptr(mean), ptr(invstd), ptr(red),
-                                       ctypes.c_void_p(red.data_ptr() + 4 * C), inv_m, N, H, W, C, st))
+            check(lib.b3d_cbn_act_bwd2(ptr(ga), ptr(y), ptr(gt), ptr(mean), ptr(invstd), 0, ptr(red),
+                                       ctypes.c_void_p(red.data_ptr() + 4 * C), 0, inv_m, N, H, W, C, st))
         ggb = None
         if want_gb:
             cb.done += 1

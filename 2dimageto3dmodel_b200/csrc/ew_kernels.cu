@@ -893,9 +893,9 @@ cbn_act_bwd2_kernel(float4* __restrict__ ga, const float4* __restrict__ y, const
 }  // namespace
 
 extern "C" {
-int b3d_cbn_act_fwd_ex(const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch, int skip_off,
-                       float* out, int N, int H, int W, int C, int up, int pad, int pad_mode, float slope, int post_leaky,
-                       void* stream) {
+int b3d_cbn_act_fwd(const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch, int skip_off,
+                    float* out, int N, int H, int W, int C, int up, int pad, int pad_mode, float slope, int post_leaky,
+                    void* stream) {
     B3D_REQUIRE(N >= 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0 && (up == 1 || up == 2) && pad >= 0, B3D_EINVAL,
                 "b3d_cbn_act_fwd: bad arguments");
     B3D_REQUIRE(pad_mode == 0 || (pad_mode == 1 && pad <= up * W), B3D_EINVAL, "b3d_cbn_act_fwd: pad mode %d with pad %d > %d columns",
@@ -924,18 +924,13 @@ int b3d_cbn_act_fwd_ex(const float* y, const float* scale, const float* shift, c
     return B3D_OK;
 }
 
-int b3d_cbn_act_fwd(const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch, int skip_off,
-                    float* out, int N, int H, int W, int C, int up, int pad, float slope, int post_leaky, void* stream) {
-    return b3d_cbn_act_fwd_ex(y, scale, shift, skip, skip_pitch, skip_off, out, N, H, W, C, up, pad, 0, slope, post_leaky, stream);
-}
-
 // S1, S2 [N,C] are zeroed by the call; gskip (nullable) is written at pixel offset gskip_off with row pitch gskip_pitch
 // (its pad columns are NOT touched: the caller zeroes the buffer when gskip_pitch != W).  stat_pitch: row pitch of mean /
 // inv_std, 0 = one row for all samples (batch statistics), C = per-sample rows (instance / no normalisation).
-int b3d_cbn_act_bwd1_ex(const float* gout, const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch,
-                        int skip_off, const float* mean, const float* invstd, int stat_pitch, float* ga, float* gskip, int gskip_pitch,
-                        int gskip_off, float* S1, float* S2, int s_pitch, int N, int H, int W, int C, int up, int pad, int pad_mode,
-                        float slope, int post_leaky, void* stream) {
+int b3d_cbn_act_bwd1(const float* gout, const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch,
+                     int skip_off, const float* mean, const float* invstd, int stat_pitch, float* ga, float* gskip, int gskip_pitch,
+                     int gskip_off, float* S1, float* S2, int s_pitch, int N, int H, int W, int C, int up, int pad, int pad_mode,
+                     float slope, int post_leaky, void* stream) {
     B3D_REQUIRE(N >= 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0 && C / 4 <= NT && NT % (C / 4) == 0 && (up == 1 || up == 2), B3D_EINVAL,
                 "b3d_cbn_act_bwd1: bad arguments (C/4 must divide %d)", NT);
     B3D_REQUIRE(stat_pitch == 0 || stat_pitch == C, B3D_EINVAL, "b3d_cbn_act_bwd1: statistics pitch %d must be 0 or C=%d", stat_pitch, C);
@@ -961,18 +956,10 @@ int b3d_cbn_act_bwd1_ex(const float* gout, const float* y, const float* scale, c
     return B3D_OK;
 }
 
-int b3d_cbn_act_bwd1(const float* gout, const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch,
-                     int skip_off, const float* mean, const float* invstd, float* ga, float* gskip, int gskip_pitch, int gskip_off,
-                     float* S1, float* S2, int s_pitch, int N, int H, int W, int C, int up, int pad, float slope, int post_leaky,
-                     void* stream) {
-    return b3d_cbn_act_bwd1_ex(gout, y, scale, shift, skip, skip_pitch, skip_off, mean, invstd, 0, ga, gskip, gskip_pitch, gskip_off,
-                               S1, S2, s_pitch, N, H, W, C, up, pad, 0, slope, post_leaky, stream);
-}
-
 // stat_pitch 0: mean / inv_std / m1 / m2 are [C] (batch statistics; m1, m2 = b3d_cbn_bwd_reduce's rows).  stat_pitch C:
 // mean / inv_std are [N, C] and m1, m2 are bwd1's per-sample sums S1, S2 at row pitch m_pitch (a multiple of 4).
-int b3d_cbn_act_bwd2_ex(float* ga, const float* y, const float* gamma_t, const float* mean, const float* invstd, int stat_pitch,
-                        const float* m1, const float* m2, int m_pitch, float inv_m, int N, int H, int W, int C, void* stream) {
+int b3d_cbn_act_bwd2(float* ga, const float* y, const float* gamma_t, const float* mean, const float* invstd, int stat_pitch,
+                     const float* m1, const float* m2, int m_pitch, float inv_m, int N, int H, int W, int C, void* stream) {
     B3D_REQUIRE(N >= 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, B3D_EINVAL, "b3d_cbn_act_bwd2: bad arguments");
     B3D_REQUIRE(stat_pitch == 0 || (stat_pitch == C && m_pitch >= C && m_pitch % 4 == 0), B3D_EINVAL,
                 "b3d_cbn_act_bwd2: statistics pitch %d must be 0 or C=%d (sums pitch %d >= C, a multiple of 4)", stat_pitch, C, m_pitch);
@@ -985,11 +972,6 @@ int b3d_cbn_act_bwd2_ex(float* ga, const float* y, const float* gamma_t, const f
                                                              inv_m, per_n, C / 4, total);
     B3D_LAUNCH_OK();
     return B3D_OK;
-}
-
-int b3d_cbn_act_bwd2(float* ga, const float* y, const float* gamma_t, const float* mean, const float* invstd, const float* m1,
-                     const float* m2, float inv_m, int N, int H, int W, int C, void* stream) {
-    return b3d_cbn_act_bwd2_ex(ga, y, gamma_t, mean, invstd, 0, m1, m2, 0, inv_m, N, H, W, C, stream);
 }
 
 // fp64 per-channel sums [2][C] (sum, sum of squares) of y [rows, C], for callers that all-reduce the sums across ranks

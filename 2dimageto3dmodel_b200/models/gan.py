@@ -350,7 +350,7 @@ class ResBlockUp(nn.Module):
         s1 = s2 = None
         if W is not None:
             # the conv epilogues accumulate the batch-norm statistics of their output (no separate pass over y)
-            if cb is not None and not getattr(self, 'disable_epilogue_stats', False):
+            if cb is not None:
                 s1, s2 = cb.stats_slot(self.norm1), cb.stats_slot(self.norm2)
             c1 = lambda t: conv2d_banked(t, W[prefix + ".conv1"], pad_y=1, stats=s1)
             c2 = lambda t: conv2d_banked(t, W[prefix + ".conv2"], pad_y=1, stats=s2)

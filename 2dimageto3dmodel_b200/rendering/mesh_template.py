@@ -148,7 +148,7 @@ class MeshTemplate:
     def compute_normals(self, vertex_positions):
         """Unit face normals of the deformed mesh (reference :113-123)."""
         f = self.mesh.faces
-        if vertex_positions.is_cuda and vertex_positions.dtype == torch.float32 and not getattr(self, 'disable_fused_normals', False):
+        if vertex_positions.is_cuda and vertex_positions.dtype == torch.float32:
             from b3d.mesh import face_normals                   # one launch each way (csrc/loss_kernels.cu)
             return face_normals(vertex_positions, f)
         a, b, c = vertex_positions[:, f[:, 0]], vertex_positions[:, f[:, 1]], vertex_positions[:, f[:, 2]]

@@ -380,22 +380,29 @@ B3D_API int b3d_leaky_bwd(const float* gy, const float* y, float* out, long long
  *   out[n, yo, xo, :] = post( leaky(y[n,ys,xs,:] * scale[n,:] + shift[n,:]) + skip[n,ys,xs,:] ),
  *   (ys, xs) = (yo / up, clamp(xo - pad, 0, up*W-1) / up);  out [N, up*H, up*W + 2*pad, C];  scale = inv_std*(1+gamma),
  *   shift = beta - mean*scale ([N,C]); skip (nullable) is read at row pitch skip_pitch, pixel offset skip_off.
+ *   pad_mode 0 = replicate (the clamp above), 1 = circular for the asymmetric generator and the discriminators (pad <= up*W;
+ *   the column wraps in upsampled coordinates, bwd1 folds every pad column back onto the column it copies).
  * bwd1: gout -> ga = d/d(pre-activation) [N,H,W,C], gskip (nullable), S1[n,c] = sum ga, S2[n,c] = sum ga*xhat: rows of
- *       pitch s_pitch floats (>= C; slices of the batched d(gamma, beta) buffer), zeroed by the call
- * bwd2 (in place on ga): dy = inv_std * (ga * gamma_t - m1 - xhat * m2), (m1, m2) [C] = inv_m * (sums of d xhat, d xhat * xhat)
+ *       pitch s_pitch floats (>= C; slices of the batched d(gamma, beta) buffer), zeroed by the call.  stat_pitch: row
+ *       pitch of mean / inv_std, 0 = per channel (batch statistics), C = per sample (instance / no normalisation).
+ * bwd2 (in place on ga): dy = inv_std * (ga * gamma_t - inv_m * m1 - xhat * inv_m * m2).  stat_pitch 0: m1, m2 [C] are
+ *       b3d_cbn_bwd_reduce's rows (batch sums of d xhat, d xhat * xhat; inv_m = 1/count; m_pitch unused).  stat_pitch C:
+ *       m1, m2 are bwd1's S1, S2 rows at pitch m_pitch (>= C, a multiple of 4), multiplied by gamma_t per sample
+ *       (inv_m = 1/HW; 0 for no normalisation).
  * b3d_cbn_prepare / b3d_cbn_bwd_reduce / b3d_bn_sums: the per-layer scalar math around these passes, one launch each
  *       (statistics -> mean / inv_std / running buffers / scale / shift; coupling-term reduction; fp64 channel sums).
  *       momentum < 0 updates the running buffers as a cumulative average (torch's momentum=None): factor
  *       1 / (num_batches_tracked + 1), read on the device before the counter is incremented.                               */
 B3D_API int b3d_cbn_act_fwd(const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch,
-                            int skip_off, float* out, int N, int H, int W, int C, int up, int pad, float slope,
+                            int skip_off, float* out, int N, int H, int W, int C, int up, int pad, int pad_mode, float slope,
                             int post_leaky, void* stream);
 B3D_API int b3d_cbn_act_bwd1(const float* gout, const float* y, const float* scale, const float* shift, const float* skip,
-                             int skip_pitch, int skip_off, const float* mean, const float* invstd, float* ga, float* gskip,
-                             int gskip_pitch, int gskip_off, float* S1, float* S2, int s_pitch, int N, int H, int W, int C,
-                             int up, int pad, float slope, int post_leaky, void* stream);
+                             int skip_pitch, int skip_off, const float* mean, const float* invstd, int stat_pitch, float* ga,
+                             float* gskip, int gskip_pitch, int gskip_off, float* S1, float* S2, int s_pitch, int N, int H,
+                             int W, int C, int up, int pad, int pad_mode, float slope, int post_leaky, void* stream);
 B3D_API int b3d_cbn_act_bwd2(float* ga, const float* y, const float* gamma_t, const float* mean, const float* invstd,
-                             const float* m1, const float* m2, float inv_m, int N, int H, int W, int C, void* stream);
+                             int stat_pitch, const float* m1, const float* m2, int m_pitch, float inv_m, int N, int H, int W,
+                             int C, void* stream);
 B3D_API int b3d_bn_sums(const float* y, long long rows, int C, double* sums, void* stream);
 B3D_API int b3d_cbn_prepare(const float* gb, int gb_pitch, int gamma_off, int beta_off, const double* sums, double count,
                             float eps, float momentum, int mode, float* running_mean, float* running_var,
@@ -403,26 +410,12 @@ B3D_API int b3d_cbn_prepare(const float* gb, int gb_pitch, int gamma_off, int be
                             int N, int C, void* stream);
 B3D_API int b3d_cbn_bwd_reduce(const float* S1, const float* S2, int s_pitch, const float* gt, float* red, int N, int C,
                                void* stream);
-/* The same passes for instance normalisation and no normalisation (models/gan.py ConditionalBatchNorm2d norm_g 'instance' /
- * 'none', the discriminators' norm_d 'instance') and for circular x-padding (the asymmetric generator, the discriminators):
+/* Statistics for instance normalisation and no normalisation (models/gan.py ConditionalBatchNorm2d norm_g 'instance' /
+ * 'none', the discriminators' norm_d 'instance'), consumed by the same passes with stat_pitch C:
  * b3d_bn_sums_per_sample: fp64 [N][2][C] (sum, sum of squares per sample) of y [N, HW, C]; zeroed by the call.
  * b3d_cbn_prepare mode 3 turns them into instance statistics (count = HW, biased variance, 1/sqrt(var + eps), also in eval
- *   mode), mode 4 writes mean 0 / inv_std 1; both write mean / inv_std as [N, C] rows and no running buffers.
- * _ex: pad_mode 0 = replicate (the plain entry points), 1 = circular (pad <= up*W; the column wraps in upsampled
- *   coordinates, bwd1 folds every pad column back onto the column it copies).  stat_pitch: row pitch of mean / inv_std,
- *   0 = per channel (the plain entry points), C = per sample.  bwd2 with stat_pitch C reads m1, m2 as bwd1's S1, S2 rows
- *   (pitch m_pitch) and uses the per-sample coupling terms inv_m * gamma_t * S (inv_m = 1/HW; 0 for no normalisation). */
+ *   mode), mode 4 writes mean 0 / inv_std 1; both write mean / inv_std as [N, C] rows and no running buffers. */
 B3D_API int b3d_bn_sums_per_sample(const float* y, int N, long long HW, int C, double* sums, void* stream);
-B3D_API int b3d_cbn_act_fwd_ex(const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch,
-                               int skip_off, float* out, int N, int H, int W, int C, int up, int pad, int pad_mode, float slope,
-                               int post_leaky, void* stream);
-B3D_API int b3d_cbn_act_bwd1_ex(const float* gout, const float* y, const float* scale, const float* shift, const float* skip,
-                                int skip_pitch, int skip_off, const float* mean, const float* invstd, int stat_pitch, float* ga,
-                                float* gskip, int gskip_pitch, int gskip_off, float* S1, float* S2, int s_pitch, int N, int H,
-                                int W, int C, int up, int pad, int pad_mode, float slope, int post_leaky, void* stream);
-B3D_API int b3d_cbn_act_bwd2_ex(float* ga, const float* y, const float* gamma_t, const float* mean, const float* invstd,
-                                int stat_pitch, const float* m1, const float* m2, int m_pitch, float inv_m, int N, int H, int W,
-                                int C, void* stream);
 /* SyncBN (sync_batchnorm/batchnorm.py:68-150: statistics over all replicas) with the collective FUSED into the consuming
  * kernel: a one-shot all-reduce over NVLink / NVSwitch peer memory (csrc/ew_kernels.cu peer_allreduce) instead of a
  * separate NCCL all-reduce per layer.  peer_data / peer_flag: host arrays of `world` device pointers (rank order) into every

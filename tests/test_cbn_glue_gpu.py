@@ -425,9 +425,11 @@ def test_cbn_bwd_reduce_uses_per_sample_gamma():
 
 @pytest.mark.parametrize("C", [12, 1040])
 @pytest.mark.parametrize("up,pad,post", [(2, 1, False), (1, 2, True)])
-def test_cbn_act_fwd_generic_kernel(C, up, pad, post):
+@pytest.mark.parametrize("pad_mode", [0, 1])
+def test_cbn_act_fwd_generic_kernel_pad_modes(pad_mode, C, up, pad, post):
     """b3d_cbn_act_fwd where C/4 does not divide 256 (the generic grid-stride kernel, include/b3d.h allows any C % 4 == 0):
-    out = post(leaky(y * scale + shift) + skip[x + skip_off]) upsampled and replicate-padded, skip with a row pitch W + 3."""
+    out = post(leaky(y * scale + shift) + skip[x + skip_off]) upsampled and x-padded (pad_mode 0 replicate, 1 circular in
+    upsampled columns), skip with a row pitch W + 3."""
     from b3d import lib, ptr, stream_ptr
     N, H, W, off, slope = 3, 5, 7, 2, 0.2
     g = torch.Generator().manual_seed(C + up)
@@ -436,8 +438,8 @@ def test_cbn_act_fwd_generic_kernel(C, up, pad, post):
     shift = (0.3 * torch.randn(N, C, generator=g)).to(DEV)
     skip = torch.randn(N, H, W + 3, C, generator=g).to(DEV)
     out = torch.empty(N, up * H, up * W + 2 * pad, C, device=DEV)
-    assert lib.b3d_cbn_act_fwd(ptr(y), ptr(scale), ptr(shift), ptr(skip), W + 3, off, ptr(out), N, H, W, C, up, pad, _f(slope),
-                               int(post), stream_ptr(y)) == 0
+    assert lib.b3d_cbn_act_fwd(ptr(y), ptr(scale), ptr(shift), ptr(skip), W + 3, off, ptr(out), N, H, W, C, up, pad, pad_mode,
+                               _f(slope), int(post), stream_ptr(y)) == 0
     torch.cuda.synchronize()
     h = F.leaky_relu(y.double() * scale.double()[:, None, None] + shift.double()[:, None, None], slope) \
         + skip.double()[:, :, off:off + W]
@@ -446,7 +448,8 @@ def test_cbn_act_fwd_generic_kernel(C, up, pad, post):
     h = h.permute(0, 3, 1, 2)
     if up == 2:
         h = F.interpolate(h, scale_factor=2, mode='nearest')
-    want = F.pad(h, (pad, pad, 0, 0), mode='replicate').permute(0, 2, 3, 1)
+    want = (F.pad(h, (pad, pad, 0, 0), mode='replicate') if pad_mode == 0 else
+            torch.cat((h[..., -pad:], h, h[..., :pad]), dim=3)).permute(0, 2, 3, 1)
     e = float((out.double() - want).abs().max())
     assert e <= 1e-6 * float(want.abs().max()), f"generic cbn_act_fwd differs by {e:.2e}"
 

@@ -118,7 +118,7 @@ def test_in_act_pad_rejects_bad_shapes_before_cuda():
         in_act_pad(torch.zeros(2, 16, 4, 4), norm, 1)
 
 
-def test_new_entry_points_validate_arguments_without_gpu():
+def test_glue_entry_points_validate_arguments_without_gpu():
     """The C entry points check their arguments before any CUDA call (error code, message, no launch)."""
     import b3d
     lib = b3d.lib
@@ -126,12 +126,12 @@ def test_new_entry_points_validate_arguments_without_gpu():
     assert lib.b3d_bn_sums_per_sample(None, 2, 32, 12, None, None) != 0
     assert b"4 * a divisor" in lib.b3d_last_error()
     assert lib.b3d_bn_sums_per_sample(None, 0, 32, 16, None, None) != 0
-    assert lib.b3d_cbn_act_fwd_ex(None, None, None, None, 0, 0, None, 2, 4, 2, 16, 1, 3, 1, 0.2, 0, None) != 0
+    assert lib.b3d_cbn_act_fwd(None, None, None, None, 0, 0, None, 2, 4, 2, 16, 1, 3, 1, 0.2, 0, None) != 0
     assert b"pad mode" in lib.b3d_last_error()
-    assert lib.b3d_cbn_act_bwd1_ex(None, None, None, None, None, 0, 0, None, None, 8, None, None, 0, 0, None, None, 16, 2, 4, 4,
-                                   16, 1, 1, 1, 0.2, 0, None) != 0
+    assert lib.b3d_cbn_act_bwd1(None, None, None, None, None, 0, 0, None, None, 8, None, None, 0, 0, None, None, 16, 2, 4, 4,
+                                16, 1, 1, 1, 0.2, 0, None) != 0
     assert b"statistics pitch" in lib.b3d_last_error()
-    assert lib.b3d_cbn_act_bwd2_ex(None, None, None, None, None, 16, None, None, 6, 0.5, 2, 4, 4, 16, None) != 0
+    assert lib.b3d_cbn_act_bwd2(None, None, None, None, None, 16, None, None, 6, 0.5, 2, 4, 4, 16, None) != 0
     assert b"statistics pitch" in lib.b3d_last_error()
     assert lib.b3d_cbn_prepare(None, 0, 0, 0, None, 0.0, 1e-5, 0.1, 5, None, None, None, None, None, None, None, None, 2, 16,
                                None) != 0

@@ -192,19 +192,22 @@ def test_generator_block_glue(blk):
     run_glue(32, [L(cout, H, W), L(cout, H, W, up, pad, skip, post)], kind='cbn', chain=True, seed=len(name))
 
 
-# reconstruction decoder (texture_res 64, batch 50): name, C_in, C_out, H x W at the block's input, up, pad, ReLU after add
+# reconstruction decoder as the benchmark trains it (texture_res 128, symmetric: half-width maps): name, C_in, C_out, H x W
+# at the block's input, up, pad, ReLU after add
 REC_BLOCKS = [("blk1", 256, 512, 4, 2, 2, 1, False), ("blk2", 512, 256, 8, 4, 2, 1, False), ("blk3", 256, 256, 16, 8, 2, 1, False),
-              ("blk4_tex", 256, 128, 32, 16, 2, 1, False), ("blk5_tex", 128, 64, 64, 32, 1, 2, True),
-              ("blk4_mesh", 256, 64, 32, 16, 1, 2, True)]
+              ("blk3b_tex", 256, 256, 32, 16, 2, 1, False), ("blk4_tex", 256, 128, 64, 32, 2, 1, False),
+              ("blk5_tex", 128, 64, 128, 64, 1, 2, True), ("blk4_mesh", 256, 64, 32, 16, 1, 2, True)]
+# batch 50 on one GPU, 13 per rank under DDP x4
+REC_CASES = [(b, n) for n in (50, 13) for b in REC_BLOCKS]
 
 
-@pytest.mark.parametrize("blk", REC_BLOCKS, ids=[b[0] for b in REC_BLOCKS])
-def test_reconstruction_block_glue(blk):
+@pytest.mark.parametrize("blk,N", REC_CASES, ids=[b[0] if n == 50 else f"{b[0]}-N{n}" for b, n in REC_CASES])
+def test_reconstruction_block_glue(blk, N):
     """ResBlock.forward_fused's two calls (BatchNorm2d weight / bias shared by the batch, ReLU = slope 0)."""
     name, cin, cout, H, W, up, pad, post = blk
     skip = 'id' if cin == cout else 'sc'
     print(name)
-    run_glue(50, [L(cin, H, W, slope=0.0), L(cout, H, W, up, pad, skip, post, slope=0.0)], kind='bn', seed=len(name))
+    run_glue(N, [L(cin, H, W, slope=0.0), L(cout, H, W, up, pad, skip, post, slope=0.0)], kind='bn', seed=len(name))
 
 
 EDGES = {

@@ -11,6 +11,8 @@ import ctypes
 import pytest
 import torch
 
+import conv_plan as P
+
 TOL = 4e-3
 B = 32
 # name, N, Cin, H, W (x-padded), Cout, k, pad_y, stride — the weight-gradient launches of one cfg3 step
@@ -32,37 +34,14 @@ def _out_size(H, W, kh, kw, pad_y, st):
     return (H + 2 * pad_y - kh) // st + 1, (W - kw) // st + 1
 
 
-def _pow2_floor(v):
-    p = 1
-    while p * 2 <= v:
-        p *= 2
-    return p
-
-
-def _k_split(N, Hout, Wout, Cin, Cout, kh, kw, st, sms):
-    """(K slices, K splits) as b3d_conv2d_wgrad_tf32 chooses them."""
-    bwk = _pow2_floor(min(Wout, 32))
-    ktotal = N * -(-Wout // bwk) * -(-Hout // (32 // bwk))
-    bn = 128 if Cin > 64 else 64
-    t = 1
-    if Wout >= 32 and st == 1 and kw == 3 and bn == 64:
-        t = 3
-    if Wout >= 32 and st == 2 and kw == 4:
-        t = 2
-    base = -(-Cout // 128) * -(-Cin // bn) * kh * (kw // t)
-    splits = min(-(-2 * sms // base), ktotal // 8)
-    return ktotal, max(splits, 1)
-
-
 def test_cfg3_has_a_ragged_k_split():
-    """On an H100 SXM (132 SMs) the K slices of some geometries do not divide evenly among their splits (the k_lo / k_hi
-    rounding of the kernel is exercised)."""
+    """On an H100 SXM (132 SMs) the K slices of some geometries do not divide evenly among the splits wgrad_splits picks
+    (the k_lo / k_hi rounding of the kernel is exercised)."""
     ragged = []
     for _, N, Cin, H, W, Cout, k, py, st in CFG3:
         kh, kw = _kh_kw(k)
-        Hout, Wout = _out_size(H, W, kh, kw, py, st)
-        ktotal, splits = _k_split(N, Hout, Wout, Cin, -(-Cout // 32) * 32, kh, kw, st, 132)
-        ragged.append(ktotal % splits != 0)
+        (launch,) = P.wgrad_tf32(N, H, W, Cin, -(-Cout // 32) * 32, kh, kw, py, st, sms=132)
+        ragged.append(launch.kslices % launch.splits != 0)
     assert any(ragged)
 
 
@@ -119,7 +98,7 @@ def _ref_wgrad(dy, x, kh, kw, pad_y, st):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,N,Cin,H,W,Cout,k,pad_y,st", CFG3, ids=[c[0] for c in CFG3])
 def test_wgrad_cfg3_geometry(name, N, Cin, H, W, Cout, k, pad_y, st):
-    from b3d import check, lib, ptr, stream_ptr
+    from b3d import check, last_variant, lib, ptr, stream_ptr
     dev = "cuda:0"
     kh, kw = _kh_kw(k)
     Cout = -(-Cout // 32) * 32                     # the channel padding b3d.conv applies to thin heads
@@ -135,6 +114,8 @@ def test_wgrad_cfg3_geometry(name, N, Cin, H, W, Cout, k, pad_y, st):
     a = torch.zeros(Cout, Cin, kh, kw, device=dev)
     check(lib.b3d_conv2d_wgrad_tf32(ptr(dy), ptr(x), ptr(a), N, H, W, Cin, Hout, Wout, Cout, kh, kw, pad_y, st, 0, 0, 0, 0,
                                     stream_ptr(x)))
+    (plan,) = P.wgrad_tf32(N, H, W, Cin, Cout, kh, kw, pad_y, st, sms=torch.cuda.get_device_properties(0).multi_processor_count)
+    assert last_variant() == plan.instance, (name, last_variant(), plan)
     b = torch.zeros(kh * kw, Cout, Cin, device=dev)
     check(lib.b3d_conv2d_wgrad_tf32(ctypes.c_void_p(dywide.data_ptr()), ptr(xwide), ptr(b), N, H, W + 2, Cin, Hout, Wout, Cout,
                                     kh, kw, pad_y, st, 1, 1, 0, pitch, stream_ptr(x)))

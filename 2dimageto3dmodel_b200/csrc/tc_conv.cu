@@ -13,9 +13,10 @@
 //   * dgrad   (dy = pad_y - r, dx = -s, Wt[t] = W[:, :, r, s]^T)  — the "full" correlation falls out of the
 //     TMA zero fill, and strided (4x4 / stride 2) dgrad runs as 4 parity classes with a strided epilogue,
 //   * strided fprop (element strides in the tensor map).
-// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread issues), warpgroups 1-2 = wgmma on pixel rows 0-63 /
-// 64-127 of the tile (BN = 64: on alternate work items, the whole tile each, weights as the M operand) and the epilogue
-// straight from the accumulator registers (bias / LeakyReLU / BN statistics / fused activation adjoint -> global).
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread issues), warpgroups 1-2 = wgmma with the weights as the
+// M operand (64-channel blocks) and the 128-pixel tile as the N operand — on alternate work items with BN <= 128, on one
+// 128-channel half of every item with BN = 256 — and the epilogue straight from the accumulator registers (bias /
+// LeakyReLU / BN statistics / fused activation adjoint -> global).
 // Persistent: a CTA per SM walks the work items; the STAGES-deep mbarrier ring keeps the producer loading the next item
 // while the consumers run the epilogue of the current one.  The fused activation adjoint's mask travels through the same
 // ring: after an item's K steps the producer loads its mask tile as BN / 32 more stages (one 128-pixel x 32-channel TMA box
@@ -24,7 +25,7 @@
 
 namespace {
 
-constexpr int BM = 128;         // output pixels per work item (two m64 warpgroup tiles)
+constexpr int BM = 128;         // output pixels per work item (the N of one m64n128k8 per 64-channel block)
 constexpr int BK = 32;          // fp32 channels per K slice = 128 B = one swizzle row
 constexpr int MMA_K = 8;        // tf32
 constexpr int MAX_TAPS = 25;
@@ -67,7 +68,7 @@ struct CSmem {
     static constexpr int B_BYTES = KW * BN * BK * 4;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int TX_BYTES = WIN_BYTES + B_BYTES;
-    static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * BN * 4 /*BN statistics*/;
+    static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
     static_assert(A_BYTES >= MASK_BYTES, "a mask chunk does not fit the A region of a stage");
 };
 
@@ -75,38 +76,47 @@ struct CSmem {
 // box's 128-byte pixel rows with the 128-byte swizzle (16-byte chunk index XOR px % 8; stages are 1024-byte aligned).
 __device__ __forceinline__ uint32_t mask_offset(int px, int ch) { return px * 128 + ((((ch >> 2) ^ px) & 7) << 4) + (ch & 3) * 4; }
 
-// BN == 64 swaps the operands: the 64 x 32 weight tile is the M operand and the whole 128-pixel tile the N operand of one
-// m64n128k8 per K step (6 KB of shared memory read per 65 536 MACs instead of 4 KB per 32 768), and each consumer
+// Every tile width swaps the operands: the BN x 32 weight tile is the M operand, in 64-channel blocks, and the whole
+// 128-pixel tile the N operand of one m64n128k8 per block and K step (6 KB of shared memory read per 65 536 MACs).  A
+// consumer warpgroup holds at most 128 channels x 128 pixels (128 accumulator registers per thread).  With BN <= 128 each
 // warpgroup owns whole work items (item k of the CTA goes to warpgroup k % 2), so one warpgroup's epilogue overlaps the
-// other's main loop.
+// other's main loop.  With BN == 256 (kCoop) both warpgroups work on every item, warpgroup h on channels 128 h .. 128 h + 127.
 template <int BN>
-constexpr bool kSwap = BN == 64;
+constexpr bool kCoop = BN > 128;
 template <int BN>
-constexpr int kAcc = kSwap<BN> ? BM / 2 : BN / 2;      // accumulator registers per consumer thread
-// Arrivals that hand a stage back to the producer.  A mask stage is read with shared-memory loads, and each warp that read
-// it arrives once (all 8 consumer warps with BN >= 128; with kSwap the 2 warps of the owner whose 32 channels it holds).
-// An operand stage, read by wgmma, gets the same total from the leader of each warpgroup that read it.
+constexpr int kBlocks = (kCoop<BN> ? BN / 2 : BN) / 64;       // 64-channel M blocks per consumer warpgroup
+// Arrivals that hand a stage back to the producer: every consumer warp that waits on the stage's full barrier takes part,
+// the 4 warps of the item's owner (8 with kCoop).  An operand stage, read by wgmma, gets 4 from the leader of each
+// warpgroup that read it once the wgmma group has retired; a mask stage gets one from each warp once the warp's loads of
+// its block are done, whether or not it read that stage.  So no stage is refilled before every warp that waits on it has
+// seen the fill: phase bits never skip a phase, and no wait can see a barrier two phases on.
 template <int BN>
-constexpr int kEmptyArrivals = kSwap<BN> ? 2 : 8;
+constexpr int kEmptyArrivals = kCoop<BN> ? 8 : 4;
+template <int BN>
+constexpr int kLeaderArrivals = kEmptyArrivals<BN> / (kCoop<BN> ? 2 : 1);     // per warpgroup leader, for an operand stage
+static_assert(kLeaderArrivals<64> == 4 && kLeaderArrivals<128> == 4 && kLeaderArrivals<256> == 4,
+              "a leader stands for the 4 warps of its warpgroup");
+// Mask stages per 64-channel block of an item: the two 32-channel chunks of the block of each warpgroup on the item.  Item
+// mask stage i holds the chunk of block i / G, warpgroup (i % G) / 2, channels c0 + 128 ((i % G) / 2) + 64 (i / G) + 32 (i % 2):
+// the chunks that the warpgroups read at the same time are in the ring at the same time (G <= STAGES), and a block's
+// stages are handed back before the next block's are waited on.
+template <int BN>
+constexpr int kMaskGroup = kCoop<BN> ? 4 : 2;
+__host__ __device__ constexpr int mask_chunk_channel(int i, int G) { return 128 * ((i % G) / 2) + 64 * (i / G) + 32 * (i % 2); }
 
-// The K loop of one work item for one consumer warpgroup: rows [64 h, 64 h + 64) of the 128 x BN accumulator, or with
-// kSwap the whole 64 x 128 (channel x pixel) transposed one.  With kSwap, `full` is the warpgroup's own row of full
-// barriers and `phase` holds the parity of its next wait on each of them: a warpgroup that skips the other's stages
-// cannot derive it from git, and on a shared barrier it could wait for a phase before the previous one completed.  A stage is handed back to the producer once the wgmma group that read it has retired (by the leader
-// of each warpgroup that reads it, see kEmptyArrivals).
+// The K loop of one work item for one consumer warpgroup: its kBlocks 64 x 128 (channel x pixel) accumulators, channels
+// cb .. of the item's weight tile.  `full` is the warpgroup's row of full barriers and `phase` holds the parity of its next
+// wait on each of them: with BN <= 128 a warpgroup skips the other's stages, so it cannot derive the parity from git.  A
+// stage is handed back to the producer once the wgmma group that read it has retired (kEmptyArrivals).
 template <int BN, int STAGES, int KW, bool FOLD>
-__device__ __forceinline__ void mainloop(float (&acc)[kAcc<BN>], unsigned char* base, uint64_t* full, uint64_t* empty, int KI,
-                                         uint32_t& git, uint32_t& phase, int h, bool leader, const int* shift) {
+__device__ __forceinline__ void mainloop(float (&acc)[kBlocks<BN>][BM / 2], unsigned char* base, uint64_t* full, uint64_t* empty,
+                                         int KI, uint32_t& git, uint32_t& phase, int cb, bool leader, const int* shift) {
     constexpr int A_BYTES = CSmem<BN, STAGES, KW>::A_BYTES, STAGE = CSmem<BN, STAGES, KW>::STAGE_BYTES;
     for (int it = 0; it < KI; ++it, ++git) {
         const int s = git % STAGES;
-        if constexpr (kSwap<BN>) {
-            tc::mbar_wait(full + s, (phase >> s) & 1);
-            phase ^= 1u << s;
-        } else {
-            tc::mbar_wait(full + s, (git / STAGES) & 1);
-        }
-        const uint32_t a = tc::smem_u32(base + s * STAGE), b = a + A_BYTES;
+        tc::mbar_wait(full + s, (phase >> s) & 1);
+        phase ^= 1u << s;
+        const uint32_t a = tc::smem_u32(base + s * STAGE), b = a + A_BYTES + cb * 128;
         tc::wgmma_fence();
 #pragma unroll
         for (int t = 0; t < KW; ++t) {
@@ -114,23 +124,19 @@ __device__ __forceinline__ void mainloop(float (&acc)[kAcc<BN>], unsigned char* 
 #pragma unroll
             for (int k = 0; k < BK / MMA_K; ++k) {
                 const uint32_t acc_flag = (it | t | k) ? 1u : 0u;
-                if constexpr (kSwap<BN>) {
-                    // on-the-fly fold: K step k = image row k of the 4-row box, a [128 px][32 B] tile of its own (32-byte swizzle)
-                    const uint64_t dp = FOLD ? tc::desc_k32(a + k * (BM * 32)) : tc::desc_k128(shifted + k * MMA_K * 4);
-                    tc::Wgmma<BM>::mma(acc, tc::desc_k128(b + t * (BN * 128) + k * MMA_K * 4), dp, acc_flag);
-                } else {
-                    const uint64_t da = FOLD ? tc::desc_k32(a + k * (BM * 32) + h * (64 * 32))
-                                             : tc::desc_k128(shifted + h * (64 * 128) + k * MMA_K * 4);
-                    tc::Wgmma<BN>::mma(acc, da, tc::desc_k128(b + t * (BN * 128) + k * MMA_K * 4), acc_flag);
-                }
+                // on-the-fly fold: K step k = image row k of the 4-row box, a [128 px][32 B] tile of its own (32-byte swizzle)
+                const uint64_t dp = FOLD ? tc::desc_k32(a + k * (BM * 32)) : tc::desc_k128(shifted + k * MMA_K * 4);
+#pragma unroll
+                for (int m = 0; m < kBlocks<BN>; ++m)
+                    tc::Wgmma<BM>::mma(acc[m], tc::desc_k128(b + t * (BN * 128) + m * (64 * 128) + k * MMA_K * 4), dp, acc_flag);
             }
         }
         tc::wgmma_commit();
         tc::wgmma_wait<1>();
-        if (it > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES, kEmptyArrivals<BN> / (kSwap<BN> ? 1 : 2));
+        if (it > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES, kLeaderArrivals<BN>);
     }
     tc::wgmma_wait<0>();
-    if (KI > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES, kEmptyArrivals<BN> / (kSwap<BN> ? 1 : 2));
+    if (KI > 0 && leader) tc::mbar_arrive(empty + (git - 1) % STAGES, kLeaderArrivals<BN>);
 }
 
 // Where a work item's 128-pixel tile lies in the output tensor (and in the mask, which has the output's geometry): pixel
@@ -154,14 +160,41 @@ __device__ __forceinline__ bool tile_pixel(const ConvParams& p, const TileAt& t,
     return t.n0 + bi < p.N && t.y0 + by < p.Hout && t.x0 + bx < p.Wout;
 }
 
-// Epilogue of a BN == 64 item: this thread holds D[co][px] for the channels c0 + cw, c0 + cw + 8 and the pixels
-// 8 j + 2 (lane % 4) + {0, 1}.  MASKED: the warp's 16 channels lie in one 32-channel chunk, whose mask stage starts at
-// shared address `mstage`; the warp loads its 32 mask values per thread from it, hands the stage back (`mempty`) and
-// applies the slope with a select: t * (m >= 0 ? 1 : slope)  is pad_leaky_bias_bwd_kernel's  !(m >= 0) -> slope  rule,
-// NaN included.  Across the warp the loads of one (j, e1, e2) cover 8 chunk indices x 4 words: conflict-free.
+// The mask of one 64-channel block as sign bits: this thread's 64 values (channels cw, cw + 8 of the warp's 32-channel
+// chunk, whose mask stage starts at shared address `mstage`; pixels 8 j + 2 (lane % 4) + {0, 1}) become bit 4 j' + 2 e2 + e1
+// of neg[j / 8] (j' = j % 8), set where !(m >= 0): the slope rule of pad_leaky_bias_bwd_kernel, NaN included.  The
+// warp then hands back all G mask stages of the block (ring positions g0 .. g0 + G - 1, see kEmptyArrivals) before any
+// epilogue arithmetic, so an item's mask stages leave the ring as soon as they are read.  Across the warp the loads of
+// one (j, e1, e2) cover 8 chunk indices x 4 words: conflict-free.
+template <int G, int STAGES>
+__device__ __forceinline__ void mask_bits(uint32_t (&neg)[2], uint32_t mstage, int cw, int lane, uint64_t* empty, uint32_t g0) {
+    int q;                                                                // a zero the compiler cannot see through, as below
+    asm volatile("mov.u32 %0, 0;" : "=r"(q));
+    q += 2 * (lane & 3);
+    // mask element [e2][e1] of pixel q + e1 and chunk channel (cw + 8 e2) % 32; pixel 8 j further is 1024 j bytes further
+    uint32_t mb[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) mb[i] = mstage + mask_offset(q + (i & 1), (cw + 8 * (i >> 1)) & 31);
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+        uint32_t bits = 0;
+#pragma unroll
+        for (int j = 0; j < BM / 16; ++j)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) bits |= (tc::lds_f32(mb[i] + 1024 * (j + 8 * hf)) >= 0.f ? 0u : 1u) << (4 * j + i);
+        neg[hf] = bits;
+    }
+    __syncwarp();
+    if (lane == 0)
+#pragma unroll
+        for (int i = 0; i < G; ++i) tc::mbar_arrive(empty + (g0 + i) % STAGES);
+}
+
+// Epilogue of one 64-channel block of an item: this thread holds D[co][px] for the channels c0 + cw, c0 + cw + 8 and the
+// pixels 8 j + 2 (lane % 4) + {0, 1}.  MASKED: the value is multiplied by the slope where its bit in `neg` (mask_bits) is set.
 template <bool MASKED>
-__device__ __forceinline__ void epilogue_swapped(const float (&acc)[BM / 2], const ConvParams& p, const TileAt& t, const float* bias,
-                                                 float* out, int c0, int cw, int lane, uint32_t mstage, uint64_t* mempty) {
+__device__ __forceinline__ void epilogue_block(const float (&acc)[BM / 2], const uint32_t (&neg)[2], const ConvParams& p, const TileAt& t,
+                                               const float* bias, float* out, int c0, int cw, int lane) {
     bool cok[2];
     float bv[2], sum[2] = {0.f, 0.f}, sq[2] = {0.f, 0.f};
 #pragma unroll
@@ -175,16 +208,6 @@ __device__ __forceinline__ void epilogue_swapped(const float (&acc)[BM / 2], con
     int q;
     asm volatile("mov.u32 %0, 0;" : "=r"(q));
     q += 2 * (lane & 3);
-    float m[MASKED ? BM / 2 : 1];                                         // [block j][e2][e1], as acc
-    if constexpr (MASKED) {
-#pragma unroll
-        for (int j = 0; j < BM / 8; ++j)
-#pragma unroll
-            for (int i = 0; i < 4; ++i)                                   // pixel 8 j + q + e1 (px % 8 == q + e1), chunk channel (cw + 8 e2) % 32
-                m[4 * j + i] = tc::lds_f32(mstage + mask_offset(8 * j + q + (i & 1), (cw + 8 * (i >> 1)) & 31));
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(mempty);
-    }
 #pragma unroll
     for (int j = 0; j < BM / 8; ++j) {
 #pragma unroll
@@ -194,7 +217,7 @@ __device__ __forceinline__ void epilogue_swapped(const float (&acc)[BM / 2], con
 #pragma unroll
             for (int e2 = 0; e2 < 2; ++e2) {
                 float v = acc[4 * j + 2 * e2 + e1];
-                if constexpr (MASKED) v *= m[4 * j + 2 * e2 + e1] >= 0.f ? 1.f : p.mslope;
+                if constexpr (MASKED) v *= (neg[j / 8] >> (4 * (j % 8) + 2 * e2 + e1)) & 1u ? p.mslope : 1.f;
                 v = valid ? v : 0.f;
                 sum[e2] += v;
                 sq[e2] += v * v;
@@ -206,7 +229,7 @@ __device__ __forceinline__ void epilogue_swapped(const float (&acc)[BM / 2], con
         }
     }
     if (p.stats) {
-        // the four lanes of a quad hold the channel's 128 pixels; warp w alone holds channels 16 w .. 16 w + 15
+        // the four lanes of a quad hold the channel's 128 pixels; warp w alone holds channels c0 + 16 w .. c0 + 16 w + 15
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
             sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 1);
@@ -221,73 +244,10 @@ __device__ __forceinline__ void epilogue_swapped(const float (&acc)[BM / 2], con
     }
 }
 
-// Epilogue of a BN >= 128 item: this thread holds two pixel rows (validity and offsets in valid[] / off[]) x the channel pairs
-// c0 + 2 (lane % 4) + 8 j + {0, 1}.  One 8-wide column block at a time, without writing the accumulators (they stay
-// wgmma-only registers).  MASKED: chunk m of the item's mask (channels c0 + 32 m ..) is in ring stage git + m; before column
-// block 4 m each thread waits for it, loads its 4 blocks x 2 rows as channel pairs and its warp hands the stage back.  A
-// stage is consumed in chunk order, so the BN / 32 chunks may outnumber the stages of the ring.  Across the warp one load
-// covers 8 pixel rows (px % 8 == lane / 4) x 2 chunk indices x 2 pairs: two wavefronts of 32 banks, the least 256 bytes take.
-template <int BN, int STAGES, int STAGE_BYTES, bool MASKED>
-__device__ __forceinline__ void epilogue_rows(const float (&acc)[BN / 2], const ConvParams& p, const bool (&valid)[2],
-                                              const size_t (&off)[2], const float* bias, float* out, float* sm_stats, int c0, int lane,
-                                              int row_a, uint32_t ring, uint64_t* full, uint64_t* empty, uint32_t git) {
-    const int cq = c0 + 2 * (lane & 3);                           // first channel of this thread's column pair in block j: cq + 8 j
-    const bool vec = (p.OC & 1) == 0;
-#pragma unroll
-    for (int m = 0; m < BN / 32; ++m) {
-        float2 mk[MASKED ? 4 : 1][2];                             // [column block][row a / b]
-        if constexpr (MASKED) {
-            const uint32_t g = git + m, s = g % STAGES;
-            tc::mbar_wait(full + s, (g / STAGES) & 1);
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) mk[jj][e] = tc::lds_f32x2(ring + s * STAGE_BYTES + mask_offset(row_a + 8 * e, 8 * jj + 2 * (lane & 3)));
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(empty + s);
-        }
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-            const int j = 4 * m + jj;
-            float v[2][2];                                            // [row a / b][column pair]
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int e = i >> 1;
-                float t = acc[4 * j + i];
-                if constexpr (MASKED) t *= ((i & 1) ? mk[jj][e].y : mk[jj][e].x) >= 0.f ? 1.f : p.mslope;
-                v[e][i & 1] = valid[e] ? t : 0.f;
-            }
-            if (p.stats) tc::stats_accumulate8(v[0], v[1], sm_stats, BN, 8 * j, p.stats_sum != 0);
-            const int co = cq + 8 * j;
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                if (!valid[e]) continue;
-                float* dst = out + off[e];
-                float o0 = v[e][0], o1 = v[e][1];
-                if (vec && co + 1 < p.Cout) {
-                    if (bias) { o0 += __ldg(bias + co); o1 += __ldg(bias + co + 1); }
-                    o0 = o0 >= 0.f ? o0 : o0 * p.leaky;
-                    o1 = o1 >= 0.f ? o1 : o1 * p.leaky;
-                    *reinterpret_cast<float2*>(dst + co) = make_float2(o0, o1);
-                } else {
-                    if (co < p.Cout) {
-                        o0 += bias ? __ldg(bias + co) : 0.f;
-                        dst[co] = o0 >= 0.f ? o0 : o0 * p.leaky;
-                    }
-                    if (co + 1 < p.Cout) {
-                        o1 += bias ? __ldg(bias + co + 1) : 0.f;
-                        dst[co + 1] = o1 >= 0.f ? o1 : o1 * p.leaky;
-                    }
-                }
-            }
-        }
-    }
-}
-
-// registers move from the producer warpgroup (one thread issues TMA) to the consumers: at an even 168 per thread the 64- and
-// 256-wide instantiations spill (the 64-wide masked epilogue holds its 32 mask values next to the accumulators);
-// 128 * (168 - 40) == 256 * (232 - 168)
-constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+// registers move from the producer warpgroup (one thread issues TMA) to the consumers: the 128- and 256-wide consumers hold
+// 128 accumulators, and gather a block's mask bits from 32 loaded values at a time next to them (at 232 that spills);
+// 128 * (168 - 24) == 256 * (240 - 168)
+constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 240;
 
 // tmap_m: the mask (masked launches only), dims {OC, OW, OH, N}, box {32, osx (BW - 1) + 1, osy (BH - 1) + 1, BI} with
 // element strides {1, osx, osy, 1}: pixel px of the box lands as row px of the tile, zero-filled outside the tensor
@@ -297,15 +257,15 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                   const __grid_constant__ CUtensorMap tmap_m, const ConvParams p, const float* __restrict__ bias,
                   float* __restrict__ out, int tiles, int work_items) {
     using S = CSmem<BN, STAGES, KW>;
-    constexpr bool SWAP = kSwap<BN>;
-    constexpr int OWNERS = SWAP ? 2 : 1;               // rows of full barriers: one per warpgroup that owns items
+    constexpr bool COOP = kCoop<BN>;
+    constexpr int OWNERS = COOP ? 1 : 2;               // rows of full barriers: one per warpgroup that owns items
+    constexpr int G = kMaskGroup<BN>;
+    static_assert(G <= STAGES, "the mask stages of one block do not fit the ring");
     extern __shared__ unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * S::STAGE_BYTES);     // [OWNERS][STAGES]
     uint64_t* empty = full + OWNERS * STAGES;
     static_assert((OWNERS + 1) * STAGES * 8 <= 256, "barriers do not fit their area");
-    float* sm_stats = reinterpret_cast<float*>(base + STAGES * S::STAGE_BYTES + 256);
-    for (int i = threadIdx.x; i < 2 * BN; i += blockDim.x) sm_stats[i] = 0.f;
     if (threadIdx.x == 0) {
         tc::tma_prefetch_desc(&tmap_x);
         tc::tma_prefetch_desc(&tmap_w);
@@ -326,7 +286,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         if (threadIdx.x == 0) {
             uint32_t git = 0;
             for (int w = blockIdx.x, k = 0; w < work_items; w += gridDim.x, ++k) {
-                uint64_t* fb = full + (SWAP ? (k & 1) * STAGES : 0);     // the owner's full barriers
+                uint64_t* fb = full + (COOP ? 0 : (k & 1) * STAGES);     // the owner's full barriers
                 // classes are the fastest index: the CTAs that work on the same pixel tiles at the same time share them in L2
                 const int cls = w % p.ncls, wq = w / p.ncls, tb = cls * p.ntaps;
                 int t = wq % tiles;
@@ -353,7 +313,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
                     const int s = git % STAGES;
                     tc::mbar_wait(empty + s, ((git / STAGES) & 1) ^ 1);
                     tc::mbar_arrive_expect_tx(fb + s, MASK_BYTES);
-                    tc::tma_load_4d(base + s * S::STAGE_BYTES, &tmap_m, fb + s, c0 + 32 * m, mx, my, n0);
+                    tc::tma_load_4d(base + s * S::STAGE_BYTES, &tmap_m, fb + s, c0 + mask_chunk_channel(m, G), mx, my, n0);
                 }
             }
         }
@@ -362,66 +322,49 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     tc::setmaxnreg_inc<CONSUMER_REGS>();
 
     const int h = wg - 1, tid = threadIdx.x & 127, lane = tid & 31;
-    float acc[kAcc<BN>];
+    float acc[kBlocks<BN>][BM / 2];
 #pragma unroll
-    for (int i = 0; i < kAcc<BN>; ++i) acc[i] = 0.f;
+    for (int m = 0; m < kBlocks<BN>; ++m)
+#pragma unroll
+        for (int i = 0; i < BM / 2; ++i) acc[m][i] = 0.f;
     uint32_t git = 0, phase = 0;
     const uint32_t ring = tc::smem_u32(base);
     TileAt at;
     at.lbw = __ffs(p.BW) - 1;
     at.lbwh = at.lbw + __ffs(p.BH) - 1;
-
-    if constexpr (SWAP) {
-        uint64_t* fb = full + h * STAGES;
-        const int cw = (tid >> 5) * 16 + (lane >> 2);
-        for (int k = h;; k += 2) {
-            const int w = blockIdx.x + k * gridDim.x;
-            if (w >= work_items) break;
-            git = (uint32_t)k * (KI + MS);                                     // skip the other warpgroup's items
-            const int wq = w / p.ncls, tile = wq % tiles, c0 = (wq / tiles) * BN;
-            tile_origin(p, at, tile, w % p.ncls);
-            if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, fb, empty, KI, git, phase, h, tid == 0, p.shift);
-            else mainloop<BN, STAGES, KW, false>(acc, base, fb, empty, KI, git, phase, h, tid == 0, p.shift);
-            if (p.mask) {
-                // every warp waits for both mask stages, so that its phase bits stay those of the barriers; warp w reads
-                // chunk w / 2 (its channels 16 w .. 16 w + 15)
-                uint32_t mstage = 0;
-                uint64_t* mempty = empty;
+    uint64_t* fb = full + (COOP ? 0 : h * STAGES);
+    const int cb = COOP ? 128 * h : 0;                 // the warpgroup's first channel in the item's tile
+    const int cw = (tid >> 5) * 16 + (lane >> 2);
+    const int mine = (COOP ? 2 * h : 0) + (tid >> 6);  // which of a block's G mask stages holds this warp's 16 channels
+    for (int k = COOP ? 0 : h;; k += COOP ? 1 : 2) {
+        const int w = blockIdx.x + k * gridDim.x;
+        if (w >= work_items) break;
+        git = (uint32_t)k * (KI + MS);                                         // skip the other warpgroup's items
+        const int wq = w / p.ncls, tile = wq % tiles, c0 = (wq / tiles) * BN + cb;
+        tile_origin(p, at, tile, w % p.ncls);
+        if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, fb, empty, KI, git, phase, cb, tid == 0, p.shift);
+        else mainloop<BN, STAGES, KW, false>(acc, base, fb, empty, KI, git, phase, cb, tid == 0, p.shift);
+        uint32_t neg[kBlocks<BN>][2] = {};
+        if (p.mask) {
+            // every warp waits for all G stages of a block, so that its phase bits stay those of the barriers, and reads the
+            // one that holds its channels; all of the item's mask stages are handed back before the first block's epilogue
 #pragma unroll
-                for (int m = 0; m < BN / 32; ++m, ++git) {
-                    const int s = git % STAGES;
+            for (int m = 0; m < kBlocks<BN>; ++m, git += G) {
+                uint32_t mstage = 0;
+#pragma unroll
+                for (int i = 0; i < G; ++i) {
+                    const int s = (git + i) % STAGES;
                     tc::mbar_wait(fb + s, (phase >> s) & 1);
                     phase ^= 1u << s;
-                    if (m == (tid >> 6)) { mstage = ring + s * S::STAGE_BYTES; mempty = empty + s; }
+                    if (i == mine) mstage = ring + s * S::STAGE_BYTES;
                 }
-                epilogue_swapped<true>(acc, p, at, bias, out, c0, cw, lane, mstage, mempty);
-            } else {
-                epilogue_swapped<false>(acc, p, at, bias, out, c0, cw, lane, 0, nullptr);
+                mask_bits<G, STAGES>(neg[m], mstage, cw, lane, empty, git);
             }
         }
-    } else {
-        const int row_a = h * 64 + (tid >> 5) * 16 + (lane >> 2);          // this thread's two accumulator rows: row_a, row_a + 8
-        for (int w = blockIdx.x; w < work_items; w += gridDim.x) {
-            const int wq = w / p.ncls, tile = wq % tiles, c0 = (wq / tiles) * BN;
-            tile_origin(p, at, tile, w % p.ncls);
-            if (KW == 1 && p.fold) mainloop<BN, STAGES, KW, true>(acc, base, full, empty, KI, git, phase, h, tid == 0, p.shift);
-            else mainloop<BN, STAGES, KW, false>(acc, base, full, empty, KI, git, phase, h, tid == 0, p.shift);
-
-            bool valid[2];
-            size_t off[2];
-    #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                uint32_t rel;
-                valid[e] = tile_pixel(p, at, row_a + 8 * e, rel);
-                off[e] = at.base + rel;
-            }
-            if (p.mask) {
-                epilogue_rows<BN, STAGES, S::STAGE_BYTES, true>(acc, p, valid, off, bias, out, sm_stats, c0, lane, row_a, ring, full, empty, git);
-                git += MS;
-            } else {
-                epilogue_rows<BN, STAGES, S::STAGE_BYTES, false>(acc, p, valid, off, bias, out, sm_stats, c0, lane, row_a, ring, full, empty, git);
-            }
-            if (p.stats) tc::stats_flush(sm_stats, BN, p.stats, p.Cout, c0, threadIdx.x - 128, 256);
+#pragma unroll
+        for (int m = 0; m < kBlocks<BN>; ++m) {
+            if (p.mask) epilogue_block<true>(acc[m], neg[m], p, at, bias, out, c0 + 64 * m, cw, lane);
+            else epilogue_block<false>(acc[m], neg[m], p, at, bias, out, c0 + 64 * m, cw, lane);
         }
     }
 }
@@ -882,7 +825,13 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
     }
     B3D_REQUIRE(!stats || mask || (osy == 1 && osx == 1), B3D_EINVAL, "b3d_conv2d_tf32: statistics need a dense output");
     // 256-wide output-channel tiles halve the input-tile bytes per FLOP through the L2 -> SM path when there are >= 256
-    // output channels and enough work items to give every SM one
+    // output channels and enough work items to give every SM one.  Every launch of cfg3, cfg4 and cfg5 this rule gives
+    // 256-wide tiles, timed against the same kernels forced to 128 (tools/time_conv128.py, H100 SXM, 700 W): 256 wins on
+    // all such forwards (d1.conv4 at batch 64 0.92 vs 1.14 ms, d1.conv3 0.97 vs 1.00 ms, the cfg4 encoder's conv3e /
+    // conv4e 0.14 / 0.12 vs 0.14 / 0.14 ms, blk4_tex.conv1 at batch 50 0.37 vs 0.43 ms) and on the 1x1 input gradients
+    // (G.blk4.short 0.06 vs 0.07 ms); 128 wins on most 3x3 and stride-2 input gradients (G.blk3a 0.10 vs 0.12 ms,
+    // d1.conv4 masked at batch 64 0.91 vs 0.95 ms).  Summed over those launches and cfg3's others 256 is ahead (17.5 vs
+    // 18.0 ms), so the rule stays as it is.
     const bool bn256 = Cout % 256 == 0 && (long long)N * Hout * Wout / BM * (Cout / 256) * ncls >= tc::num_sms();
     const int BN = bn256 ? 256 : Cout > 64 ? 128 : 64;
     cudaStream_t st = (cudaStream_t)stream;
@@ -981,7 +930,7 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
             const uint32_t es[4] = {1, (uint32_t)sx, (uint32_t)sy, 1};
             if (int rc = tc::make_tmap_f32(&mx, x, 4, dims, strides, box, es)) return rc;
         }
-        // ring depth: as many stages as fit next to the statistics / barrier area (~192 KB of operands)
+        // ring depth: as many stages as fit next to the barrier area (~192 KB of operands)
         if (BN == 256) return launch_conv<256, 4>(mx, mw, mm, p, bias, out, tiles, st);
         if (BN == 128) return launch_conv<128, 6>(mx, mw, mm, p, bias, out, tiles, st);
         return launch_conv<64, 8>(mx, mw, mm, p, bias, out, tiles, st);

@@ -5,7 +5,7 @@ conv_wgmma_rowwin<64,KW,S> instances), at cfg3's geometries: batch 32 for the ge
 
 --ref-lib loads a second build of libb3d (for instance the previous commit's) and times its b3d_conv2d_tf32 on the same
 operands, alternating with this tree's library launch window by launch window.  Each entry is the median over --reps
-windows of --n launches, CUDA events around each window."""
+windows of --n launches, CUDA events around each window, and its spread (slowest - fastest window)."""
 import argparse
 import ctypes
 import json
@@ -20,7 +20,7 @@ import torch  # noqa: E402
 import b3d  # noqa: E402
 import b3d.conv as C  # noqa: E402
 from b3d.ew import fold_rows  # noqa: E402
-from tools.time_wgrad import card, timed  # noqa: E402
+from tools.time_wgrad import card, windows  # noqa: E402
 
 B = 32
 
@@ -87,11 +87,13 @@ def main():
 
     tot = {n: 0.0 for n, _ in libs}
     for name, (flop, fn) in cases("cuda:0").items():
-        ms = timed([on(lib, fn) for _, lib in libs], a.reps, a.n)
+        ts = windows([on(lib, fn) for _, lib in libs], a.reps, a.n)
         C.lib = b3d.lib
         row = {"launch": name, "gflop": round(flop / 1e9, 1)}
-        for (ln, _), m in zip(libs, ms):
+        for (ln, _), t in zip(libs, ts):
+            m = sorted(t)[len(t) // 2]
             row[f"ms_{ln}"] = round(m, 4)
+            row[f"spread_{ln}"] = round(max(t) - min(t), 4)
             row[f"tflops_{ln}"] = round(flop / m / 1e9, 1)
             tot[ln] += m
         print(json.dumps(row), flush=True)

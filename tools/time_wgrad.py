@@ -54,8 +54,8 @@ def window(fn, n):
     return e0.elapsed_time(e1) / n
 
 
-def timed(fns, reps, n):
-    """Median ms per call of each fn, the fns alternated window by window."""
+def windows(fns, reps, n):
+    """ms per call of each fn in each of reps windows of n calls, the fns alternated window by window."""
     for f in fns:
         f()
     torch.cuda.synchronize()
@@ -63,7 +63,12 @@ def timed(fns, reps, n):
     for _ in range(reps):
         for i, f in enumerate(fns):
             ts[i].append(window(f, n))
-    return [sorted(t)[len(t) // 2] for t in ts]
+    return ts
+
+
+def timed(fns, reps, n):
+    """Median ms per call of each fn, the fns alternated window by window."""
+    return [sorted(t)[len(t) // 2] for t in windows(fns, reps, n)]
 
 
 def wgrad_call(lib, dy, x, dw, N, H, W, Cin, Hout, Wout, Cout, kh, kw, pad_y, st, tap_major=1, fold_kh=0):

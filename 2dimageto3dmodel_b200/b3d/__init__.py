@@ -118,6 +118,7 @@ _sig("b3d_gather_fields", _vp, _i, _vp, _vp, _i, _vp)
 _sig("b3d_image_batch", _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp)
 _sig("b3d_texel_visibility", _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp)
 _sig("b3d_pseudogt_pack", _vp, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp)
+_sig("b3d_sample_pack", _vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp)
 
 
 def mode_id(mode):

@@ -3,7 +3,8 @@ b3d_gather_fields: one launch that assembles a GAN batch from packed per-record 
 mirroring).  The stores may sit in device memory or in pinned host memory (read over PCIe).
 b3d_image_batch: one launch that builds a reconstruction batch (crop, cv2-style resize, mirror, poses) from packed photo
 windows in device memory.
-b3d_pseudogt_pack: one launch that masks, transposes and rounds a batch of pseudo-ground-truth records to fp16."""
+b3d_pseudogt_pack: one launch that masks, transposes and rounds a batch of pseudo-ground-truth records to fp16.
+b3d_sample_pack: one launch that turns a batch of sample renders and textures into the bytes of their PNGs."""
 import ctypes
 
 import torch
@@ -140,3 +141,34 @@ def pseudogt_pack(vis, tex, alpha, image, tex_out, alpha_out, image_out):
             raise B3DError(f"pseudogt_pack: {name} has shape {tuple(t.shape)}; expected {list(shape)}")
     check(lib.b3d_pseudogt_pack(ptr(vis), Th, Tw, ptr(tex), ptr(alpha), B, R, C, ptr(image), Ci, h, w, ptr(tex_out),
                                 ptr(alpha_out), ptr(image_out), stream_ptr(vis)))
+
+
+def sample_pack(image, imidx, tex, tiles_out, tex8_out):
+    """b3d_sample_pack: one launch turns a batch of renders and textures into the bytes of the exported PNGs.
+    image fp32 [B,H,W,3] (the Renderer output), imidx int32 [B,H,W] (its face-index buffer, 0 = background), tex fp32
+    [B,3,T,T] -> tiles_out uint8 [B,H/2,W/2,3] (background 1.0, / 2 + 0.5, 2 x 2 average pool, * 255, clamp, truncate),
+    tex8_out uint8 [B,T,T,3] (/ 2 + 0.5, * 255, clamp, truncate), rounded as the torch ops round.  H and W even; all
+    tensors contiguous on the device.  Shapes are checked before the device, so a malformed call fails the same way on
+    any machine."""
+    def need(t, dtype, name, dim):
+        if not (isinstance(t, torch.Tensor) and t.dtype == dtype and t.dim() == dim and t.is_contiguous()):
+            raise B3DError(f"sample_pack: {name} must be a contiguous {dtype} tensor with {dim} dimensions")
+    need(image, torch.float32, 'image', 4)
+    need(imidx, torch.int32, 'imidx', 3)
+    need(tex, torch.float32, 'tex', 4)
+    need(tiles_out, torch.uint8, 'tiles_out', 4)
+    need(tex8_out, torch.uint8, 'tex8_out', 4)
+    B, H, W = imidx.shape
+    T = tex.shape[2]
+    if H % 2 or W % 2:
+        raise B3DError(f"sample_pack: the render is {H} x {W}; the 2 x 2 pool needs an even height and width")
+    for name, t, shape in (('image', image, (B, H, W, 3)), ('tex', tex, (B, 3, T, T)),
+                           ('tiles_out', tiles_out, (B, H // 2, W // 2, 3)), ('tex8_out', tex8_out, (B, T, T, 3))):
+        if tuple(t.shape) != shape:
+            raise B3DError(f"sample_pack: {name} has shape {tuple(t.shape)}; expected {list(shape)}")
+    for name, t in (('image', image), ('imidx', imidx), ('tex', tex), ('tiles_out', tiles_out), ('tex8_out', tex8_out)):
+        if not t.is_cuda:
+            raise B3DError(f"sample_pack: {name} is on {t.device}; libb3d runs on CUDA tensors only, there is no CPU "
+                           "fallback")
+    check(lib.b3d_sample_pack(ptr(image), ptr(imidx), B, H, W, ptr(tex), T, ptr(tiles_out), ptr(tex8_out),
+                              stream_ptr(image)))

@@ -341,6 +341,60 @@ __global__ void __launch_bounds__(PACK_NT) pseudogt_pack_kernel(const __grid_con
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Sample export (main.py:874-895): the 2x2 anti-aliased render tiles and the texture images as the bytes written to PNG.
+
+struct SamplePackArgs {
+    const float* image;      // [B, H, W, 3]
+    const int32_t* imidx;    // [B, H, W] face index + 1, 0 = background
+    int H, W;
+    const float* tex;        // [B, 3, T, T]
+    int T;
+    long long tile_total, texel_total;
+    int tile_blocks;
+    uint8_t* tiles;          // [B, H/2, W/2, 3]
+    uint8_t* tex8;           // [B, T, T, 3]
+};
+
+// x / 2 + 0.5 as two roundings (halving is exact, so x * 0.5 rounds as x / 2 does)
+__device__ __forceinline__ float to_unit(float x) { return __fadd_rn(__fmul_rn(x, 0.5f), 0.5f); }
+
+// (v * 255).clamp(0, 255).byte(): one rounding, then truncation toward zero
+__device__ __forceinline__ uint8_t to_byte(float v) {
+    v = __fmul_rn(v, 255.f);
+    v = v < 0.f ? 0.f : (v > 255.f ? 255.f : v);
+    return (uint8_t)__float2uint_rz(v);
+}
+
+__global__ void __launch_bounds__(PACK_NT) sample_pack_kernel(const __grid_constant__ SamplePackArgs a) {
+    if ((int)blockIdx.x < a.tile_blocks) {
+        const long long t = (long long)blockIdx.x * PACK_NT + threadIdx.x;
+        if (t >= a.tile_total) return;
+        const int Wo = a.W >> 1, Ho = a.H >> 1;
+        const long long b = t / ((long long)Ho * Wo);
+        const int pos = (int)(t - b * Ho * Wo), yo = pos / Wo, xo = pos - yo * Wo;
+        const long long p00 = (b * a.H + 2 * yo) * a.W + 2 * xo;
+        const long long p[4] = {p00, p00 + 1, p00 + a.W, p00 + a.W + 1};     // avg_pool2d's window, row by row
+        bool bg[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) bg[k] = a.imidx[p[k]] <= 0;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            float s = 0.f;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) s = __fadd_rn(s, to_unit(bg[k] ? 1.f : a.image[p[k] * 3 + c]));
+            a.tiles[t * 3 + c] = to_byte(__fmul_rn(s, 0.25f));
+        }
+    } else {
+        const long long t = (long long)(blockIdx.x - a.tile_blocks) * PACK_NT + threadIdx.x;
+        if (t >= a.texel_total) return;
+        const long long plane = (long long)a.T * a.T;
+        const long long b = t / plane, pos = t - b * plane;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) a.tex8[t * 3 + c] = to_byte(to_unit(a.tex[(b * 3 + c) * plane + pos]));
+    }
+}
+
 int check_device_ptr(const void* p, const char* what, const char* fn = "b3d_image_batch") {
     cudaPointerAttributes at;
     B3D_CUDA_OK(cudaPointerGetAttributes(&at, p));
@@ -469,6 +523,33 @@ int b3d_pseudogt_pack(const uint8_t* vis, int Th, int Tw, const float* tex, cons
         if (rc != B3D_OK) return rc;
     }
     pseudogt_pack_kernel<<<(unsigned)blocks, PACK_NT, 0, (cudaStream_t)stream>>>(a);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+int b3d_sample_pack(const float* image, const int32_t* imidx, int B, int H, int W, const float* tex, int T,
+                    uint8_t* tiles, uint8_t* tex8, void* stream) {
+    B3D_REQUIRE(B >= 0 && H >= 2 && W >= 2 && T >= 1, B3D_EINVAL,
+                "b3d_sample_pack: bad sizes (B %d, render %d x %d, texture %d)", B, H, W, T);
+    B3D_REQUIRE(H % 2 == 0 && W % 2 == 0, B3D_EINVAL,
+                "b3d_sample_pack: the render is %d x %d; the 2 x 2 pool needs an even height and width", H, W);
+    if (B == 0) return B3D_OK;
+    SamplePackArgs a = {};
+    a.image = image, a.imidx = imidx, a.H = H, a.W = W, a.tex = tex, a.T = T, a.tiles = tiles, a.tex8 = tex8;
+    a.tile_total = (long long)B * (H / 2) * (W / 2);
+    a.texel_total = (long long)B * T * T;
+    const long long tile_blocks = (a.tile_total + PACK_NT - 1) / PACK_NT;
+    const long long blocks = tile_blocks + (a.texel_total + PACK_NT - 1) / PACK_NT;
+    B3D_REQUIRE(blocks < (1LL << 31), B3D_EINVAL, "b3d_sample_pack: batch too large");
+    a.tile_blocks = (int)tile_blocks;
+    const void* ptrs[] = {image, imidx, tex, tiles, tex8};
+    const char* names[] = {"image", "imidx", "tex", "tiles", "tex8"};
+    for (int i = 0; i < 5; ++i) {
+        B3D_REQUIRE(ptrs[i], B3D_EINVAL, "b3d_sample_pack: null %s", names[i]);
+        const int rc = check_device_ptr(ptrs[i], names[i], "b3d_sample_pack");
+        if (rc != B3D_OK) return rc;
+    }
+    sample_pack_kernel<<<(unsigned)blocks, PACK_NT, 0, (cudaStream_t)stream>>>(a);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }

@@ -21,7 +21,6 @@ reference's main.py:170-174); the Inception weights come from a local file (util
 computed from the render's index buffers instead of the full adjoint of the render.
 """
 import os
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
@@ -33,6 +32,7 @@ from b3d.mesh import render_indices, texel_visibility
 from data.pseudo_gt import pseudo_gt_dir, save_poses_metadata, save_pseudo_gt
 from fid_evaluation import save_real_statistics
 from rendering.inverse_renderer import InverseRenderer
+from staging import Staging, byte_layout, views
 from utils.fid import FIDStatistics, forward_inception_features, init_inception
 
 INCEPTION_RES = 299
@@ -60,19 +60,12 @@ def imagenet_rows(paths):
 def _layout(B, C, R, img_shape, mesh_shape):
     """Byte offsets of one batch's fields in the staging buffer: fp16 texture / alpha / image, fp32 mesh map and pose rows
     (scale, tx, ty, tz, qw, qx, qy, qz), int64 indices; every field 16-byte aligned."""
-    fields = (('texture', torch.float16, (B, C, R, R)), ('texture_alpha', torch.float16, (B, 1, R, R)),
-              ('image', torch.float16, (B,) + tuple(img_shape)), ('mesh', torch.float32, (B,) + tuple(mesh_shape)),
-              ('pose', torch.float32, (B, 8)), ('ind', torch.int64, (B,)))
-    out, off = {}, 0
-    for name, dt, shape in fields:
-        out[name] = (off, dt, shape)
-        off += (int(np.prod(shape)) * torch.empty(0, dtype=dt).element_size() + 15) // 16 * 16
-    return out, off
+    return byte_layout((('texture', torch.float16, (B, C, R, R)), ('texture_alpha', torch.float16, (B, 1, R, R)),
+                        ('image', torch.float16, (B,) + tuple(img_shape)), ('mesh', torch.float32, (B,) + tuple(mesh_shape)),
+                        ('pose', torch.float32, (B, 8)), ('ind', torch.int64, (B,))))
 
 
-def _views(buf, layout):
-    return {k: buf[o:o + int(np.prod(s)) * torch.empty(0, dtype=dt).element_size()].view(dt).view(s)
-            for k, (o, dt, s) in layout.items()}
+_views = views
 
 
 def staged_records(views):
@@ -127,7 +120,8 @@ class PseudoGTExporter:
 
     def _reset(self):
         """Forget the buffers and statistics of a previous export (each export allocates its own once)."""
-        self._bufs = self._vis = self._words = self._stats = self._staging = self._slots = None
+        self._bufs = self._vis = self._words = self._stats = None
+        self._staging = Staging(self.device, 'export')
 
     def _buffers(self, B):
         """Render / visibility buffers for batches of up to B samples, allocated once per export."""
@@ -141,8 +135,8 @@ class PseudoGTExporter:
 
     @torch.no_grad()
     def _device_batch(self, batch, keep):
-        """GPU work of one batch: fills the device staging buffer (allocated with the two pinned slots at the first batch,
-        the largest) and returns the batch's byte layout and size."""
+        """GPU work of one batch: fills the device staging buffer (allocated at the first batch, the largest) and returns
+        the batch's byte layout and size."""
         X, img299, hd, scale, translation, rot, ind = (t.to(self.device) for t in batch)
         ind = ind.reshape(-1)
         B = X.shape[0]
@@ -169,13 +163,7 @@ class PseudoGTExporter:
 
         inv_tex, inv_alpha = self.inverse_renderer(vtx, hd)
         lay, nbytes = _layout(B, inv_tex.shape[3], self.R, img299.shape[1:], mesh_map.shape[1:])
-        if self._staging is None:
-            self._staging = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            self._slots = [torch.empty(nbytes, dtype=torch.uint8, pin_memory=True) for _ in range(2)]
-        if nbytes > self._staging.numel():
-            raise b3d.B3DError(f'export: a batch of {B} needs {nbytes} staging bytes, {self._staging.numel()} were '
-                               'allocated for the first batch; only the last batch may be smaller')
-        v = _views(self._staging, lay)
+        v = _views(self._staging.device_buffer(nbytes, B), lay)
         pseudogt_pack(vis, inv_tex.contiguous(), inv_alpha.contiguous(), img299.contiguous(), v['texture'],
                       v['texture_alpha'], v['image'])
         v['mesh'].copy_(mesh_map)
@@ -203,38 +191,19 @@ class PseudoGTExporter:
             keep = torch.zeros(len(paths), device=self.device)
             keep[imagenet_rows(paths)] = 1
         self._reset()
-        events = [None, None]
-        poses, pending, futures = {}, None, []
-        stream = torch.cuda.current_stream(self.device)
+        poses = {}
 
-        def drain(p):
-            """Host side of one staged batch: wait for its copy, clone every sample out of the pinned slot, queue the writes."""
-            slot, lay, nbytes = p
-            events[slot].synchronize()
-            for idx, rec, pose in staged_records(_views(self._slots[slot], lay)):
+        def device_batch(batch):
+            lay, nbytes = self._device_batch(batch, keep)
+            return lay, nbytes, lay['ind'][2][0]
+
+        def drain(host, lay, submit):
+            """Host side of one staged batch: clone every sample out of the pinned slot, queue the writes."""
+            for idx, rec, pose in staged_records(_views(host, lay)):
                 poses[idx] = pose
-                futures.append(pool.submit(save_pseudo_gt, out_dir, idx, rec))
+                submit(save_pseudo_gt, out_dir, idx, rec)
 
-        with ThreadPoolExecutor(max_workers=max(1, int(writers))) as pool:
-            try:
-                for n, batch in enumerate(batches):
-                    # slot n % 2 last held batch n - 2, whose samples drain() cloned out during iteration n - 1
-                    slot = n % 2
-                    lay, nbytes = self._device_batch(batch, keep)
-                    self._slots[slot][:nbytes].copy_(self._staging[:nbytes], non_blocking=True)
-                    events[slot] = torch.cuda.Event()
-                    events[slot].record(stream)
-                    if pending is not None:
-                        drain(pending)
-                    pending = (slot, lay, nbytes)
-                    self._throttle(futures, max(4 * int(writers), 2 * lay['ind'][2][0]))
-                if pending is not None:
-                    drain(pending)
-                for f in futures:
-                    f.result()                  # a failed write raises here
-            finally:
-                for f in futures:
-                    f.cancel()
+        self._staging.run(batches, device_batch, drain, writers)
         if not poses:
             raise ValueError('export: no batches')
 
@@ -254,12 +223,6 @@ class PseudoGTExporter:
             out['num_images_testval'] = vstats.n
             out['fid_testval'] = self._save_stats(vstats, cache_dir, 'testval')
         return out
-
-    @staticmethod
-    def _throttle(futures, limit):
-        """Keep at most `limit` records queued: each holds its planes in host memory until it is written."""
-        while sum(1 for f in futures if not f.done()) > limit:
-            next(f for f in futures if not f.done()).result()
 
     @staticmethod
     def _save_stats(stats, cache_dir, split):

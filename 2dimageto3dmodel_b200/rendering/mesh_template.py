@@ -12,6 +12,7 @@ import os
 import numpy as np
 import torch
 import torch.nn.functional as F
+from PIL import Image
 
 from .utils import circpad, grid_sample_bilinear
 
@@ -238,22 +239,29 @@ class MeshTemplate:
         return image, alpha
 
     def export_obj(self, path_prefix, vertex_positions, texture):
-        """Write <prefix>.obj/.mtl (+ .png when imageio is installed) — reference :188-219."""
+        """Write <prefix>.obj / .mtl / .png — reference :188-219.  vertex_positions [V,3]; texture [3,T,T] in [0, 1]."""
         if vertex_positions.dim() != 2:
             raise ValueError("export_obj takes one mesh: vertex_positions [V,3]")
+        tex8 = (texture.permute(1, 2, 0) * 255).clamp(0, 255).byte().cpu().numpy()
+        ObjWriter(self.mesh).write(path_prefix, vertex_positions.detach().cpu().numpy(), tex8)
+
+
+class ObjWriter:
+    """The files of one textured mesh as the reference's export_obj writes them (:188-219): <prefix>.obj, <prefix>.mtl
+    naming <prefix>.png, and that PNG.  The vt and f lines depend only on the template, so they are formatted once."""
+
+    def __init__(self, mesh):
+        self.vt = ''.join('vt {:.5f} {:.5f}\n'.format(*t) for t in mesh.uvs.tolist())
+        self.f = ''.join('f ' + ' '.join(f'{a + 1}/{b + 1}' for a, b in zip(f, t)) + '\n'
+                         for f, t in zip(mesh.faces.tolist(), mesh.face_textures.tolist()))
+
+    def write(self, path_prefix, vertices, texture):
+        """vertices: float32 [V,3] (numpy); texture: uint8 [T,T,3], the PNG's pixels."""
         name = os.path.basename(path_prefix)
+        v = ''.join('v {:.5f} {:.5f} {:.5f}\n'.format(*p) for p in vertices.tolist())
         with open(path_prefix + '.obj', 'w') as fh:
-            fh.write(f'mtllib {name}.mtl\n')
-            fh.writelines('v {:.5f} {:.5f} {:.5f}\n'.format(*v) for v in vertex_positions.tolist())
-            fh.writelines('vt {:.5f} {:.5f}\n'.format(*t) for t in self.mesh.uvs.tolist())
-            fh.write(f'usemtl {name}\n')
-            for f, t in zip(self.mesh.faces.tolist(), self.mesh.face_textures.tolist()):
-                fh.write('f ' + ' '.join(f'{a + 1}/{b + 1}' for a, b in zip(f, t)) + '\n')
+            fh.write(f'mtllib {name}.mtl\n{v}{self.vt}usemtl {name}\n{self.f}')
         with open(path_prefix + '.mtl', 'w') as fh:
             fh.write(f'newmtl {name}\nKa 1.000 1.000 1.000\nKd 1.000 1.000 1.000\nKs 0.000 0.000 0.000\n'
                      f'd 1.0\nillum 1\nmap_Ka {name}.png\nmap_Kd {name}.png\n')
-        try:
-            import imageio
-        except ImportError:
-            return
-        imageio.imwrite(path_prefix + '.png', (texture.permute(1, 2, 0) * 255).clamp(0, 255).byte().cpu().numpy())
+        Image.fromarray(texture).save(path_prefix + '.png')

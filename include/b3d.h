@@ -519,6 +519,20 @@ B3D_API int b3d_pseudogt_pack(const uint8_t* vis, int Th, int Tw, const float* t
                               const float* image, int Ci, int h, int w, uint16_t* tex_out, uint16_t* alpha_out,
                               uint16_t* image_out, void* stream);
 
+/* ---- Sample export (reference: main.py:874-895, rendering/mesh_template.py:216-219) ---------------------------------
+ *   image_pred[alpha_pred.expand_as(image_pred) == 0] = 1          (alpha: the hard mask, imidx > 0)
+ *   image_pred = F.avg_pool2d(image_pred.permute(0, 3, 1, 2) / 2 + 0.5, 2)
+ *   grid = (make_grid(image_pred).permute(1, 2, 0) * 255).clamp(0, 255).byte()
+ *   png = ((pred_tex[i] / 2 + 0.5).permute(1, 2, 0) * 255).clamp(0, 255).byte()
+ * b3d_sample_pack  image [B,H,W,3] fp32 (the render), imidx [B,H,W] int32 (face index + 1, 0 = background), tex [B,3,T,T]
+ *                  fp32 -> tiles [B,H/2,W/2,3] and tex8 [B,T,T,3] uint8.  A pixel with imidx <= 0 takes the value 1.0 in
+ *                  every channel.  Every operation rounds once in fp32, as the torch ops do: x / 2 + 0.5 (two roundings),
+ *                  the pool sum ((((0 + a) + b) + c) + d) over the window row by row, then / 4 (exact), then * 255, a clamp
+ *                  to [0, 255] and truncation toward zero; no fused multiply-add.  H and W must be even and every pointer
+ *                  device memory (B3D_EINVAL otherwise).                                                              */
+B3D_API int b3d_sample_pack(const float* image, const int32_t* imidx, int B, int H, int W, const float* tex, int T,
+                            uint8_t* tiles, uint8_t* tex8, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -80,7 +80,7 @@ def reference_construction(exp, batch):
 
 def exporter_batch(exp, batch, slot):
     lay, nbytes = exp._device_batch(batch, None)
-    exp._slots[slot][:nbytes].copy_(exp._staging[:nbytes], non_blocking=True)
+    exp._staging.slots[slot][:nbytes].copy_(exp._staging.buffer[:nbytes], non_blocking=True)
 
 
 def time_batches(exp, B, reps):

@@ -32,6 +32,6 @@ void count_launch(int n) { g_launches.fetch_add((uint64_t)n, std::memory_order_r
 extern "C" {
 const char* b3d_last_error(void) { return b3d::g_err; }
 const char* b3d_last_variant(void) { return b3d::g_variant; }
-int b3d_version(void) { return 410; }   // 4.1: b3d_sample_pack (sample export)
+int b3d_version(void) { return 420; }   // 4.2: weight-gradient consumers keep a wgmma group in flight; shared-memory X transpose
 uint64_t b3d_launch_count(void) { return b3d::g_launches.load(std::memory_order_relaxed); }
 }

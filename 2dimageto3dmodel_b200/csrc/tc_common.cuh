@@ -1,6 +1,5 @@
 // sm_90a tensor-core plumbing shared by the implicit-GEMM conv kernels: mbarrier, TMA (cp.async.bulk.tensor) and
-// warpgroup MMA (wgmma.mma_async kind tf32) wrappers in inline PTX, wgmma shared-memory descriptors, the operand
-// transpose used where an operand arrives M/N-major (wgmma reads tf32 operands K-major only) and the host-side
+// warpgroup MMA (wgmma.mma_async kind tf32) wrappers in inline PTX, wgmma shared-memory descriptors and the host-side
 // tensor-map encoder (driver entry point resolved at run time through
 // cudaGetDriverEntryPoint: the library does not link libcuda).
 #pragma once
@@ -98,6 +97,19 @@ __device__ __forceinline__ float2 lds_f32x2(uint32_t smem_addr) {       // 8-byt
     asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(smem_addr) : "memory");
     return v;
 }
+__device__ __forceinline__ float4 lds_f32x4(uint32_t smem_addr) {     // 16-byte aligned
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(smem_addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void sts_f32x4(uint32_t smem_addr, float a, float b, float c, float d) {     // 16-byte aligned
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(smem_addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+// Operand fence: the register is read and written here as far as register allocation can tell.  A wgmma reads its
+// register operands (and writes its accumulators) after it issues; fencing them after the wgmma_wait that retires it keeps
+// them live, in place, until then.
+__device__ __forceinline__ void fence_operand(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
+__device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 // per-thread register budget of the executing warpgroup (warp-specialized kernels move registers from producer to consumers)
 template <int N>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
@@ -184,21 +196,6 @@ __device__ __forceinline__ uint64_t desc_k32(uint32_t smem_addr) {
     d |= (uint64_t)(256 >> 4) << 32;                    // stride byte offset: 8 rows x 32 B
     d |= (uint64_t)3 << 62;                             // layout type: SWIZZLE_32B
     return d;
-}
-
-// One 32-wide K slice of an operand that TMA delivered M/N-major (NHWC pixels along K: the weight gradient's X)
-// as `rows` / 32 boxes [k][32 mn] (no swizzle; boxes blk_stride floats apart), K rows k0 .. k0 + 31 rewritten K-major
-// into `dst` in the 128-byte-swizzled layout that desc_k128 reads: row mn, 16-byte chunk c at byte
-// mn * 128 + ((c ^ (mn % 8)) << 4).  Executed by the 128 threads of the producer warpgroup; consecutive threads take
-// consecutive rows (conflict-free reads and stores).
-__device__ __forceinline__ void transpose_slice_k128(const float* raw, unsigned char* dst, int rows, int tid, int blk_stride = 1024,
-                                                     int k0 = 0) {
-    for (int i = tid; i < rows * 8; i += 128) {
-        const int mn = i % rows, kc = i / rows;
-        const float* src = raw + (mn >> 5) * blk_stride + (k0 + kc * 4) * 32 + (mn & 31);
-        const float4 v = make_float4(src[0], src[32], src[64], src[96]);
-        *reinterpret_cast<float4*>(dst + mn * 128 + ((kc ^ (mn & 7)) << 4)) = v;
-    }
 }
 
 // ---------------------------------------------------------------------------------------------- host: tensor maps

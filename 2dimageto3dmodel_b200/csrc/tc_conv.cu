@@ -376,11 +376,11 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
 // [32 pixels][32 channels] boxes (four for dY, BN/32 for X, the X boxes shifted by the tap on the OUTER dims: zero fill =
 // padding, element strides for stride 2) into an NRAW-deep staging ring.  wgmma reads tf32 operands from shared memory
 // K-major only, so the producer warpgroup rewrites each X slice K-major into the swizzled stage the consumers read
-// (tc::transpose_slice_k128).  dY is the A operand, which wgmma also takes from registers: the consumers load their
+// (wgrad_transpose: 16-byte shared-memory loads and stores around a 4 x 4 register transpose).  dY is the A operand, which wgmma also takes from registers: the consumers load their
 // fragments straight from the staged dY tile (128-byte swizzled by TMA, conflict-free: dy_tile_offset) and hand the raw
 // slot back as soon as the loads are done.  No NCHW copy is ever made.  T > 1 (row of taps): a K slice is a 32-pixel row
-// segment, the X box is a window of 32 + T - 1 (rounded to 36) pixels, and the producer writes T K-major B tiles from it
-// — tap t is the window shifted by t pixels — which share the dY fragments: T accumulators per consumer warpgroup, T taps
+// segment, the X box is a window of 32 + T - 1 (rounded to 36) pixels, and the producer reads it once and writes T K-major
+// B tiles from it — tap t is the window shifted by t pixels — which share the dY fragments: T accumulators per consumer warpgroup, T taps
 // per byte of dY.  One CTA per (co tile, ci tile, tap group, K split); partial sums are reduced into dW with global atomics.
 // ----------------------------------------------------------------------------------------------
 struct WgradParams {
@@ -421,6 +421,102 @@ __host__ __device__ constexpr int dy_tile_offset(int co, int px) {
     return (co >> 5) * 4096 + px * 128 + ((((co >> 2) & 7) ^ (px & 7)) << 4) + (co & 3) * 4;
 }
 
+// The producer's transpose of a raw X slice (per 32-channel block: wrows pixels of 128 bytes, unswizzled) into the K-major,
+// 128-byte swizzled B tiles (row = channel, 16-byte chunk c = pixels 4c .. 4c + 3, stored at chunk c ^ (row % 8)).  Task i
+// (0 .. 2 BN) covers block i / 64, channels 4 (i % 8) .. + 3 and chunk xt_chunk(i) of every tap's tile: T + 3 16-byte loads
+// of consecutive window pixels (xt_src_offset), a 4 x 4 register transpose per tap, and 4 T 16-byte stores (xt_dst_offset).
+// The eight tasks of a quarter warp have i % 8 = 0 .. 7, so their loads hit eight different chunk positions of a 128-byte row,
+// and for each store their chunks xt_chunk(i) ^ (row % 8) are eight different values: both are conflict-free.
+__host__ __device__ constexpr int xt_chunk(int i) { return (((i & 7) >> 1) ^ ((i >> 4) & 3)) | (((i >> 3) & 1) << 2); }
+__host__ __device__ constexpr int xt_src_offset(int i, int px, int wrows) { return ((i >> 6) * wrows + px) * 128 + (i & 7) * 16; }
+__host__ __device__ constexpr int xt_dst_offset(int i, int j) {     // channel j (0..3) of task i
+    return ((i >> 6) * 32 + 4 * (i & 7) + j) * 128 + ((xt_chunk(i) ^ ((4 * (i & 7) + j) & 7)) << 4);
+}
+template <int BN, int T, int WROWS>
+__device__ __forceinline__ void wgrad_transpose(uint32_t src, uint32_t dst, int tid) {
+    // A producer warp is alone on its SM sub-partition, so nothing hides its load latency: every load of the thread's
+    // tasks (tid, tid + 128) is issued before the first store, one wait per slice instead of one per task and tap.
+    constexpr int NT = 2 * BN / 128;
+    float4 v[NT][T + 3];                                      // task n: pixels 4q .. 4q + T + 2 of the window, channels 4 (i % 8) ..
+#pragma unroll
+    for (int n = 0; n < NT; ++n)
+#pragma unroll
+        for (int u = 0; u < T + 3; ++u) v[n][u] = tc::lds_f32x4(src + xt_src_offset(tid + 128 * n, 4 * xt_chunk(tid + 128 * n) + u, WROWS));
+#pragma unroll
+    for (int n = 0; n < NT; ++n) {
+        const int i = tid + 128 * n;
+#pragma unroll
+        for (int t = 0; t < T; ++t) {
+            const uint32_t d = dst + t * (BN * 128);
+            const float4* w = v[n] + t;
+            tc::sts_f32x4(d + xt_dst_offset(i, 0), w[0].x, w[1].x, w[2].x, w[3].x);
+            tc::sts_f32x4(d + xt_dst_offset(i, 1), w[0].y, w[1].y, w[2].y, w[3].y);
+            tc::sts_f32x4(d + xt_dst_offset(i, 2), w[0].z, w[1].z, w[2].z, w[3].z);
+            tc::sts_f32x4(d + xt_dst_offset(i, 3), w[0].w, w[1].w, w[2].w, w[3].w);
+        }
+    }
+}
+
+// The consumer loop of both weight-gradient kernels, for one warpgroup: K slices first, first + step, ... < KI, each the
+// dY fragments of its raw slot (aoff: dy_tile_offset of K step 0) against the T K-major B tiles (N channels each) of its
+// stage.  One wgmma group stays in flight: the next slice's fragments load into the other register set while a slice's
+// group runs, and the previous slice's stage is handed back once wgmma_wait<1> has retired its group.  The operand fences
+// keep the retiring set's registers from being reused before then.
+template <int N, int T, int STAGES, int NRAW, int RAW_BYTES, int STAGE_BYTES>
+__device__ __forceinline__ void wgrad_consume(float (&acc)[T][N / 2], uint32_t raw_s, uint32_t stage_s, uint64_t* full,
+                                              uint64_t* empty, uint64_t* rawfull, uint64_t* rawempty, const int (&aoff)[4],
+                                              int first, int step, int KI, int tid, bool zero_first) {
+    using Frag = uint32_t[BK / MMA_K][4];
+    auto load = [&](Frag& f, int j) {
+        const int rb = j % NRAW;
+        tc::mbar_wait(rawfull + rb, (j / NRAW) & 1);
+#pragma unroll
+        for (int k = 0; k < BK / MMA_K; ++k)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) f[k][e] = tc::lds_u32(raw_s + rb * RAW_BYTES + aoff[e] + k * 1024);
+        __syncwarp();
+        if ((tid & 31) == 0) tc::mbar_arrive(rawempty + rb);      // the loads are complete: TMA may refill the slot
+    };
+    auto slice = [&](int j, Frag& f, Frag& g) {              // f: slice j's fragments, g: the previous slice's
+        const int st = j % STAGES;
+        tc::mbar_wait(full + st, (j / STAGES) & 1);
+        const uint32_t b = stage_s + st * STAGE_BYTES;
+        tc::wgmma_fence();
+#pragma unroll
+        for (int t = 0; t < T; ++t)
+#pragma unroll
+            for (int k = 0; k < BK / MMA_K; ++k)
+                tc::Wgmma<N>::mma_rs(acc[t], f[k], tc::desc_k128(b + t * (N * 128) + k * MMA_K * 4), (zero_first && j == first && k == 0) ? 0u : 1u);
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();
+#pragma unroll
+        for (int k = 0; k < BK / MMA_K; ++k)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) tc::fence_operand(g[k][e]);
+        if (j != first && tid == 0) tc::mbar_arrive(empty + (j - step) % STAGES);
+        if (j + step < KI) load(g, j + step);
+    };
+    Frag f0, f1;
+    if (first < KI) load(f0, first);
+    for (int j = first; j < KI; j += 2 * step) {
+        slice(j, f0, f1);
+        if (j + step < KI) slice(j + step, f1, f0);
+    }
+    tc::wgmma_wait<0>();
+#pragma unroll
+    for (int k = 0; k < BK / MMA_K; ++k)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            tc::fence_operand(f0[k][e]);
+            tc::fence_operand(f1[k][e]);
+        }
+#pragma unroll
+    for (int t = 0; t < T; ++t)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) tc::fence_operand(acc[t][i]);
+    if (first < KI && tid == 0) tc::mbar_arrive(empty + (first + (KI - 1 - first) / step * step) % STAGES);
+}
+
 template <int BN, int STAGES, int NRAW, int T>
 __global__ void __launch_bounds__(NTHREADS, 1)
 wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x,
@@ -443,27 +539,30 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_con
     const long long ktotal = (long long)p.N * per_img;
     const long long k_lo = ktotal * split / p.splits, k_hi = ktotal * (split + 1) / p.splits;
     const int KI = (int)(k_hi - k_lo);
+    // consumer warpgroups with output channels below Cout: the second one's 64 are all past it when Cout <= co0 + 64 (the
+    // 64-channel layers of the generator), and it leaves at once instead of multiplying the zero-filled half of the dY tile
+    const int nact = co0 + 64 < p.Cout ? 2 : 1;
 
     if (threadIdx.x == 0) {
         tc::tma_prefetch_desc(&tmap_dy);
         tc::tma_prefetch_desc(&tmap_x);
         for (int i = 0; i < STAGES; ++i) {
             tc::mbar_init(full + i, 128);
-            tc::mbar_init(empty + i, 2);
+            tc::mbar_init(empty + i, nact);
         }
         for (int i = 0; i < NRAW; ++i) {
             tc::mbar_init(rawfull + i, 1);
-            tc::mbar_init(rawempty + i, 8);
+            tc::mbar_init(rawempty + i, 4 * nact);
         }
         tc::fence_barrier_init();
     }
     __syncthreads();
     const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
 
-    // registers move from the producer (transpose loops) to the consumers (T accumulators and the dY fragments);
-    // 128 * (168 - 56) == 256 * (224 - 168)
+    // registers move from the producer (the window transpose holds up to 2 (T + 3) float4) to the consumers (T accumulators
+    // and two sets of dY fragments); 128 * (168 - 80) >= 256 * (208 - 168)
     if (wg == 0) {
-        tc::setmaxnreg_dec<56>();
+        tc::setmaxnreg_dec<80>();
         auto issue = [&](int j) {
             if (tid != 0) return;
             const long long k = k_lo + j;
@@ -478,25 +577,23 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_con
             tc::tma_load_5d(dst + S::DY_BYTES, &tmap_x, rawfull + rb, 0, p.st * x0 + s + p.xoff, p.st * y0 + r - p.pad_y, n, ci0 / 32);
         };
         for (int j = 0; j < NRAW - 1 && j < KI; ++j) issue(j);
+        const uint32_t raw_s = tc::smem_u32(raw), base_s = tc::smem_u32(base);
         for (int it = 0; it < KI; ++it) {
             if (it + NRAW - 1 < KI) issue(it + NRAW - 1);     // its buffer was last read in iteration it - 1
             const int rb = it % NRAW, st = it % STAGES;
             tc::mbar_wait(rawfull + rb, (it / NRAW) & 1);
             tc::mbar_wait(empty + st, ((it / STAGES) & 1) ^ 1);
-            const float* src = reinterpret_cast<const float*>(raw + rb * S::RAW_BYTES + S::DY_BYTES);
-            unsigned char* dst = base + st * S::STAGE_BYTES;
-#pragma unroll
-            for (int t = 0; t < T; ++t)
-                tc::transpose_slice_k128(src, dst + t * (BN * 128), BN, tid, S::WROWS * 32, t);
+            wgrad_transpose<BN, T, S::WROWS>(raw_s + rb * S::RAW_BYTES + S::DY_BYTES, base_s + st * S::STAGE_BYTES, tid);
             tc::fence_proxy_async();
             tc::mbar_arrive(full + st);
             tc::named_sync(2, 128);                               // the raw X boxes are consumed before they are loaded again
         }
         return;
     }
-    tc::setmaxnreg_inc<224>();
+    tc::setmaxnreg_inc<208>();
 
     const int h = wg - 1, lane = tid & 31;
+    if (h >= nact) return;
     // this thread's fragment registers a[0..3] of K step 0 in the staged dY tile (K step k: + 1024 k)
     int aoff[4];
 #pragma unroll
@@ -507,33 +604,8 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_con
     for (int t = 0; t < T; ++t)
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[t][i] = 0.f;
-    // A wgmma reads its register operands after it issues, and register allocation does not see that: fragments
-    // double-buffered across slices may be given the same registers, and the compiler then waits for every wgmma before
-    // the next one issues.  So one set of fragments, reloaded once the slice's wgmma group has retired; the other consumer
-    // warpgroup's group keeps the tensor cores busy meanwhile.
-    const uint32_t raw_s = tc::smem_u32(raw);
-    for (int it = 0; it < KI; ++it) {
-        const int st = it % STAGES, rb = it % NRAW;
-        tc::mbar_wait(rawfull + rb, (it / NRAW) & 1);
-        uint32_t frag[BK / MMA_K][4];
-#pragma unroll
-        for (int k = 0; k < BK / MMA_K; ++k)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) frag[k][e] = tc::lds_u32(raw_s + rb * S::RAW_BYTES + aoff[e] + k * 1024);
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(rawempty + rb);      // the loads are complete: TMA may refill the slot
-        tc::mbar_wait(full + st, (it / STAGES) & 1);
-        const uint32_t b = tc::smem_u32(base + st * S::STAGE_BYTES);
-        tc::wgmma_fence();
-#pragma unroll
-        for (int t = 0; t < T; ++t)
-#pragma unroll
-            for (int k = 0; k < BK / MMA_K; ++k)
-                tc::Wgmma<BN>::mma_rs(acc[t], frag[k], tc::desc_k128(b + t * (BN * 128) + k * MMA_K * 4), (it | k) ? 1u : 0u);
-        tc::wgmma_commit();
-        tc::wgmma_wait<0>();
-        if (tid == 0) tc::mbar_arrive(empty + st);
-    }
+    wgrad_consume<BN, T, STAGES, NRAW, S::RAW_BYTES, S::STAGE_BYTES>(acc, tc::smem_u32(raw), tc::smem_u32(base), full, empty, rawfull,
+                                                                     rawempty, aoff, 0, 1, KI, tid, true);
     if (KI == 0) return;
     const int m_a = (tid >> 5) * 16 + (lane >> 2);                // this thread's accumulator rows m_a, m_a + 8
     const int cq = ci0 + 2 * (lane & 3);
@@ -582,6 +654,7 @@ int launch_wgrad(const CUtensorMap& mdy, const CUtensorMap& mx, const WgradParam
 // with five 64 x 64 accumulators over the whole 64-channel tile; both are reduced into dW by fp32 atomics.
 // ----------------------------------------------------------------------------------------------
 constexpr int STEM_KW = 5, STEM_STAGES = 4, STEM_NRAW = 3;
+constexpr int STEM_BATCH = 3;                                         // producer expansion tasks whose loads are in flight together
 struct StemSmem {
     static constexpr int DY_BYTES = 64 * BK * 4;
     static constexpr int WPX = BK + STEM_KW - 1;                       // raw pixels per K slice: 32 + 4
@@ -649,22 +722,37 @@ wgrad_stem_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_cons
         }
         for (int j = 0; j < STEM_NRAW - 1 && j < KI; ++j) issue(j);
         const int ntask = fold_kh * 8 * STEM_KW * 8;
+        const uint32_t raw_s = tc::smem_u32(raw), base_s = tc::smem_u32(base);
         for (int it = 0; it < KI; ++it) {
             if (it + STEM_NRAW - 1 < KI) issue(it + STEM_NRAW - 1);
             const int rb = it % STEM_NRAW, st = it % STEM_STAGES;
             tc::mbar_wait(rawfull + rb, (it / STEM_NRAW) & 1);
             tc::mbar_wait(empty + st, ((it / STEM_STAGES) & 1) ^ 1);
-            const float* src = reinterpret_cast<const float*>(raw + rb * S::RAW_BYTES + S::DY_BYTES);    // [row][36 px][8 ch]
-            unsigned char* dst = base + st * S::STAGE_BYTES;
+            const uint32_t src = raw_s + rb * S::RAW_BYTES + S::DY_BYTES;       // [row][36 px][8 ch]
+            const uint32_t dst = base_s + st * S::STAGE_BYTES;
             // task (r, q, s, ci), ci fastest: 16-byte chunk q (pixels 4q .. 4q + 3) of row c = 8r + ci of tap s's tile.  Eight
             // lanes of a store phase write chunks q ^ ci of eight rows (conflict-free); the reads of a warp's four (s, q)
-            // groups start on pixels 4q + s, mostly different banks mod 4 pixels.
-            for (int i = tid; i < ntask; i += 128) {
-                const int ci = i & 7, u = i >> 3;
-                const int s = u % STEM_KW, q = (u / STEM_KW) & 7, r = u / (STEM_KW * 8);
-                const float* a = src + (r * S::WPX + 4 * q + s) * 8 + ci;
-                const int c = 8 * r + ci;
-                *reinterpret_cast<float4*>(dst + s * S::TILE_BYTES + c * 128 + ((q ^ ci) << 4)) = make_float4(a[0], a[8], a[16], a[24]);
+            // groups start on pixels 4q + s, mostly different banks mod 4 pixels.  Shared-memory loads of STEM_BATCH tasks are
+            // issued before their stores (the producer warp alone on its sub-partition would otherwise wait out each load).
+            for (int i0 = tid; i0 < ntask; i0 += STEM_BATCH * 128) {
+                float v[STEM_BATCH][4];
+                uint32_t d[STEM_BATCH];
+#pragma unroll
+                for (int g = 0; g < STEM_BATCH; ++g) {
+                    const int i = i0 + 128 * g;
+                    if (i >= ntask) break;
+                    const int ci = i & 7, u = i >> 3;
+                    const int s = u % STEM_KW, q = (u / STEM_KW) & 7, r = u / (STEM_KW * 8);
+                    const uint32_t a = src + ((r * S::WPX + 4 * q + s) * 8 + ci) * 4;
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) v[g][e] = tc::lds_f32(a + 32 * e);
+                    d[g] = dst + s * S::TILE_BYTES + (8 * r + ci) * 128 + ((q ^ ci) << 4);
+                }
+#pragma unroll
+                for (int g = 0; g < STEM_BATCH; ++g) {
+                    if (i0 + 128 * g >= ntask) break;
+                    tc::sts_f32x4(d[g], v[g][0], v[g][1], v[g][2], v[g][3]);
+                }
             }
             tc::fence_proxy_async();
             tc::mbar_arrive(full + st);
@@ -684,29 +772,9 @@ wgrad_stem_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_cons
     for (int t = 0; t < STEM_KW; ++t)
 #pragma unroll
         for (int i = 0; i < 32; ++i) acc[t][i] = 0.f;
-    const uint32_t raw_s = tc::smem_u32(raw);
-    for (int it = h; it < KI; it += 2) {
-        const int st = it % STEM_STAGES, rb = it % STEM_NRAW;
-        tc::mbar_wait(rawfull + rb, (it / STEM_NRAW) & 1);
-        uint32_t frag[BK / MMA_K][4];
-#pragma unroll
-        for (int k = 0; k < BK / MMA_K; ++k)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) frag[k][e] = tc::lds_u32(raw_s + rb * S::RAW_BYTES + aoff[e] + k * 1024);
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(rawempty + rb);
-        tc::mbar_wait(full + st, (it / STEM_STAGES) & 1);
-        const uint32_t b = tc::smem_u32(base + st * S::STAGE_BYTES);
-        tc::wgmma_fence();
-#pragma unroll
-        for (int t = 0; t < STEM_KW; ++t)
-#pragma unroll
-            for (int k = 0; k < BK / MMA_K; ++k)
-                tc::Wgmma<64>::mma_rs(acc[t], frag[k], tc::desc_k128(b + t * S::TILE_BYTES + k * MMA_K * 4), 1u);
-        tc::wgmma_commit();
-        tc::wgmma_wait<0>();
-        if (tid == 0) tc::mbar_arrive(empty + st);
-    }
+    static_assert(S::TILE_BYTES == 64 * 128, "a tap's B tile is 64 channel rows of 128 bytes");
+    wgrad_consume<64, STEM_KW, STEM_STAGES, STEM_NRAW, S::RAW_BYTES, S::STAGE_BYTES>(acc, tc::smem_u32(raw), tc::smem_u32(base), full, empty,
+                                                                                     rawfull, rawempty, aoff, h, 2, KI, tid, false);
     if (h >= KI) return;
     const int m_a = (tid >> 5) * 16 + (lane >> 2);
 #pragma unroll

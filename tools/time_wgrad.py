@@ -2,11 +2,14 @@
 discriminator stem (5x5, 8 -> 64 channels at 256^2) both ways: materialised fold + generic kernel, and the raw-input kernel;
 its forward both ways too.
 
-    python tools/time_wgrad.py [--ref-lib OTHER/libb3d.so] [--reps 7] [--n 20]
+    python tools/time_wgrad.py [--ref-lib OTHER/libb3d.so ...] [--reps 7] [--n 20]
 
---ref-lib loads a second build of libb3d (for instance the previous commit's) and times its b3d_conv2d_wgrad_tf32 on the
-same operands, alternating with this tree's library launch window by launch window: the difference is the change in the
-K-split rule.  Each entry is the median over --reps windows of --n launches, CUDA events around each window."""
+--ref-lib (repeatable) loads other builds of libb3d (for instance the previous commit's) and times their
+b3d_conv2d_wgrad_tf32 on the same operands, alternating with this tree's library launch window by launch window; a build is
+named by its file name.  Each entry is the median over --reps windows of --n launches, CUDA events around each window, and
+its spread (slowest - fastest window).  step_ms is one cfg3 step's share: the generator's launches once, the
+discriminator's twice (two D steps at batch 64), without D1.c1.khfold, the materialised fold that the raw-input stem
+kernel (the stem line, wgrad_raw) replaces."""
 import argparse
 import ctypes
 import json
@@ -80,34 +83,40 @@ def wgrad_call(lib, dy, x, dw, N, H, W, Cin, Hout, Wout, Cout, kh, kw, pad_y, st
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--ref-lib", default=None)
+    ap.add_argument("--ref-lib", action="append", default=[])
     ap.add_argument("--reps", type=int, default=7)
     ap.add_argument("--n", type=int, default=20)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("time_wgrad: needs a CUDA device")
     libs = [("this", b3d.lib)]
-    if a.ref_lib:
-        ref = ctypes.CDLL(os.path.abspath(a.ref_lib))
+    for path in a.ref_lib:
+        ref = ctypes.CDLL(os.path.abspath(path))
         ref.b3d_last_error.restype = ctypes.c_char_p
-        libs.append(("ref", ref))
+        libs.append((os.path.splitext(os.path.basename(path))[0], ref))
     print(json.dumps({"card": card(), "libs": [n for n, _ in libs], "reps": a.reps, "n": a.n}))
     dev = "cuda:0"
     tot = {n: 0.0 for n, _ in libs}
+    step = {n: 0.0 for n, _ in libs}
     for name, N, Cin, H, W, Cout, k, py, st in CFG3:
         kh, kw = k if isinstance(k, tuple) else (k, k)
         Hout, Wout = (H + 2 * py - kh) // st + 1, (W - kw) // st + 1
         x = torch.randn(N, H, W, Cin, device=dev)
         dy = torch.randn(N, Hout, Wout, Cout, device=dev)
         dw = torch.zeros(kh * kw, Cout, Cin, device=dev)
-        ms = timed([wgrad_call(lib, dy, x, dw, N, H, W, Cin, Hout, Wout, Cout, kh, kw, py, st) for _, lib in libs], a.reps, a.n)
+        ts = windows([wgrad_call(lib, dy, x, dw, N, H, W, Cin, Hout, Wout, Cout, kh, kw, py, st) for _, lib in libs], a.reps, a.n)
         row = {"layer": name, "gflop": 2.0 * N * Hout * Wout * Cout * Cin * kh * kw / 1e9}
-        for (ln, _), m in zip(libs, ms):
+        per_step = 0 if name == "D1.c1.khfold" else 2 if name.startswith("D") else 1
+        for (ln, _), t in zip(libs, ts):
+            m = sorted(t)[len(t) // 2]
             row[f"ms_{ln}"] = round(m, 4)
+            row[f"spread_{ln}"] = round(max(t) - min(t), 4)
             tot[ln] += m
-        print(json.dumps(row))
+            step[ln] += per_step * m
+        print(json.dumps(row), flush=True)
         del x, dy, dw
-    print(json.dumps({"total_ms": {k: round(v, 3) for k, v in tot.items()}}))
+    print(json.dumps({"total_ms": {k: round(v, 3) for k, v in tot.items()},
+                      "step_ms": {k: round(v, 3) for k, v in step.items()}}))
 
     # the stem of cfg3's D step: raw input [64, 256, 260, 8], 5 rows folded into 64 channels (y padding 2)
     N, H, W, Cout, pad = 2 * B, 256, 260, 64, 2
@@ -122,11 +131,15 @@ def main():
             "wgrad_on_fold": wgrad_call(b3d.lib, dy, xf, dw, N, H, W, 64, Hout, Wout, Cout, 1, 5, 0, 1),
             "fwd_fold_then_rowwin": lambda: _fprop(fold_rows(xr, 5, pad, 64), wf, None, 1, 5),
             "fwd_on_the_fly": lambda: _fprop(xr, wf, None, 1, 5, fold_kh=5, fold_pad=pad)}
-    if b3d.lib.b3d_version() >= 350:
-        rows["wgrad_raw"] = wgrad_call(b3d.lib, dy, xr, dw, N, H, W, 64, Hout, Wout, Cout, 1, 5, pad, 1, fold_kh=5)
-    ms = timed(list(rows.values()), a.reps, a.n)
-    print(json.dumps({"stem": "D1.conv1 cfg3 (N 64, 256x256, 8 -> 64, 5x5)",
-                      **{f"ms_{k}": round(m, 4) for k, m in zip(rows, ms)}}))
+    for ln, lib in libs:
+        if lib.b3d_version() >= 350:
+            rows[f"wgrad_raw_{ln}"] = wgrad_call(lib, dy, xr, dw, N, H, W, 64, Hout, Wout, Cout, 1, 5, pad, 1, fold_kh=5)
+    ts = windows(list(rows.values()), a.reps, a.n)
+    out = {"stem": "D1.conv1 cfg3 (N 64, 256x256, 8 -> 64, 5x5)"}
+    for k, t in zip(rows, ts):
+        out[f"ms_{k}"] = round(sorted(t)[len(t) // 2], 4)
+        out[f"spread_{k}"] = round(max(t) - min(t), 4)
+    print(json.dumps(out))
 
 
 if __name__ == "__main__":

@@ -97,19 +97,28 @@ class FIDEvaluator:
 
     # ------------------------------------------------------------------------------------------------ the loop
     @torch.no_grad()
-    def evaluate(self, eval_batches, fast=False, seed=None, keep_features=False, distributed=False):
+    def evaluate(self, eval_batches, fast=False, seed=None, keep_features=False, distributed=False, samples=None):
         """eval_batches: iterable of dicts like the reference's eval_loader yields — 'idx' [B], 'rotation' [B,4], 'scale' [B]
         or [B,1], 'translation' [B,3]; optional 'class' [B] or [B,1], 'image' [B,3,R,R] in (0,1) (needed while the real
         statistics are not set), 'texture' + 'mesh' (pseudo-ground-truth: enables the texture-only / mesh-only scores unless
         fast).  seed: main.py:223-227 (args.evaluate): reseeds the noise stream.  distributed: every rank passes ITS shard of
         the evaluation set; the feature sums are all-reduced (torch.distributed) before the distances, so all ranks return the
-        scores of the whole set (the validation-subset scores need the individual features and stay per rank).  Returns a dict
-        of scores (+ the feature matrices with keep_features)."""
+        scores of the whole set (the validation-subset scores need the individual features and stay per rank).  samples:
+        dataset indices whose images to hand back, main.py's visualisation set (:196-202, :296-340): out['samples'] maps
+        'fake', 'fake_tex', 'fake_mesh' and, with pseudo-ground-truth, 'real', 'real_tex', 'fake_texture_only',
+        'fake_mesh_only' to device tensors ordered as `samples` lists the indices found in this rank's batches ('index':
+        those indices); selecting them costs one synchronisation per batch.  Returns a dict of scores (+ the feature
+        matrices with keep_features)."""
         self.generator.eval()
         gen = torch.Generator().manual_seed(seed) if seed is not None else None
         st = {k: FIDStatistics(self.dim, self.device) for k in ("combined", "texture_only", "mesh_only", "real")}
         feats = {k: [] for k in st} if (keep_features or (self.m_real_val is not None and not fast)) else None
         has_pseudogt = False
+        picks = found = None
+        if samples is not None:
+            picks = torch.as_tensor(np.asarray(samples), dtype=torch.int64, device=self.device)
+            found = {k: [] for k in ('index', 'fake', 'fake_mesh', 'fake_tex', 'real', 'real_tex', 'fake_texture_only',
+                                     'fake_mesh_only')}
         for data in eval_batches:
             data = {k: (v.to(self.device) if isinstance(v, torch.Tensor) else v) for k, v in data.items()}
             has_pseudogt = 'texture' in data and not fast
@@ -123,10 +132,28 @@ class FIDEvaluator:
             B = data['rotation'].shape[0]
             noise = truncated_noise(B, self.latent_dim, self.truncation_sigma, gen).to(self.device)
             pred_tex, pred_mesh_map, _ = self.generator(noise, c, None, return_attention=True)
-            self.render_and_score(pred_mesh_map, pred_tex, data, st["combined"], feats["combined"] if feats else None)
+            fake = self.render_and_score(pred_mesh_map, pred_tex, data, st["combined"], feats["combined"] if feats else None)
+            rows = None
+            if picks is not None:
+                rows = torch.isin(data['idx'], picks).nonzero().flatten()
+                if rows.numel():
+                    found['index'].append(data['idx'][rows])
+                    for k, v in (('fake', fake), ('fake_mesh', pred_mesh_map), ('fake_tex', pred_tex)):
+                        found[k].append(v[rows])
+                    if has_pseudogt and 'image' in data:
+                        found['real'].append(data['image'][rows])
+                    if has_pseudogt:
+                        found['real_tex'].append(data['texture'][rows])
+                else:
+                    rows = None
             if has_pseudogt:
-                self.render_and_score(data['mesh'], pred_tex, data, st["texture_only"], feats["texture_only"] if feats else None)
-                self.render_and_score(pred_mesh_map, data['texture'], data, st["mesh_only"], feats["mesh_only"] if feats else None)
+                tex_only = self.render_and_score(data['mesh'], pred_tex, data, st["texture_only"],
+                                                 feats["texture_only"] if feats else None)
+                mesh_only = self.render_and_score(pred_mesh_map, data['texture'], data, st["mesh_only"],
+                                                  feats["mesh_only"] if feats else None)
+                if rows is not None:
+                    found['fake_texture_only'].append(tex_only[rows])
+                    found['fake_mesh_only'].append(mesh_only[rows])
         if distributed:
             for k in st:
                 st[k].all_reduce()
@@ -152,7 +179,20 @@ class FIDEvaluator:
         if keep_features:
             out["features"] = {k: torch.cat(v, dim=0) for k, v in feats.items() if v}
         out["num_generated"] = st["combined"].n
+        if found is not None:
+            out["samples"] = ordered_samples(found, picks)
         return out
+
+
+def ordered_samples(found, picks):
+    """The collected visualisation rows, reordered from evaluation order to the order of `picks` (main.py:199, :330-340:
+    argsort(argsort(indices)) on the sorted indices); the indices not found are left out."""
+    if not found['index']:
+        return {'index': picks[:0]}
+    index = torch.cat(found['index'])
+    pos = (index.unsqueeze(1) == picks.unsqueeze(0)).int().argmax(dim=1)    # position of each found index in picks
+    order = torch.argsort(pos)
+    return {k: torch.cat(v)[order] for k, v in found.items() if v}
 
 
 def select_best_checkpoint(trainer, evaluator, checkpoint_dir, eval_batches, seed=None, distributed=False):
@@ -162,7 +202,8 @@ def select_best_checkpoint(trainer, evaluator, checkpoint_dir, eval_batches, see
     the best one only on a strictly smaller FID.  The best checkpoint is then loaded and evaluated in full.  evaluator
     must score trainer's running-average generator (FIDEvaluator(trainer.trainer.generator_running_avg, ...)): the
     loads copy into it in place.  seed and distributed are passed to every evaluate call (the reference seeds every
-    evaluation with 1234 in this mode).  -> dict(fast_fid={epoch: fid} in visit order, best_path, scores)."""
+    evaluation with 1234 in this mode).  -> dict(fast_fid={epoch: fid} in visit order,
+    paths={epoch: path}, best_path, scores)."""
     checkpoints = {}
     for path in sorted(glob.glob(os.path.join(checkpoint_dir, 'checkpoint_[0-9]*.pth'))):
         m = re.search('checkpoint_([0-9]+).pth', path)
@@ -182,4 +223,4 @@ def select_best_checkpoint(trainer, evaluator, checkpoint_dir, eval_batches, see
         raise ValueError(f'no finite fast FID among {sorted(checkpoints)}')
     trainer.load_checkpoint(best_path, 'evaluate')
     scores = evaluator.evaluate(eval_batches, seed=seed, distributed=distributed)
-    return dict(fast_fid=fast_fid, best_path=best_path, scores=scores)
+    return dict(fast_fid=fast_fid, paths=checkpoints, best_path=best_path, scores=scores)

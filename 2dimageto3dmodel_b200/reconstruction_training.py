@@ -41,6 +41,11 @@ def default_args(**kw):
 
 
 class ReconTrainer:
+    # keep_last_images: forward_loss keeps the batch and its render in `last_images` (run_reconstruction.py's
+    # training-image summaries, :321-323, :487-488); off by default, as it holds one batch of renders into the next step
+    keep_last_images = False
+    last_images = None
+
     def __init__(self, args, mesh_template, dataset_size, device='cuda', capturable=False):
         if args.loss not in ('mse', 'l1'):
             raise ValueError(f"ReconTrainer: loss={args.loss!r}; the reference's criteria are 'mse' and 'l1'")
@@ -81,6 +86,8 @@ class ReconTrainer:
             z0 = dp(gt_idx, 'z0')
         raw_vtx, vtx = self.tpl.vertices_and_pose(mesh_map, scale, trans, gt_rot, z0)
         image_pred, alpha_pred = self.tpl.forward_renderer(self.renderer, vtx, pred_tex)
+        if self.keep_last_images:
+            self.last_images = (X_real, image_pred.detach(), alpha_pred.detach())
         recon_loss, miou = self.criterion(image_pred, alpha_pred, X_real)
         flat_loss = loss_flat(self.tpl.mesh, self.tpl.compute_normals(raw_vtx))
         loss = recon_loss + (a.mesh_regularization * self.flat_warmup) * flat_loss
@@ -164,7 +171,7 @@ class ReconTrainer:
             self.flat_warmup.fill_(chk.get('flat_warmup', 10.0))
 
     @torch.no_grad()
-    def evaluate(self, batches, distributed=False):
+    def evaluate(self, batches, distributed=False, samples=None):
         """The validation pass evaluate_all (:255-319) without its TensorBoard images: every batch (X_real, gt_scale,
         gt_translation, gt_rot[, idx]) is posed with the DATASET-MEAN DatasetParams (transform_vertices(..., None), :274)
         and scored with the configured criterion, loss_flat and mean IoU.  -> dict(recon_loss, flat_loss, miou, N): the
@@ -172,8 +179,13 @@ class ReconTrainer:
         '[TEST] recon_loss {:.5f}, flat_loss {:.5f}, mIoU {:.5f}, N {}'.  A batch whose predicted and target alpha are
         both empty has a NaN IoU, as in the reference.  The sums stay on the device in fp64 (one host sync at the end).
         distributed: every rank passes its shard; the sums are all-reduced before the division, so every rank returns the
-        values of the whole set (eval-mode batch norm couples no samples)."""
+        values of the whole set (eval-mode batch norm couples no samples).  samples: positions in the sequence of
+        `batches` (run_reconstruction.py's debug_ids, :161, :172, :287-299) whose images to hand back: the result's
+        'samples' holds 'real' and 'fake' ([k,4,H,W] on the device, in position order) and 'render', the
+        render_multiview tiles of the first four."""
         a, dp = self.args, self.dataset_params
+        picks = sorted(int(i) for i in samples) if samples is not None else None
+        real, fake, render, pos = [], [], [], 0
         self.generator.eval()
         sums = torch.zeros(4, dtype=torch.float64, device=next(self.generator.parameters()).device)
         for X_real, gt_scale, gt_translation, gt_rot, *_ in batches:
@@ -190,10 +202,23 @@ class ReconTrainer:
             recon_loss, miou = self.criterion(image_pred, alpha_pred, X_real)
             flat_loss = loss_flat(self.tpl.mesh, self.tpl.compute_normals(raw_vtx))
             sums += torch.stack((recon_loss.double(), flat_loss.double(), miou.double(), sums.new_ones(()))) * B
+            if picks is not None:
+                rows = [i - pos for i in picks if pos <= i < pos + B]
+                if rows:
+                    real.append(X_real[rows])
+                    fake.append(torch.cat((image_pred, alpha_pred), dim=3).permute(0, 3, 1, 2)[rows])
+                    for r in rows:
+                        if len(render) < 4:
+                            render.append(self.render_multiview(raw_vtx, pred_tex, r))
+            pos += B
         if distributed:
             dist.all_reduce(sums, op=dist.ReduceOp.SUM)
         recon, flat, miou, n = sums.tolist()
-        return dict(recon_loss=recon / n, flat_loss=flat / n, miou=miou / n, N=int(n))
+        out = dict(recon_loss=recon / n, flat_loss=flat / n, miou=miou / n, N=int(n))
+        if picks is not None:
+            out['samples'] = dict(real=torch.cat(real) if real else None, fake=torch.cat(fake) if fake else None,
+                                  render=render)
+        return out
 
     @torch.no_grad()
     def render_multiview(self, raw_vtx, pred_tex, idx=0):

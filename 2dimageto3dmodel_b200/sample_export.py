@@ -34,18 +34,22 @@ RENDER_RES = 512          # main.py:158, "For exporting images: higher resolutio
 GRID_COLUMNS = 8          # make_grid(nrow=8)
 
 
-def grid_shape(n, tile_h, tile_w, nrow=GRID_COLUMNS):
-    """torchvision.utils.make_grid's layout with padding 0: min(nrow, n) columns, ceil(n / columns) rows."""
+def grid_shape(n, tile_h, tile_w, nrow=GRID_COLUMNS, padding=0):
+    """torchvision.utils.make_grid's layout: min(nrow, n) columns, ceil(n / columns) rows, `padding` pixels before every
+    row and column and after the last ones."""
     cols = min(nrow, n)
-    return (math.ceil(n / cols) * tile_h, cols * tile_w, 3), cols
+    rows = math.ceil(n / cols)
+    return (rows * (tile_h + padding) + padding, cols * (tile_w + padding) + padding, 3), cols
 
 
-def place_tiles(grid, cols, k0, tiles):
-    """Tiles k0, k0 + 1, ... into their grid cells, row-major over `cols` columns."""
+def place_tiles(grid, cols, k0, tiles, padding=0):
+    """Tiles k0, k0 + 1, ... ([k, h, w, 3], numpy or torch like grid) into their grid cells, row-major over `cols`
+    columns."""
     h, w = tiles.shape[1], tiles.shape[2]
     for i in range(tiles.shape[0]):
         r, c = divmod(k0 + i, cols)
-        grid[r * h:(r + 1) * h, c * w:(c + 1) * w] = tiles[i]
+        y, x = r * (h + padding) + padding, c * (w + padding) + padding
+        grid[y:y + h, x:x + w] = tiles[i]
 
 
 def assemble_grid(tiles, nrow=GRID_COLUMNS):

@@ -61,6 +61,12 @@ def splat_grid(pg, V, mode="R"):
     return grid
 
 
+def _silhouette_fwd(srt, bins, taps, sc, B, N, V, mode, sil, ws, st):
+    h = host_floats(taps)
+    check(lib.b3d_pc_silhouette_fwd_hosttaps(ptr(srt), ptr(bins), ctypes.cast(h, ctypes.c_void_p), len(taps), ptr(sc), B, N,
+                                             V, mode, ptr(sil), ptr(ws), ws.numel() * 4, st))
+
+
 class _EffectiveLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, points, quat, scale, taps, V, mode, fov, cam_dist):
@@ -74,16 +80,18 @@ class _EffectiveLoss(torch.autograd.Function):
                 raise B3DError(f"scale must hold one value per sample, got shape {tuple(scale.shape)}")
         pg, srt, bins = project(points, quat, V, fov, cam_dist, want_bins=True)
         sil = torch.empty(B, V, V, device=points.device, dtype=torch.float32)
-        h = host_floats(taps)
-        check(lib.b3d_pc_silhouette_fwd_hosttaps(ptr(srt), ptr(bins), ctypes.cast(h, ctypes.c_void_p), len(taps),
-                                                 ptr(sc), B, N, V, mode, ptr(sil), None, 0, stream_ptr(points)))
-        ctx.save_for_backward(points, quat, pg, srt, bins, sc if sc is not None else torch.empty(0))
+        # mode P: the splat grid and the occupancy blurred along x and y (2 B V^3 floats), kept for the backward
+        nbytes = lib.b3d_pc_silhouette_workspace_bytes(B, V, mode)
+        ws = torch.empty(nbytes // 4, device=points.device, dtype=torch.float32)
+        _silhouette_fwd(srt, bins, taps, sc, B, N, V, mode, sil, ws, stream_ptr(points))
+        ctx.save_for_backward(points, quat, pg, srt, bins, sc if sc is not None else torch.empty(0), ws)
         ctx.cfg = (taps, V, mode, fov, cam_dist, scale.shape if scale is not None else None)
+        ctx.ws_spent = False
         return sil
 
     @staticmethod
     def backward(ctx, dsil):
-        points, quat, pg, srt, bins, sc = ctx.saved_tensors
+        points, quat, pg, srt, bins, sc, ws = ctx.saved_tensors
         taps, V, mode, fov, cam_dist, scale_shape = ctx.cfg
         has_scale = scale_shape is not None
         B, N, _ = points.shape
@@ -92,9 +100,14 @@ class _EffectiveLoss(torch.autograd.Function):
         dscale = torch.empty(B, device=points.device, dtype=torch.float32) if has_scale else None
         h = host_floats(taps)
         st = stream_ptr(points)
+        if ctx.ws_spent and ws.numel():
+            # a second backward through the same graph (retain_graph=True): the first one overwrote the workspace with
+            # its gradients, so the forward refills it
+            _silhouette_fwd(srt, bins, taps, sc if has_scale else None, B, N, V, mode, torch.empty_like(dsil), ws, st)
+        ctx.ws_spent = True
         check(lib.b3d_pc_silhouette_bwd_hosttaps(ptr(srt), ptr(bins), ctypes.cast(h, ctypes.c_void_p), len(taps),
                                                  ptr(sc) if has_scale else None, ptr(dsil), B, N, V, mode, ptr(dpg),
-                                                 ptr(dscale), None, 0, st))
+                                                 ptr(dscale), ptr(ws), ws.numel() * 4, st))
         dpoints = torch.empty_like(points)
         dquat = torch.empty_like(quat)
         check(lib.b3d_pc_project_bwd(ptr(points), ptr(quat), ptr(pg), ptr(dpg), B, N, V, fov, cam_dist, ptr(dpoints),
@@ -104,14 +117,18 @@ class _EffectiveLoss(torch.autograd.Function):
 
 def effective_loss(points, quat, scale=None, V=64, taps=None, mode="R", fov=FIELD_OF_VIEW,
                    cam_dist=CAMERA_VIEW_DISTANCE):
-    """points [B,N,3] (z,y,x), quat [B,4], scale [B,1]|None -> silhouette [B,V,V] (differentiable)."""
+    """points [B,N,3] (z,y,x), quat [B,4], scale [B,1]|None -> silhouette [B,V,V] (differentiable).
+
+    mode "R": one fused kernel per direction, the grid never leaves shared memory.  mode "P": the x / y blur couples the
+    columns, so the grid goes through a workspace of 2 B V^3 floats held from the forward to the backward (four grid
+    transfers forward, five backward)."""
     if taps is None:
         taps = smoothing_taps(3.0, 21, mode)
     return _EffectiveLoss.apply(points, quat, scale, list(taps), int(V), mode_id(mode), float(fov), float(cam_dist))
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# dense-grid path: stand-alone VoxelsSmooth / termination_probs surface and the paper semantics (mode P)
+# dense-grid path: the stand-alone VoxelsSmooth / termination_probs surface, one autograd function per stage
 # ------------------------------------------------------------------------------------------------------------------
 def _taps_arr(taps):
     h = host_floats(taps)
@@ -240,8 +257,8 @@ def occupancy_grid(points, quat, V, mode="R", fov=FIELD_OF_VIEW, cam_dist=CAMERA
 def effective_loss_dense(points, quat, scale=None, V=64, taps=None, mode="P", fov=FIELD_OF_VIEW,
                          cam_dist=CAMERA_VIEW_DISTANCE):
     """The effective loss over a MATERIALISED grid: splat -> clamp -> blur (z only in mode R; x, y, z chained in
-    mode P) -> scale/clamp -> ray termination -> silhouette.  This is the only path for mode P (its 3-axis blur
-    couples the columns); for mode R it is the slow twin of the fused kernel and serves as a cross-check."""
+    mode P) -> scale/clamp -> ray termination -> silhouette, one stand-alone full-grid kernel per stage.  It is the
+    slow twin of `effective_loss` in both modes (the fused entry points) and serves as a cross-check."""
     if taps is None:
         taps = smoothing_taps(3.0, 21, mode)
     occ = occupancy_grid(points, quat, V, mode, fov, cam_dist)

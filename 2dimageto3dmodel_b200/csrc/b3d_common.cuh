@@ -74,4 +74,9 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// dpg[b, original index] = d/d(grid coords) of every bin-sorted point, gathered at its 8 corners of dgrid [B,V,V,V]
+// (csrc/vox_kernels.cu; b3d_vox_gather masks dgrid first, the mode-P silhouette backward has masked it already)
+int vox_gather_launch(const float* sorted, const int32_t* bin_start, const float* dgrid, int B, int N, int V, int mode,
+                      float* dpg, cudaStream_t st);
+
 }  // namespace b3d

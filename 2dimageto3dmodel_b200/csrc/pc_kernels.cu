@@ -12,8 +12,12 @@
 //   pc_sil_bwd_kernel        recomputes the patch (+1 halo so every point is owned by exactly one CTA),
 //                            runs the ray-march / clamp / blur adjoints column-wise in shared memory and
 //                            gathers d/d(grid coords) per point: no dense gradient grid in HBM either.
+//   pc_blur_xy_kernel        mode P: clamp + x blur + y blur of one z slice tile with its halo (forward), or the
+//                            transposed y, x blur + clamp mask (backward), between the two workspace grids.
+//   pc_sil_p_fwd_kernel      mode P: the mode-R forward without its splat (z blur, scale/clamp, ray march) over the
+//                            x/y-blurred grid; pc_sil_p_bwd_kernel its column adjoints, written back over that grid.
 //   pc_project_bwd_kernel    adjoint of projection + rotation + quaternion normalisation.
-//   pc_splat_grid_kernel     materialised occupancy grid (parity tests, mode P).
+//   pc_splat_grid_kernel     materialised occupancy grid (parity tests).
 //
 // Reference lines restated: quaternions/points_quaternions.py:41-81, quaternions/operations.py:68-136,
 // camera/coordinate_system_transformation.py:20-39, utils/trilinear_interpolation.py:17-74,
@@ -288,9 +292,56 @@ __device__ __forceinline__ void clamp_patch(float* A, int n) {
 }
 
 // ----------------------------------------------------------------------------------------------
-// forward.  Work items are (column, block of ZB depths): every item blurs its block, turns it into
-// occupancies and reduces it to (transmittance of the block, silhouette gathered inside the block);
-// a second, short pass chains the blocks of each column.
+// forward of one patch of TY x TX columns A [V][ncol] (row pitch TX, first column (ty0, tx0)), shared by both modes.
+// Work items are (column, block of ZB depths): every item blurs its block along z, turns it into occupancies and
+// reduces it to (transmittance of the block, silhouette gathered inside the block); a second, short pass chains the
+// blocks of each column.  ABS: A holds clamped occupancies with the clamp mask in the sign bit (mode R); otherwise A
+// holds plain values (mode P: the occupancy already blurred along x and y).  zlo / zhi are read only when skip_ok.
+// ----------------------------------------------------------------------------------------------
+template <int KT, bool ABS>
+__device__ __forceinline__ void sil_fwd_columns(const float* A, float* blkP, float* blkS, const int* zlo, const int* zhi,
+                                                bool skip_ok, const Taps& taps, bool has_scale, float sc, float c0, int b,
+                                                int V, int ncol, int ty0, int tx0, float* __restrict__ sil) {
+    const int tid = threadIdx.x, nzb = (V + ZB - 1) / ZB;
+    const int HB = (KT > 0 ? KT : taps.n) / 2;
+    for (int it = tid; it < nzb * ncol; it += TILE_THREADS) {
+        const int col = it % ncol, zb = (it / ncol) * ZB;
+        float S[ZB];
+        if (skip_ok && (zb + ZB - 1 < zlo[col] - HB || zb > zhi[col] + HB)) {
+#pragma unroll
+            for (int j = 0; j < ZB; ++j) S[j] = 0.f;             // no occupied cell within the taps' reach: the blur is exactly 0
+        } else {
+            blur_window<KT, false, ABS>(A + col, ncol, V, zb, taps, S);
+        }
+        float T = 1.f, acc = 0.f;
+#pragma unroll
+        for (int j = 0; j < ZB; ++j) {
+            if (zb + j < V) {
+                const float o = clamp_nan(scaled(S[j], has_scale, sc), TERM_EPS, 1.f - TERM_EPS);
+                float term = o * T;                       // o_k * prod_{j<k}(1-o_j)
+                if (zb + j == 0) term *= c0;
+                acc += term;
+                T *= (1.f - o);
+            }
+        }
+        blkP[it] = T;
+        blkS[it] = acc;
+    }
+    __syncthreads();
+    for (int col = tid; col < ncol; col += TILE_THREADS) {
+        const int y = ty0 + col / TX, x = tx0 + col % TX;
+        if (y >= V || x >= V) continue;
+        float T = 1.f, acc = 0.f;
+        for (int k = 0; k < nzb; ++k) {
+            acc = fmaf(T, blkS[k * ncol + col], acc);
+            T *= blkP[k * ncol + col];
+        }
+        sil[((size_t)b * V + (V - 1 - y)) * V + x] = acc;   // flip(1): effective_loss_function.py:81
+    }
+}
+
+// ----------------------------------------------------------------------------------------------
+// forward, mode R: splat into the patch with shared-memory atomics, clamp, then the column work above
 // ----------------------------------------------------------------------------------------------
 template <int KT>
 __global__ void __launch_bounds__(TILE_THREADS)
@@ -325,86 +376,21 @@ pc_sil_fwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__
     const float c0 = (mode == B3D_MODE_REFERENCE) ? expf(TERM_EPS) : 1.f;   // D10 pad row
     // sparsity skip: exact only when 0 * tap and 0 * scale are 0 (finite taps / scale; NaN must propagate, SURVEY D4)
     const bool skip_ok = taps.finite && (!has_scale || fabsf(sc) <= 3.0e38f);
-    const int HB = (KT > 0 ? KT : taps.n) / 2;
-    for (int it = tid; it < nzb * ncol; it += TILE_THREADS) {
-        const int col = it % ncol, zb = (it / ncol) * ZB;
-        float S[ZB];
-        if (skip_ok && (zb + ZB - 1 < zlo[col] - HB || zb > zhi[col] + HB)) {
-#pragma unroll
-            for (int j = 0; j < ZB; ++j) S[j] = 0.f;             // no occupied cell within the taps' reach: the blur is exactly 0
-        } else {
-            blur_window<KT, false, true>(A + col, ncol, V, zb, taps, S);
-        }
-        float T = 1.f, acc = 0.f;
-#pragma unroll
-        for (int j = 0; j < ZB; ++j) {
-            if (zb + j < V) {
-                const float o = clamp_nan(scaled(S[j], has_scale, sc), TERM_EPS, 1.f - TERM_EPS);
-                float term = o * T;                       // o_k * prod_{j<k}(1-o_j)
-                if (zb + j == 0) term *= c0;
-                acc += term;
-                T *= (1.f - o);
-            }
-        }
-        blkP[it] = T;
-        blkS[it] = acc;
-    }
-    __syncthreads();
-    for (int col = tid; col < ncol; col += TILE_THREADS) {
-        const int y = ty0 + col / TX, x = tx0 + col % TX;
-        if (y >= V || x >= V) continue;
-        float T = 1.f, acc = 0.f;
-        for (int k = 0; k < nzb; ++k) {
-            acc = fmaf(T, blkS[k * ncol + col], acc);
-            T *= blkP[k * ncol + col];
-        }
-        sil[((size_t)b * V + (V - 1 - y)) * V + x] = acc;   // flip(1): effective_loss_function.py:81
-    }
+    sil_fwd_columns<KT, true>(A, blkP, blkS, zlo, zhi, skip_ok, taps, has_scale, sc, c0, b, V, ncol, ty0, tx0, sil);
 }
 
 // ----------------------------------------------------------------------------------------------
-// backward (patch with a +1 halo so that every point is owned by exactly one CTA)
+// backward of one patch, shared by both modes: A1 [V][ncol] holds the forward's input of the z blur (ABS as in
+// sil_fwd_columns), row pitch `pitch`; columns with cy < TY and cx < TX are owned (their terms go into dscale).
+// On return A1 holds d(input of the z blur) — masked by the sign bit when ABS — and A2 is scratch.
 // ----------------------------------------------------------------------------------------------
-template <int KT>
-__global__ void __launch_bounds__(TILE_THREADS)
-pc_sil_bwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__ bin_start, const Taps taps,
-                  const float* __restrict__ scale, const float* __restrict__ dsil, int N, int V, int TY, int mode,
-                  int nbx, int nby, float4* __restrict__ dpg, float* __restrict__ dscale) {
-    extern __shared__ __align__(128) float sm[];
-    __shared__ float red[32];
-    const int b = blockIdx.z, ty0 = blockIdx.y * TY, tx0 = blockIdx.x * TX;
-    const int cy1 = min(ty0 + TY, V - 1), cx1 = min(tx0 + TX, V - 1);     // extended patch, clipped to the grid
-    const int EX = TX + 1, ncol = (TY + 1) * EX, nzb = (V + ZB - 1) / ZB;
-    float* A1 = sm;                      // clamped occupancy (sign = clamp mask) -> dG
-    float* A2 = A1 + V * ncol;           // blurred S -> dS
-    float* blkA = A2 + V * ncol;         // [nzb][ncol] transmittance of the block
-    float* blkB = blkA + nzb * ncol;     // [nzb][ncol] offset of the block's Q recurrence -> Q just after the block
-    float* blkT = blkB + nzb * ncol;     // [nzb][ncol] transmittance at the start of the block
-    int* zlo = reinterpret_cast<int*>(blkT + nzb * ncol);    // [ncol] first / last occupied depth of the column
-    int* zhi = zlo + ncol;
-    const int tid = threadIdx.x;
-    const float4* sp = sorted + (size_t)b * N;
-    const int32_t* bs = bin_start + (size_t)b * (nbx * nby + 1);
-    for (int i = tid; i < V * ncol; i += TILE_THREADS) A1[i] = 0.f;
-    for (int i = tid; i < ncol; i += TILE_THREADS) { zlo[i] = V; zhi[i] = -1; }
-    __syncthreads();
-    for_each_record(sp, bs, nbx, max(ty0 - 1, 0) / BIN_Y, min(cy1 / BIN_Y, nby - 1), max(tx0 - 1, 0) / BIN_X,
-                    min(cx1 / BIN_X, nbx - 1),
-                    [&](const float4 g) { splat_record(g, ty0, cy1, tx0, cx1, EX, ncol, mode, A1, zlo, zhi); });
-    __syncthreads();
-    const int oy1 = min(ty0 + TY, V) - 1, ox1 = min(tx0 + TX, V) - 1;   // owned base cells (the gather at the end)
-    const int gby_lo = ty0 / BIN_Y, gby_hi = min(oy1 / BIN_Y, nby - 1);
-    const int gbx_lo = tx0 / BIN_X, gbx_hi = min(ox1 / BIN_X, nbx - 1);
-    clamp_patch(A1, V * ncol);
-    __syncthreads();
-
-    const bool has_scale = scale != nullptr;
-    const float sc = has_scale ? scale[b] : 1.f;
-    const float c0 = (mode == B3D_MODE_REFERENCE) ? expf(TERM_EPS) : 1.f;
+template <int KT, bool ABS>
+__device__ __forceinline__ void sil_bwd_columns(float* A1, float* A2, float* blkA, float* blkB, float* blkT, const int* zlo,
+                                                const int* zhi, bool skip_ok, const Taps& taps, bool has_scale, float sc,
+                                                float c0, const float* __restrict__ dsil, int b, int V, int ncol, int pitch,
+                                                int TY, int ty0, int tx0, float* red, float* __restrict__ dscale) {
+    const int tid = threadIdx.x, nzb = (V + ZB - 1) / ZB;
     const int nitems = nzb * ncol;
-    // sparsity skip (see the forward kernel): S == 0 exactly outside [zlo - H, zhi + H]; there o = eps is clamped, so
-    // d sil / d S == 0 as well, and the transposed blur of dS vanishes outside [zlo - 2H, zhi + 2H]
-    const bool skip_ok = taps.finite && (!has_scale || fabsf(sc) <= 3.0e38f);
     const int HB = (KT > 0 ? KT : taps.n) / 2;
 
     // pass 1: S = blur_z(O); per block: a = prod(1-o), b = Q at block start for Q = 0 after the block
@@ -415,7 +401,7 @@ pc_sil_bwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__
 #pragma unroll
             for (int j = 0; j < ZB; ++j) S[j] = 0.f;
         } else {
-            blur_window<KT, false, true>(A1 + col, ncol, V, zb, taps, S);
+            blur_window<KT, false, ABS>(A1 + col, ncol, V, zb, taps, S);
         }
         float a = 1.f, q = 0.f;
 #pragma unroll
@@ -450,7 +436,7 @@ pc_sil_bwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__
     float dsc = 0.f;
     for (int it = tid; it < nitems; it += TILE_THREADS) {
         const int col = it % ncol, zb = (it / ncol) * ZB;
-        const int cy = col / EX, cx = col % EX;
+        const int cy = col / pitch, cx = col % pitch;
         const int y = ty0 + cy, x = tx0 + cx;
         if (y >= V || x >= V) continue;
         if (skip_ok && (zb + ZB - 1 < zlo[col] - HB || zb > zhi[col] + HB)) continue;     // dS == 0 == what A2 already holds
@@ -498,10 +484,57 @@ pc_sil_bwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__
 #pragma unroll
         for (int j = 0; j < ZB; ++j) {
             const int z = zb + j;
-            if (z < V) A1[z * ncol + col] = signbit(A1[z * ncol + col]) ? 0.f : D[j];
+            if (z < V) A1[z * ncol + col] = (ABS && signbit(A1[z * ncol + col])) ? 0.f : D[j];
         }
     }
     __syncthreads();
+}
+
+// ----------------------------------------------------------------------------------------------
+// backward, mode R (patch with a +1 halo so that every point is owned by exactly one CTA): splat + clamp as in the
+// forward, the column adjoints above, then the gather to the points straight from shared memory
+// ----------------------------------------------------------------------------------------------
+template <int KT>
+__global__ void __launch_bounds__(TILE_THREADS)
+pc_sil_bwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__ bin_start, const Taps taps,
+                  const float* __restrict__ scale, const float* __restrict__ dsil, int N, int V, int TY, int mode,
+                  int nbx, int nby, float4* __restrict__ dpg, float* __restrict__ dscale) {
+    extern __shared__ __align__(128) float sm[];
+    __shared__ float red[32];
+    const int b = blockIdx.z, ty0 = blockIdx.y * TY, tx0 = blockIdx.x * TX;
+    const int cy1 = min(ty0 + TY, V - 1), cx1 = min(tx0 + TX, V - 1);     // extended patch, clipped to the grid
+    const int EX = TX + 1, ncol = (TY + 1) * EX, nzb = (V + ZB - 1) / ZB;
+    float* A1 = sm;                      // clamped occupancy (sign = clamp mask) -> dG
+    float* A2 = A1 + V * ncol;           // blurred S -> dS
+    float* blkA = A2 + V * ncol;         // [nzb][ncol] transmittance of the block
+    float* blkB = blkA + nzb * ncol;     // [nzb][ncol] offset of the block's Q recurrence -> Q just after the block
+    float* blkT = blkB + nzb * ncol;     // [nzb][ncol] transmittance at the start of the block
+    int* zlo = reinterpret_cast<int*>(blkT + nzb * ncol);    // [ncol] first / last occupied depth of the column
+    int* zhi = zlo + ncol;
+    const int tid = threadIdx.x;
+    const float4* sp = sorted + (size_t)b * N;
+    const int32_t* bs = bin_start + (size_t)b * (nbx * nby + 1);
+    for (int i = tid; i < V * ncol; i += TILE_THREADS) A1[i] = 0.f;
+    for (int i = tid; i < ncol; i += TILE_THREADS) { zlo[i] = V; zhi[i] = -1; }
+    __syncthreads();
+    for_each_record(sp, bs, nbx, max(ty0 - 1, 0) / BIN_Y, min(cy1 / BIN_Y, nby - 1), max(tx0 - 1, 0) / BIN_X,
+                    min(cx1 / BIN_X, nbx - 1),
+                    [&](const float4 g) { splat_record(g, ty0, cy1, tx0, cx1, EX, ncol, mode, A1, zlo, zhi); });
+    __syncthreads();
+    const int oy1 = min(ty0 + TY, V) - 1, ox1 = min(tx0 + TX, V) - 1;   // owned base cells (the gather at the end)
+    const int gby_lo = ty0 / BIN_Y, gby_hi = min(oy1 / BIN_Y, nby - 1);
+    const int gbx_lo = tx0 / BIN_X, gbx_hi = min(ox1 / BIN_X, nbx - 1);
+    clamp_patch(A1, V * ncol);
+    __syncthreads();
+
+    const bool has_scale = scale != nullptr;
+    const float sc = has_scale ? scale[b] : 1.f;
+    const float c0 = (mode == B3D_MODE_REFERENCE) ? expf(TERM_EPS) : 1.f;
+    // sparsity skip (see the forward kernel): S == 0 exactly outside [zlo - H, zhi + H]; there o = eps is clamped, so
+    // d sil / d S == 0 as well, and the transposed blur of dS vanishes outside [zlo - 2H, zhi + 2H]
+    const bool skip_ok = taps.finite && (!has_scale || fabsf(sc) <= 3.0e38f);
+    sil_bwd_columns<KT, true>(A1, A2, blkA, blkB, blkT, zlo, zhi, skip_ok, taps, has_scale, sc, c0, dsil, b, V, ncol, EX, TY,
+                              ty0, tx0, red, dscale);
 
     // gather: every in-bounds point is owned by the patch holding its base cell
     float4* dp = dpg + (size_t)b * N;
@@ -530,6 +563,146 @@ pc_sil_bwd_kernel(const float4* __restrict__ sorted, const int32_t* __restrict__
         dp[__float_as_int(g.w)] = make_float4(dz, dy, dx, 0.f);
     };
     for_each_record(sp, bs, nbx, gby_lo, gby_hi, gbx_lo, gbx_hi, gather);
+}
+
+// ----------------------------------------------------------------------------------------------
+// mode P.  The blur runs along x, y and z, so the columns are coupled and the grid goes through HBM, in the caller's
+// workspace (grid A: raw splat, grid B: clamped occupancy blurred along x and y; both [B,V,V,V], z-major):
+//   fwd  b3d_vox_splat_sorted -> A;  pc_blur_xy_kernel<., false>: A -> clamp -> x blur -> y blur -> B;
+//        pc_sil_p_fwd_kernel: B -> z blur -> scale / clamp -> ray march -> sil (sil_fwd_columns)
+//   bwd  pc_sil_p_bwd_kernel: B -> the column adjoints (sil_bwd_columns) -> dB, in place over B;
+//        pc_blur_xy_kernel<., true>: dB -> y^T -> x^T -> mask 0 <= A <= 1 -> dA, in place over A;
+//        b3d::vox_gather_launch: dA -> dpg
+// ----------------------------------------------------------------------------------------------
+constexpr int XY_TX = 64, XY_TY = 32;  // output tile of the x / y blur: one z slice, 64 x 32 cells, halo ktaps/2 around
+constexpr int XY_THREADS = 256;
+
+// shared memory of pc_blur_xy_kernel for half-width H: the tile with its halo [RY][P] (P odd: a warp walking down the
+// rows hits 32 banks) and the tile after the first blur ([RY][XY_TX + 1] forward, [XY_TY][P] adjoint)
+inline size_t xy_tile_floats(int H) {
+    const size_t P = XY_TX + 2 * H + 1, RY = XY_TY + 2 * H;
+    const size_t mid_f = RY * (XY_TX + 1), mid_a = XY_TY * P;
+    return RY * P + (mid_f > mid_a ? mid_f : mid_a);
+}
+
+// forward (ADJ false): dst = blur_y(blur_x(clamp(src, 0, 1))).   adjoint (ADJ true): dst = [0 <= raw <= 1] *
+// blur_x^T(blur_y^T(src)); raw and dst may be the same buffer (each cell is read and written by one thread).
+// Zero padding, taps in the order of vox_blur_axis_kernel.  grid (B*V slices, tiles of the slice).
+template <int KT, bool ADJ>
+__global__ void __launch_bounds__(XY_THREADS)
+pc_blur_xy_kernel(const float* __restrict__ src, const float* raw, float* dst, const Taps taps, int V, int ntx) {
+    extern __shared__ __align__(128) float sm[];
+    const int H = (KT > 0 ? KT : taps.n) / 2;
+    const int W = XY_TX + 2 * H, P = W + 1, RY = XY_TY + 2 * H;
+    float* in = sm;
+    float* mid = sm + RY * P;
+    const size_t slice = (size_t)blockIdx.x * V * V;
+    const int ty0 = (blockIdx.y / ntx) * XY_TY, tx0 = (blockIdx.y % ntx) * XY_TX;
+    const int tid = threadIdx.x;
+    for (int i = tid; i < RY * P; i += XY_THREADS) {
+        const int r = i / P, c = i % P, y = ty0 - H + r, x = tx0 - H + c;
+        float v = 0.f;
+        if (c < W && y >= 0 && y < V && x >= 0 && x < V) {
+            v = src[slice + (size_t)y * V + x];
+            if (!ADJ) v = clamp_nan(v, 0.f, 1.f);            // trilinear_interpolation.py:74
+        }
+        in[i] = v;
+    }
+    __syncthreads();
+    float o[ZB];
+    if (!ADJ) {
+        constexpr int MP = XY_TX + 1;
+        for (int it = tid; it < RY * (XY_TX / ZB); it += XY_THREADS) {        // x blur of every row, halo rows included
+            const int r = it % RY, xb = (it / RY) * ZB;
+            blur_window<KT, false, false>(in + r * P, 1, P, xb + H, taps, o);
+#pragma unroll
+            for (int j = 0; j < ZB; ++j) mid[r * MP + xb + j] = o[j];
+        }
+        __syncthreads();
+        for (int it = tid; it < XY_TX * (XY_TY / ZB); it += XY_THREADS) {     // y blur
+            const int c = it % XY_TX, yb = (it / XY_TX) * ZB, x = tx0 + c;
+            if (x >= V) continue;
+            blur_window<KT, false, false>(mid + c, MP, RY, yb + H, taps, o);
+#pragma unroll
+            for (int j = 0; j < ZB; ++j)
+                if (ty0 + yb + j < V) dst[slice + (size_t)(ty0 + yb + j) * V + x] = o[j];
+        }
+    } else {
+        for (int it = tid; it < W * (XY_TY / ZB); it += XY_THREADS) {         // y^T of every column, halo columns included
+            const int c = it % W, yb = (it / W) * ZB;
+            blur_window<KT, true, false>(in + c, P, RY, yb + H, taps, o);
+#pragma unroll
+            for (int j = 0; j < ZB; ++j) mid[(yb + j) * P + c] = o[j];
+        }
+        __syncthreads();
+        for (int it = tid; it < XY_TY * (XY_TX / ZB); it += XY_THREADS) {     // x^T, then the clamp mask
+            const int r = it % XY_TY, xb = (it / XY_TY) * ZB, y = ty0 + r;
+            if (y >= V) continue;
+            blur_window<KT, true, false>(mid + r * P, 1, P, xb + H, taps, o);
+#pragma unroll
+            for (int j = 0; j < ZB; ++j) {
+                const int x = tx0 + xb + j;
+                if (x < V) {
+                    const size_t i = slice + (size_t)y * V + x;
+                    const float g = raw[i];
+                    dst[i] = (g >= 0.f && g <= 1.f) ? o[j] : 0.f;
+                }
+            }
+        }
+    }
+}
+
+// patch [V][TY * TX] of grid G [B,V,V,V] at (ty0, tx0); cells outside the grid read as 0
+__device__ __forceinline__ void load_patch(const float* __restrict__ G, int b, int V, int ty0, int tx0, int ncol, float* A) {
+    for (int i = threadIdx.x; i < V * ncol; i += TILE_THREADS) {
+        const int z = i / ncol, c = i % ncol, y = ty0 + c / TX, x = tx0 + c % TX;
+        A[i] = (y < V && x < V) ? G[(((size_t)b * V + z) * V + y) * V + x] : 0.f;
+    }
+}
+
+// z blur + scale / clamp + ray march of grid B (mode P): the mode-R forward without its splat
+template <int KT>
+__global__ void __launch_bounds__(TILE_THREADS)
+pc_sil_p_fwd_kernel(const float* __restrict__ G, const Taps taps, const float* __restrict__ scale, int V, int TY,
+                    float* __restrict__ sil) {
+    extern __shared__ __align__(128) float sm[];
+    const int b = blockIdx.z, ty0 = blockIdx.y * TY, tx0 = blockIdx.x * TX;
+    const int ncol = TY * TX, nzb = (V + ZB - 1) / ZB;
+    float* A = sm;                       // [V][ncol]
+    float* blkP = A + V * ncol;          // [nzb][ncol]
+    float* blkS = blkP + nzb * ncol;     // [nzb][ncol]
+    load_patch(G, b, V, ty0, tx0, ncol, A);
+    __syncthreads();
+    const bool has_scale = scale != nullptr;
+    const float sc = has_scale ? scale[b] : 1.f;
+    // no sparsity skip: grid B is dense after the x / y blur, and no occupied-depth ranges are known here
+    sil_fwd_columns<KT, false>(A, blkP, blkS, nullptr, nullptr, false, taps, has_scale, sc, 1.f, b, V, ncol, ty0, tx0, sil);
+}
+
+// column adjoints of the above: grid B -> d(grid B), in place (the z direction is column-local); dscale accumulated
+template <int KT>
+__global__ void __launch_bounds__(TILE_THREADS)
+pc_sil_p_bwd_kernel(float* __restrict__ G, const Taps taps, const float* __restrict__ scale,
+                    const float* __restrict__ dsil, int V, int TY, float* __restrict__ dscale) {
+    extern __shared__ __align__(128) float sm[];
+    __shared__ float red[32];
+    const int b = blockIdx.z, ty0 = blockIdx.y * TY, tx0 = blockIdx.x * TX;
+    const int ncol = TY * TX, nzb = (V + ZB - 1) / ZB;
+    float* A1 = sm;                      // grid B -> d(grid B)
+    float* A2 = A1 + V * ncol;           // S -> dS
+    float* blkA = A2 + V * ncol;
+    float* blkB = blkA + nzb * ncol;
+    float* blkT = blkB + nzb * ncol;
+    load_patch(G, b, V, ty0, tx0, ncol, A1);
+    __syncthreads();
+    const bool has_scale = scale != nullptr;
+    const float sc = has_scale ? scale[b] : 1.f;
+    sil_bwd_columns<KT, false>(A1, A2, blkA, blkB, blkT, nullptr, nullptr, false, taps, has_scale, sc, 1.f, dsil, b, V, ncol,
+                               TX, TY, ty0, tx0, red, dscale);
+    for (int i = threadIdx.x; i < V * ncol; i += TILE_THREADS) {
+        const int z = i / ncol, c = i % ncol, y = ty0 + c / TX, x = tx0 + c % TX;
+        if (y < V && x < V) G[(((size_t)b * V + z) * V + y) * V + x] = A1[i];
+    }
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -621,19 +794,17 @@ __global__ void __launch_bounds__(NTHREADS) clamp01_kernel(float* __restrict__ x
 // ----------------------------------------------------------------------------------------------
 constexpr size_t SMEM_BUDGET = 210 * 1024;      // the patch, within the 227 KB a CTA may use
 
-size_t patch_bytes(int V, int ty, bool bwd) {
+// halo: the mode-R backward's +1 column halo (every point owned by one CTA); the mode-P kernels have none
+size_t patch_bytes(int V, int ty, bool bwd, bool halo) {
     const size_t nzb = (V + ZB - 1) / ZB;
-    if (bwd) {
-        const size_t ncol = (size_t)(ty + 1) * (TX + 1);
-        return 4 * (2 * V * ncol + 3 * nzb * ncol + 2 * ncol);
-    }
-    const size_t ncol = (size_t)ty * TX;
+    const size_t ncol = halo ? (size_t)(ty + 1) * (TX + 1) : (size_t)ty * TX;
+    if (bwd) return 4 * (2 * V * ncol + 3 * nzb * ncol + 2 * ncol);
     return 4 * (V * ncol + 2 * nzb * ncol + 2 * ncol);
 }
 
-int pick_ty(int V, bool bwd) {
+int pick_ty(int V, bool bwd, bool halo) {
     for (int ty = 16; ty >= 1; ty >>= 1)
-        if (patch_bytes(V, ty, bwd) <= SMEM_BUDGET) return ty;
+        if (patch_bytes(V, ty, bwd, halo) <= SMEM_BUDGET) return ty;
     return 0;
 }
 
@@ -658,9 +829,9 @@ int launch_sil_fwd(dim3 grid, size_t smem, cudaStream_t st, const float* sorted,
 
 int sil_fwd_impl(const float* sorted, const int32_t* bin_start, const Taps& t, const float* scale, int B, int N,
                  int V, int mode, float* sil, cudaStream_t st) {
-    const int TY = pick_ty(V, false);
+    const int TY = pick_ty(V, false, false);
     B3D_REQUIRE(TY > 0, B3D_EINVAL, "b3d_pc_silhouette_fwd: V=%d does not fit the shared-memory patch", V);
-    const size_t smem = patch_bytes(V, TY, false);
+    const size_t smem = patch_bytes(V, TY, false, false);
     dim3 grid(b3d::ceil_div(V, TX), b3d::ceil_div(V, TY), B);
     if (t.n == 21) return launch_sil_fwd<21>(grid, smem, st, sorted, bin_start, t, scale, N, V, TY, mode, sil);
     return launch_sil_fwd<0>(grid, smem, st, sorted, bin_start, t, scale, N, V, TY, mode, sil);
@@ -678,23 +849,93 @@ int launch_sil_bwd(dim3 grid, size_t smem, cudaStream_t st, const float* sorted,
 
 int sil_bwd_impl(const float* sorted, const int32_t* bin_start, const Taps& t, const float* scale,
                  const float* dsil, int B, int N, int V, int mode, float* dpg, float* dscale, cudaStream_t st) {
-    const int TY = pick_ty(V, true);
+    const int TY = pick_ty(V, true, true);
     B3D_REQUIRE(TY > 0, B3D_EINVAL, "b3d_pc_silhouette_bwd: V=%d does not fit the shared-memory patch", V);
-    const size_t smem = patch_bytes(V, TY, true);
+    const size_t smem = patch_bytes(V, TY, true, true);
     if (dscale) B3D_CUDA_OK(cudaMemsetAsync(dscale, 0, sizeof(float) * B, st));
     dim3 grid(b3d::ceil_div(V, TX), b3d::ceil_div(V, TY), B);
     if (t.n == 21) return launch_sil_bwd<21>(grid, smem, st, sorted, bin_start, t, scale, dsil, N, V, TY, mode, dpg, dscale);
     return launch_sil_bwd<0>(grid, smem, st, sorted, bin_start, t, scale, dsil, N, V, TY, mode, dpg, dscale);
 }
 
+// ---- mode P ------------------------------------------------------------------------------------
+template <bool ADJ>
+int launch_blur_xy(const float* src, const float* raw, float* dst, const Taps& t, int B, int V, cudaStream_t st) {
+    const int ntx = b3d::ceil_div(V, XY_TX);
+    const dim3 grid((unsigned)B * V, ntx * b3d::ceil_div(V, XY_TY));
+    const size_t smem = sizeof(float) * xy_tile_floats(t.n / 2);
+    if (t.n == 21) {
+        if (int rc = set_smem(pc_blur_xy_kernel<21, ADJ>, smem)) return rc;
+        pc_blur_xy_kernel<21, ADJ><<<grid, XY_THREADS, smem, st>>>(src, raw, dst, t, V, ntx);
+    } else {
+        if (int rc = set_smem(pc_blur_xy_kernel<0, ADJ>, smem)) return rc;
+        pc_blur_xy_kernel<0, ADJ><<<grid, XY_THREADS, smem, st>>>(src, raw, dst, t, V, ntx);
+    }
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+template <int KT>
+int launch_sil_p_fwd(dim3 grid, size_t smem, cudaStream_t st, const float* G, const Taps& t, const float* scale, int V,
+                     int TY, float* sil) {
+    if (int rc = set_smem(pc_sil_p_fwd_kernel<KT>, smem)) return rc;
+    pc_sil_p_fwd_kernel<KT><<<grid, TILE_THREADS, smem, st>>>(G, t, scale, V, TY, sil);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+template <int KT>
+int launch_sil_p_bwd(dim3 grid, size_t smem, cudaStream_t st, float* G, const Taps& t, const float* scale, const float* dsil,
+                     int V, int TY, float* dscale) {
+    if (int rc = set_smem(pc_sil_p_bwd_kernel<KT>, smem)) return rc;
+    pc_sil_p_bwd_kernel<KT><<<grid, TILE_THREADS, smem, st>>>(G, t, scale, dsil, V, TY, dscale);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+int sil_fwd_paper(const float* sorted, const int32_t* bin_start, const Taps& t, const float* scale, int B, int N, int V,
+                  float* sil, float* ws, cudaStream_t st) {
+    const int TY = pick_ty(V, false, false);
+    B3D_REQUIRE(TY > 0, B3D_EINVAL, "b3d_pc_silhouette_fwd: V=%d does not fit the shared-memory patch", V);
+    float* gA = ws;
+    float* gB = ws + (size_t)B * V * V * V;
+    if (int rc = b3d_vox_splat_sorted(sorted, bin_start, B, N, V, B3D_MODE_PAPER, gA, st)) return rc;
+    if (int rc = launch_blur_xy<false>(gA, nullptr, gB, t, B, V, st)) return rc;
+    const size_t smem = patch_bytes(V, TY, false, false);
+    const dim3 grid(b3d::ceil_div(V, TX), b3d::ceil_div(V, TY), B);
+    if (t.n == 21) return launch_sil_p_fwd<21>(grid, smem, st, gB, t, scale, V, TY, sil);
+    return launch_sil_p_fwd<0>(grid, smem, st, gB, t, scale, V, TY, sil);
+}
+
+int sil_bwd_paper(const float* sorted, const int32_t* bin_start, const Taps& t, const float* scale, const float* dsil, int B,
+                  int N, int V, float* dpg, float* dscale, float* ws, cudaStream_t st) {
+    const int TY = pick_ty(V, true, false);
+    B3D_REQUIRE(TY > 0, B3D_EINVAL, "b3d_pc_silhouette_bwd: V=%d does not fit the shared-memory patch", V);
+    float* gA = ws;
+    float* gB = ws + (size_t)B * V * V * V;
+    if (dscale) B3D_CUDA_OK(cudaMemsetAsync(dscale, 0, sizeof(float) * B, st));
+    const size_t smem = patch_bytes(V, TY, true, false);
+    const dim3 grid(b3d::ceil_div(V, TX), b3d::ceil_div(V, TY), B);
+    const int rc = t.n == 21 ? launch_sil_p_bwd<21>(grid, smem, st, gB, t, scale, dsil, V, TY, dscale)
+                             : launch_sil_p_bwd<0>(grid, smem, st, gB, t, scale, dsil, V, TY, dscale);
+    if (rc) return rc;
+    if (int rc2 = launch_blur_xy<true>(gB, gA, gA, t, B, V, st)) return rc2;
+    if (N == 0) return B3D_OK;
+    return b3d::vox_gather_launch(sorted, bin_start, gA, B, N, V, B3D_MODE_PAPER, dpg, st);
+}
+
 int check_sil_args(const char* who, const void* sorted, const void* bin_start, const void* taps, int ktaps, int B,
-                   int N, int V, int mode) {
+                   int N, int V, int mode, const void* workspace, size_t workspace_bytes) {
     B3D_REQUIRE(B >= 0 && N >= 0 && V >= 2, B3D_EINVAL, "%s: bad sizes B=%d N=%d V=%d", who, B, N, V);
     B3D_REQUIRE(ktaps >= 1 && ktaps <= MAX_TAPS && (ktaps & 1), B3D_EINVAL, "%s: ktaps=%d must be odd, <= %d", who,
                 ktaps, MAX_TAPS);
-    B3D_REQUIRE(mode == B3D_MODE_REFERENCE, B3D_EINVAL,
-                "%s: mode %d not available in this build (only B3D_MODE_REFERENCE)", who, mode);
+    B3D_REQUIRE(mode == B3D_MODE_REFERENCE || mode == B3D_MODE_PAPER, B3D_EINVAL, "%s: unknown mode %d", who, mode);
     B3D_REQUIRE(taps && (B == 0 || (bin_start && (sorted || N == 0))), B3D_EINVAL, "%s: null pointer", who);
+    const size_t need = b3d_pc_silhouette_workspace_bytes(B, V, mode);
+    B3D_REQUIRE(need == 0 || (workspace && workspace_bytes >= need), B3D_EINVAL,
+                "%s: mode %d needs a workspace of %zu bytes (got %s, %zu bytes)", who, mode, need,
+                workspace ? "a buffer" : "NULL", workspace_bytes);
+    if (need) B3D_CHECK_ALIGNED(workspace);
     return B3D_OK;
 }
 
@@ -750,28 +991,32 @@ size_t b3d_pc_silhouette_workspace_bytes(int B, int V, int mode) {
 int b3d_pc_silhouette_fwd_hosttaps(const float* sorted, const int32_t* bin_start, const float* taps_host, int ktaps,
                                    const float* scale, int B, int N, int V, int mode, float* sil, void* workspace,
                                    size_t workspace_bytes, void* stream) {
-    (void)workspace;
-    (void)workspace_bytes;
-    if (int rc = check_sil_args("b3d_pc_silhouette_fwd", sorted, bin_start, taps_host, ktaps, B, N, V, mode)) return rc;
+    if (int rc = check_sil_args("b3d_pc_silhouette_fwd", sorted, bin_start, taps_host, ktaps, B, N, V, mode, workspace,
+                                workspace_bytes))
+        return rc;
     if (B == 0) return B3D_OK;
     B3D_REQUIRE(sil, B3D_EINVAL, "b3d_pc_silhouette_fwd: null output");
     Taps t;
     fill_taps(t, taps_host, ktaps);
+    if (mode == B3D_MODE_PAPER)
+        return sil_fwd_paper(sorted, bin_start, t, scale, B, N, V, sil, (float*)workspace, (cudaStream_t)stream);
     return sil_fwd_impl(sorted, bin_start, t, scale, B, N, V, mode, sil, (cudaStream_t)stream);
 }
 
 int b3d_pc_silhouette_bwd_hosttaps(const float* sorted, const int32_t* bin_start, const float* taps_host, int ktaps,
                                    const float* scale, const float* dsil, int B, int N, int V, int mode, float* dpg,
                                    float* dscale, void* workspace, size_t workspace_bytes, void* stream) {
-    (void)workspace;
-    (void)workspace_bytes;
-    if (int rc = check_sil_args("b3d_pc_silhouette_bwd", sorted, bin_start, taps_host, ktaps, B, N, V, mode)) return rc;
+    if (int rc = check_sil_args("b3d_pc_silhouette_bwd", sorted, bin_start, taps_host, ktaps, B, N, V, mode, workspace,
+                                workspace_bytes))
+        return rc;
     if (B == 0) return B3D_OK;
     B3D_REQUIRE(dsil && (dpg || N == 0), B3D_EINVAL, "b3d_pc_silhouette_bwd: null pointer");
     B3D_REQUIRE((scale == nullptr) == (dscale == nullptr), B3D_EINVAL,
                 "b3d_pc_silhouette_bwd: scale and dscale must both be given or both be NULL");
     Taps t;
     fill_taps(t, taps_host, ktaps);
+    if (mode == B3D_MODE_PAPER)
+        return sil_bwd_paper(sorted, bin_start, t, scale, dsil, B, N, V, dpg, dscale, (float*)workspace, (cudaStream_t)stream);
     return sil_bwd_impl(sorted, bin_start, t, scale, dsil, B, N, V, mode, dpg, dscale, (cudaStream_t)stream);
 }
 

@@ -5,7 +5,8 @@
 //   vox_blur_axis     VoxelsSmooth.smooth, one separable kernel   utils/smooth_voxels.py:62-73 (zero padding)
 //   vox_scale_clamp   "* scale, clamp(0,1)"                         utils/smooth_voxels.py:80-82   (+ adjoint)
 //   vox_termination   termination_probs / silhouette               utils/effective_loss_function.py:18-56,79-81 (+ adjoint)
-//   vox_gather        adjoint of the trilinear splat: d/d(grid coords) from the 8 corners of dGrid
+//   vox_gather        adjoint of the trilinear splat: d/d(grid coords) from the 8 corners of dGrid (also the last step of
+//                     the fused mode-P silhouette backward, csrc/pc_kernels.cu)
 #include "b3d_common.cuh"
 
 namespace {
@@ -193,6 +194,16 @@ inline int capped(long long n) {
 }
 }  // namespace
 
+namespace b3d {
+int vox_gather_launch(const float* sorted, const int32_t* bin_start, const float* dgrid, int B, int N, int V, int mode,
+                      float* dpg, cudaStream_t st) {
+    vox_gather_kernel<<<dim3(blocks(N), B), NT, 0, st>>>((const float4*)sorted, bin_start, b3d_pc_bin_count(V), N, V, mode, dgrid,
+                                                        (float4*)dpg);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+}  // namespace b3d
+
 extern "C" {
 
 int b3d_vox_blur_axis(const float* in, float* out, const float* taps_host, int ktaps, int axis, int reversed, int B, int V,
@@ -283,9 +294,6 @@ int b3d_vox_gather(const float* sorted, const int32_t* bin_start, const float* r
     const long long cells = (long long)B * V * V * V;
     vox_mask01_kernel<<<capped(cells), NT, 0, st>>>(dgrid, raw, cells);
     B3D_LAUNCH_OK();
-    vox_gather_kernel<<<dim3(blocks(N), B), NT, 0, st>>>((const float4*)sorted, bin_start, b3d_pc_bin_count(V), N, V, mode, dgrid,
-                                                        (float4*)dpg);
-    B3D_LAUNCH_OK();
-    return B3D_OK;
+    return b3d::vox_gather_launch(sorted, bin_start, dgrid, B, N, V, mode, dpg, st);
 }
 }

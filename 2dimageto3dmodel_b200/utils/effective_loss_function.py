@@ -11,7 +11,7 @@ import torch.nn as nn
 
 from b3d import B3DError, mode_id
 from b3d import pointcloud as _pc
-from b3d.pointcloud import CAMERA_VIEW_DISTANCE, FIELD_OF_VIEW, effective_loss, effective_loss_dense, smoothing_taps
+from b3d.pointcloud import CAMERA_VIEW_DISTANCE, FIELD_OF_VIEW, effective_loss, smoothing_taps
 
 
 class EffectiveLossFunction(nn.Module):
@@ -47,9 +47,8 @@ class EffectiveLossFunction(nn.Module):
         inside; scale [B,1] or None.  Returns the projection [B,V,V] (differentiable)."""
         if point_cloud.dim() != 3 or point_cloud.size(-1) != 3:
             raise B3DError(f"point_cloud must be [B,N,3], got {tuple(point_cloud.shape)}")
-        fn = effective_loss if mode_id(self.semantics) == 0 else effective_loss_dense     # mode P needs the dense grid
-        return fn(point_cloud, rotation, scale, V=self.voxel_size, taps=self._current_taps(),
-                  mode=self.semantics, fov=FIELD_OF_VIEW, cam_dist=CAMERA_VIEW_DISTANCE)
+        return effective_loss(point_cloud, rotation, scale, V=self.voxel_size, taps=self._current_taps(),
+                              mode=self.semantics, fov=FIELD_OF_VIEW, cam_dist=CAMERA_VIEW_DISTANCE)
 
     def termination_probs(self, voxels, epsilon=1e-5):
         """Smoothed occupancies [B,V,V,V] -> ray-termination probabilities [B,V+1,V,V] (reference :18-56)."""

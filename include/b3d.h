@@ -76,14 +76,20 @@ B3D_API int b3d_pc_project(const float* points, const float* quat, int B, int N,
                            float cam_dist, float* pg, float* coords, int32_t* base, uint8_t* inb,
                            float* sorted, int32_t* bin_start, void* stream);
 
-/* Splat + z-blur + scale/clamp + ray termination + silhouette in ONE kernel (mode R): the V^3 grid lives
- * only in shared memory.
+/* Splat + blur + scale/clamp + ray termination + silhouette.
  *   TrilinearInterpolation.trilinear_interpolation / positions_update  utils/trilinear_interpolation.py:37-74
  *   VoxelsSmooth.smooth                                                utils/smooth_voxels.py:44-84
  *   EffectiveLossFunction.termination_probs + sum + flip               utils/effective_loss_function.py:18-56,79-81
- * (sorted, bin_start) from b3d_pc_project; taps [ktaps] the 1-D smoothing kernel (the host computes it with
- * the reference's expression, smooth_voxels.py:24-31); scale [B] nullable; sil [B,V,V] out.
- * workspace: b3d_pc_silhouette_workspace_bytes(B,V,mode) bytes (0 for mode R; may be NULL then).
+ * (sorted, bin_start) from b3d_pc_project; taps [ktaps] the 1-D smoothing kernel, ktaps odd <= 63 (the host computes it
+ * with the reference's expression, smooth_voxels.py:24-31); scale [B] nullable; sil [B,V,V] out.
+ * mode B3D_MODE_REFERENCE: ONE kernel, z blur only; the V^3 grid lives only in shared memory.
+ * mode B3D_MODE_PAPER: the blur runs along x, y and z, so the grid goes through the workspace (three launches:
+ *   splat, clamp + x/y blur, z blur + ray march; 4 full-grid transfers).
+ * workspace: b3d_pc_silhouette_workspace_bytes(B,V,mode) bytes, 16-byte aligned (0 for mode R, which ignores it and
+ *   takes NULL; 2*B*V^3 floats for mode P, where NULL or a smaller buffer returns B3D_EINVAL).  Mode P: the
+ *   forward leaves the grids in the workspace for the backward. Pass the same workspace to
+ *   b3d_pc_silhouette_bwd_hosttaps, unmodified, with the same sorted / bin_start / taps / scale. The backward
+ *   overwrites it with its gradients, so a second backward of the same forward needs the forward to be run again first.
  * The taps are read from HOST memory (no device->host read of 21 floats).                              */
 B3D_API size_t b3d_pc_silhouette_workspace_bytes(int B, int V, int mode);
 B3D_API int b3d_pc_silhouette_fwd_hosttaps(const float* sorted, const int32_t* bin_start,
@@ -92,7 +98,9 @@ B3D_API int b3d_pc_silhouette_fwd_hosttaps(const float* sorted, const int32_t* b
                                            size_t workspace_bytes, void* stream);
 
 /* Backward of the above: dsil [B,V,V] -> dpg [B,N,4] (d/d grid coords, indexed by ORIGINAL point index,
- * written for in-bounds points only; .w unused), dscale [B] (nullable iff scale is NULL; zeroed by the call). */
+ * written for in-bounds points only; .w unused), dscale [B] (nullable iff scale is NULL; zeroed by the call).
+ * Mode P: workspace is the one the forward filled (see above); three launches (column adjoints, x/y adjoints + clamp
+ * mask, gather; 5 full-grid transfers), after which the workspace holds gradients. */
 B3D_API int b3d_pc_silhouette_bwd_hosttaps(const float* sorted, const int32_t* bin_start,
                                            const float* taps_host, int ktaps, const float* scale,
                                            const float* dsil, int B, int N, int V, int mode, float* dpg,
@@ -106,7 +114,7 @@ B3D_API int b3d_pc_project_bwd(const float* points, const float* quat, const flo
 
 /* Materialised occupancy grid [B,V,V,V] (clamped to [0,1]) — the tensor
  * TrilinearInterpolation.trilinear_interpolation returns (trilinear_interpolation.py:74).
- * Used by mode P and by the parity tests; grid is zeroed by the call. */
+ * Used by the parity tests; grid is zeroed by the call. */
 B3D_API int b3d_pc_splat_grid(const float* pg, int B, int N, int V, int mode, float* grid, void* stream);
 
 /* ------------------------------------------------------------------------------------------

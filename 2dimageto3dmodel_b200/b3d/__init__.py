@@ -116,6 +116,11 @@ _sig("b3d_rgba_l1_bwd", _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp)
 _sig("b3d_mesh_render_bwd", _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp)
 _sig("b3d_gather_fields", _vp, _i, _vp, _vp, _i, _vp)
 _sig("b3d_image_batch", _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp)
+_sig("b3d_mesh_render_filtered_fwd", _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp)
+_sig("b3d_mesh_render_filtered_bwd", _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp)
+_sig("b3d_mesh_face_pack", _vp, _vp, _vp, _f, _i, _i, _vp, _vp)
+_sig("b3d_mesh_raster_attr_fwd", _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _f, _f, _vp, _vp, _vp, _vp, _vp)
+_sig("b3d_mesh_raster_attr_bwd", _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp)
 _sig("b3d_texel_visibility", _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp)
 _sig("b3d_pseudogt_pack", _vp, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp)
 _sig("b3d_sample_pack", _vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp)

@@ -49,11 +49,16 @@ def face_setup(verts, faces, uv=None, ft=None, want_normals=True):
     return fgeo, fuv, normal1
 
 
+# Renderer(filtering=...) -> B3D_FILTER_* of include/b3d.h (grid_sample's modes the shader kernels are built for)
+FILTERS = {"bilinear": 0, "nearest": 1, "bicubic": 2}
+
+
 class _Render(torch.autograd.Function):
-    """(vertices, uv, texture) -> (imout [B,H,W,3], improb [B,H,W,1], imidx [B,H,W] int32, normal1 [B,F,3])."""
+    """(vertices, uv, texture) -> (imout [B,H,W,3], improb [B,H,W,1], imidx [B,H,W] int32, normal1 [B,F,3]).
+    filt: B3D_FILTER_* id of the texture filter (ignored without a texture)."""
 
     @staticmethod
-    def forward(ctx, verts, uv, texture, faces, ft, background, H, W):
+    def forward(ctx, verts, uv, texture, faces, ft, background, H, W, filt=0):
         verts_d = dev(verts.detach(), "vertices")
         uv_d = uv.detach()
         fgeo, fuv, normal1 = face_setup(verts_d, faces, uv_d, ft)
@@ -71,11 +76,16 @@ class _Render(torch.autograd.Function):
         imwei = torch.empty(B, H, W, 3, device=d, dtype=torch.float32)
         imout = torch.empty(B, H, W, 3, device=d, dtype=torch.float32)
         improb = torch.empty(B, H, W, 1, device=d, dtype=torch.float32)
-        check(lib.b3d_mesh_render_fwd(ptr(fgeo), ptr(fuv), ptr(tex), ptr(bg), B, F, H, W, Th, Tw, ptr(imidx),
-                                      ptr(imwei), ptr(imout), ptr(improb), stream_ptr(verts_d)))
+        if tex is not None:
+            check(lib.b3d_mesh_render_filtered_fwd(ptr(fgeo), ptr(fuv), ptr(tex), ptr(bg), B, F, H, W, Th, Tw, filt,
+                                                   ptr(imidx), ptr(imwei), ptr(imout), ptr(improb), stream_ptr(verts_d)))
+        else:
+            check(lib.b3d_mesh_render_fwd(ptr(fgeo), ptr(fuv), None, None, B, F, H, W, 0, 0, ptr(imidx), ptr(imwei),
+                                          ptr(imout), ptr(improb), stream_ptr(verts_d)))
         ctx.save_for_backward(fgeo, fuv, tex if tex is not None else torch.empty(0), imidx, imwei,
                               _i32(faces, "faces"), _i32(faces if ft is None else ft, "face_textures"))
         ctx.cfg = (H, W, Th, Tw, tex is not None, bg is not None, verts.shape, uv.shape, uv.dim() == 3 and uv.stride(0) != 0)
+        ctx.filt = filt
         ctx.mark_non_differentiable(imidx, normal1)
         return imout, improb, imidx, normal1
 
@@ -90,9 +100,14 @@ class _Render(torch.autograd.Function):
         dfp2d = torch.empty(B, F, 6, device=d, dtype=torch.float32)
         dfuv = torch.empty(B, F, 6, device=d, dtype=torch.float32)
         dtex = torch.empty(B, 3, Th, Tw, device=d, dtype=torch.float32) if has_tex else None
-        check(lib.b3d_mesh_render_bwd(ptr(fgeo), ptr(fuv), ptr(tex) if has_tex else None, int(has_bg), B, F, H, W, Th,
-                                      Tw, ptr(imidx), ptr(imwei), ptr(d_imout), ptr(d_improb), ptr(dfp2d), ptr(dfuv),
-                                      ptr(dtex), stream_ptr(fgeo)))
+        if has_tex:
+            check(lib.b3d_mesh_render_filtered_bwd(ptr(fgeo), ptr(fuv), ptr(tex), int(has_bg), B, F, H, W, Th, Tw,
+                                                   ctx.filt, ptr(imidx), ptr(imwei), ptr(d_imout), ptr(d_improb),
+                                                   ptr(dfp2d), ptr(dfuv), ptr(dtex), stream_ptr(fgeo)))
+        else:
+            check(lib.b3d_mesh_render_bwd(ptr(fgeo), ptr(fuv), None, int(has_bg), B, F, H, W, Th, Tw, ptr(imidx),
+                                          ptr(imwei), ptr(d_imout), ptr(d_improb), ptr(dfp2d), ptr(dfuv), None,
+                                          stream_ptr(fgeo)))
         # scatter the per-face-corner gradients back to vertices / uvs (482 vertices: plumbing)
         dverts = torch.zeros(vshape, device=d, dtype=torch.float32)
         fl = faces.long()
@@ -108,13 +123,102 @@ class _Render(torch.autograd.Function):
             for i in range(3):
                 duv_b.index_add_(1, tl[:, i], gu[:, :, i])
             duv = duv_b if len(uvshape) == 3 and uv_batched else (duv_b.sum(0) if len(uvshape) == 2 else duv_b)
-        return dverts, duv, dtex, None, None, None, None, None
+        return dverts, duv, dtex, None, None, None, None, None, None
 
 
-def render(verts, faces, uv, texture, ft=None, background=None, H=256, W=256):
+def filter_id(filtering):
+    """grid_sample mode name -> B3D_FILTER_* id; ValueError for a mode the shader is not built for (as grid_sample)."""
+    try:
+        return FILTERS[filtering]
+    except (KeyError, TypeError):
+        raise ValueError(f"texture filtering must be one of {sorted(FILTERS)}, got {filtering!r}") from None
+
+
+def render(verts, faces, uv, texture, ft=None, background=None, H=256, W=256, filtering="bilinear"):
     if verts.dim() != 3 or verts.size(-1) != 3:
         raise B3DError(f"vertices must be [B,P,3], got {tuple(verts.shape)}")
-    return _Render.apply(verts, uv, texture, faces, ft, background, int(H), int(W))
+    return _Render.apply(verts, uv, texture, faces, ft, background, int(H), int(W), filter_id(filtering))
+
+
+# kaolin linear_rasterizer's keyword defaults (expand, knum, multiplier, delta)
+RASTER_DEFAULTS = (0.02, 30, 1000.0, 7000.0)
+
+
+def raster_params(expand=None, knum=None, multiplier=None, delta=None):
+    """kaolin's keyword arguments with its defaults filled in, checked as the C entry points check them."""
+    e, k, m, dl = (d if v is None else v for v, d in zip((expand, knum, multiplier, delta), RASTER_DEFAULTS))
+    if int(k) != k or k < 1:
+        raise B3DError(f"linear_rasterizer: knum={k}, need an integer >= 1")
+    if not m > 0 or not dl > 0 or not e >= 0:
+        raise B3DError(f"linear_rasterizer: need multiplier > 0, delta > 0, expand >= 0 (got {m}, {dl}, {e})")
+    return float(e), int(k), float(m), float(dl)
+
+
+class _RasterAttr(torch.autograd.Function):
+    """kaolin linear_rasterizer on its own inputs: (points3d [B,F,9], points2d [B,F,6], normalz [B,F,1], attr [B,F,3d])
+    -> (imfeat [B,H,W,d], improb [B,H,W,1], imidx [B,H,W] int32, imwei [B,H,W,3]).  Differentiable w.r.t. points2d and
+    attr; points3d / normalz get zero gradients (kaolin semantics)."""
+
+    @staticmethod
+    def forward(ctx, p3d, p2d, normalz, attr, H, W, params):
+        expand, knum, mult, delta = params
+        p3d_d = dev(p3d.detach(), "points3d")
+        p2d_d = dev(p2d.detach(), "points2d")
+        nz = dev(normalz.detach(), "normalz")
+        at = dev(attr.detach(), "vertex_attr")
+        B, F = p2d_d.shape[0], p2d_d.shape[1]
+        d = at.shape[2] // 3
+        dv = p2d_d.device
+        fgeo = torch.empty(B, F, 12, device=dv, dtype=torch.float32)
+        imidx = torch.empty(B, H, W, device=dv, dtype=torch.int32)
+        imwei = torch.empty(B, H, W, 3, device=dv, dtype=torch.float32)
+        imfeat = torch.empty(B, H, W, d, device=dv, dtype=torch.float32)
+        improb = torch.empty(B, H, W, 1, device=dv, dtype=torch.float32)
+        st = stream_ptr(p2d_d)
+        check(lib.b3d_mesh_face_pack(ptr(p3d_d), ptr(p2d_d), ptr(nz), mult, B, F, ptr(fgeo), st))
+        check(lib.b3d_mesh_raster_attr_fwd(ptr(fgeo), ptr(at), d, B, F, H, W, expand, knum, mult, delta, ptr(imidx),
+                                           ptr(imwei), ptr(imfeat), ptr(improb), st))
+        ctx.save_for_backward(fgeo, at, imidx, imwei)
+        ctx.cfg = (H, W, params, p3d.shape, normalz.shape)
+        ctx.mark_non_differentiable(imidx, imwei)
+        return imfeat, improb, imidx, imwei
+
+    @staticmethod
+    def backward(ctx, d_imfeat, d_improb, _d_idx, _d_wei):
+        fgeo, at, imidx, imwei = ctx.saved_tensors
+        H, W, (expand, knum, mult, delta), s3, sn = ctx.cfg
+        B, F, d = fgeo.shape[0], fgeo.shape[1], at.shape[2] // 3
+        dv = fgeo.device
+        d_imfeat = dev(d_imfeat, "grad imfeat") if d_imfeat is not None else torch.zeros(B, H, W, d, device=dv)
+        d_improb = dev(d_improb, "grad improb") if d_improb is not None else None
+        dp2d = torch.empty(B, F, 6, device=dv, dtype=torch.float32)
+        dattr = torch.empty(B, F, 3 * d, device=dv, dtype=torch.float32)
+        check(lib.b3d_mesh_raster_attr_bwd(ptr(fgeo), ptr(at), d, B, F, H, W, expand, knum, mult, delta, ptr(imidx),
+                                           ptr(imwei), ptr(d_imfeat), ptr(d_improb), ptr(dp2d), ptr(dattr),
+                                           stream_ptr(fgeo)))
+        d3 = torch.zeros(s3, device=dv) if ctx.needs_input_grad[0] else None
+        dn = torch.zeros(sn, device=dv) if ctx.needs_input_grad[2] else None
+        return d3, dp2d, dn, dattr, None, None, None
+
+
+def raster_attr(points3d, points2d, normalz, vertex_attr, H, W, expand=None, knum=None, multiplier=None, delta=None):
+    """kaolin linear_rasterizer(W, H, points3d, points2d, normalz, vertex_attr, expand, knum, multiplier, delta) with
+    the face-index and barycentric buffers: -> (imfeat [B,H,W,d], improb [B,H,W,1], imidx [B,H,W] int32 face + 1,
+    imwei [B,H,W,3])."""
+    params = raster_params(expand, knum, multiplier, delta)
+    if points2d.dim() != 3 or points2d.shape[2] != 6:
+        raise B3DError(f"linear_rasterizer: points2d must be [B,F,6], got {tuple(points2d.shape)}")
+    B, F = points2d.shape[0], points2d.shape[1]
+    if tuple(points3d.shape) != (B, F, 9):
+        raise B3DError(f"linear_rasterizer: points3d must be [{B},{F},9], got {tuple(points3d.shape)}")
+    if tuple(normalz.shape) != (B, F, 1):
+        raise B3DError(f"linear_rasterizer: normalz must be [{B},{F},1], got {tuple(normalz.shape)}")
+    if vertex_attr.dim() != 3 or tuple(vertex_attr.shape[:2]) != (B, F) or vertex_attr.shape[2] < 3 \
+            or vertex_attr.shape[2] % 3:
+        raise B3DError(f"linear_rasterizer: vertex_attr must be [{B},{F},3d] with d >= 1, got {tuple(vertex_attr.shape)}")
+    if int(H) < 1 or int(W) < 1:
+        raise B3DError(f"linear_rasterizer: bad image size {H} x {W}")
+    return _RasterAttr.apply(points3d, points2d, normalz, vertex_attr, int(H), int(W), params)
 
 
 @torch.no_grad()

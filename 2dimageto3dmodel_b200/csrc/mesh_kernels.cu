@@ -10,9 +10,17 @@
 //                            compaction (face order decides z ties and the knum cap), stages the binned face
 //                            records through shared memory and walks only those: ~20 tests per pixel, not 960.
 //   mesh_raster_bwd_kernel   adjoint: gradients to the 2-D vertices (barycentrics of the covering face +
-//                            soft-silhouette distances), to the per-face UVs and to the texture.  Per-face
-//                            gradients are accumulated in shared memory per tile and flushed once; the
+//                            soft-silhouette distances), to the per-face UVs / attributes and to the texture.
+//                            Per-face gradients are accumulated in shared memory per tile and flushed once; the
 //                            knum x 5 per-pixel side buffers kaolin stores are recomputed instead.
+//   mesh_face_pack_kernel    the same per-face record from kaolin's own inputs (points3d depths, points2d x
+//                            multiplier, normalz) for the stand-alone `linear_rasterizer`.
+//
+// One rasteriser, five outputs (the MODE template parameter): OUT_UV (interpolated (u, v, hard mask), what
+// Renderer's rasteriser call returns), OUT_ATTR (any number d of per-vertex attributes, kaolin's imfeat) and the
+// shaded image with grid_sample's bilinear (align_corners=True), nearest or bicubic (align_corners=False) filters.
+// The raster parameters (multiplier, expand, delta, knum) are run-time values; the Renderer entry points pass kaolin's
+// defaults.
 //
 // Index buffer (imidx) arithmetic uses round-to-nearest intrinsics in the oracle's operation order so that
 // the face-index / visibility buffers are reproduced bit for bit.
@@ -24,14 +32,51 @@ constexpr int TILE = 16;
 constexpr int NT = TILE * TILE;
 constexpr int CHUNK = 64;          // face records staged per step
 constexpr int CAPN = 768;          // per-tile shared-memory accumulators (faces beyond use global atomics)
-constexpr float MULT = 1000.f;     // kaolin default `multiplier`
-constexpr float EXPAND = 0.02f * 1000.f;
-constexpr float DELTA = 7000.f;
-constexpr int KNUM = 30;
 constexpr float DEPTH_INIT = -1000.f;
 constexpr float BARY_EPS = 1e-10f;
 constexpr float SEG_EPS = 1e-10f;
 constexpr float NORMAL_EPS = 1e-8f;
+
+// kaolin linear_rasterizer's keyword arguments, as the kernels use them
+struct RasterParams {
+    float mult;      // `multiplier`: 2-D coordinates are scaled by it before every test
+    float expand;    // `expand` x multiplier: bounding-box margin of the soft-silhouette faces
+    float delta;     // `delta`: sharpness of the soft silhouette
+    float mm;        // multiplier^2
+    float inv_mm;    // RN(1 / multiplier^2)
+    float slope;     // RN(-delta / multiplier^2)
+    int knum;        // at most this many faces (in face order) shape an uncovered pixel's soft silhouette
+    float sx, sy;    // pixel pitches RN(multiplier / W), RN(multiplier / H)
+};
+// The kernels take the parameters as scalars (a by-value struct parameter costs the existing instantiations registers
+// and spills) and rebuild the struct in registers.
+#define RASTER_PARAMS float rp_mult, float rp_expand, float rp_delta, float rp_mm, float rp_inv_mm, float rp_slope, \
+                      int rp_knum, float rp_sx, float rp_sy
+#define RASTER_PARAMS_LOCAL const RasterParams rp{rp_mult, rp_expand, rp_delta, rp_mm, rp_inv_mm, rp_slope, rp_knum, rp_sx, rp_sy}
+#define RASTER_PARAMS_ARGS(p) p.mult, p.expand, p.delta, p.mm, p.inv_mm, p.slope, p.knum, p.sx, p.sy
+// kaolin's defaults (renderer.py:60-67 passes none): expand 0.02, knum 30, multiplier 1000, delta 7000
+constexpr float DEFAULT_MULT = 1000.f;
+RasterParams make_params(float mult, float expand_scaled, float delta, int knum) {
+    const float mm = mult * mult;
+    return RasterParams{mult, expand_scaled, delta, mm, 1.f / mm, -delta / mm, knum, 0.f, 0.f};
+}
+RasterParams default_params() { return make_params(DEFAULT_MULT, 0.02f * DEFAULT_MULT, 7000.f, 30); }
+
+// x / multiplier^2, correctly rounded (Markstein: q = RN(x * RN(1/m)), one fma residual step) for the x = -delta * d2 of
+// the soft silhouette: the same value as the division, without the division's slow-path call inside the face loops
+__device__ __forceinline__ float div_mm(float x, const RasterParams& rp) {
+    const float q = __fmul_rn(x, rp.inv_mm);
+    return __fmaf_rn(__fmaf_rn(-q, rp.mm, x), rp.inv_mm, q);
+}
+
+// what the rasteriser writes to imout
+enum : int {
+    OUT_UV = 0,          // (u, v, hard mask) from fuv [B,F,6]
+    OUT_ATTR = 1,        // d interpolated attributes from attr [B,F,3d]
+    OUT_BILINEAR = 2,    // shaded, grid_sample bilinear, align_corners=True (fragment_shader.py's own helper)
+    OUT_NEAREST = 3,     // shaded, grid_sample nearest, align_corners=False, zero padding
+    OUT_BICUBIC = 4,     // shaded, grid_sample bicubic, align_corners=False, zero padding
+};
 
 __device__ __forceinline__ float mul(float a, float b) { return __fmul_rn(a, b); }
 __device__ __forceinline__ float add(float a, float b) { return __fadd_rn(a, b); }
@@ -69,6 +114,7 @@ mesh_face_setup_kernel(const float* __restrict__ verts, const int32_t* __restric
     const float ny = __fmaf_rn(e1z, e2x, -mul(e1x, e2z));
     const float nz = __fmaf_rn(e1x, e2y, -mul(e1y, e2x));
     float4* g = fgeo + ((size_t)b * F + f) * 3;
+    constexpr float MULT = DEFAULT_MULT;
     g[0] = make_float4(mul(MULT, v[0][0]), mul(MULT, v[0][1]), mul(MULT, v[1][0]), mul(MULT, v[1][1]));
     g[1] = make_float4(mul(MULT, v[2][0]), mul(MULT, v[2][1]), v[0][2], v[1][2]);
     g[2] = make_float4(v[2][2], nz, 0.f, 0.f);
@@ -90,9 +136,26 @@ mesh_face_setup_kernel(const float* __restrict__ verts, const int32_t* __restric
     }
 }
 
+// kaolin's inputs as given: points3d [B,F,9] (only the depths are read), points2d [B,F,6], normalz [B,F,1]
+__global__ void __launch_bounds__(NT)
+mesh_face_pack_kernel(const float* __restrict__ p3d, const float* __restrict__ p2d, const float* __restrict__ normalz,
+                      float mult, int F, float4* __restrict__ fgeo) {
+    const int b = blockIdx.y;
+    const int f = blockIdx.x * NT + threadIdx.x;
+    if (f >= F) return;
+    const size_t bf = (size_t)b * F + f;
+    const float* q = p2d + bf * 6;
+    const float* z = p3d + bf * 9;
+    float4* g = fgeo + bf * 3;
+    g[0] = make_float4(mul(mult, q[0]), mul(mult, q[1]), mul(mult, q[2]), mul(mult, q[3]));
+    g[1] = make_float4(mul(mult, q[4]), mul(mult, q[5]), z[2], z[5]);
+    g[2] = make_float4(z[8], normalz[bf], 0.f, 0.f);
+}
+
 // pixel centres, SURVEY App. B step 2 (row 0 is the top of the image)
-__device__ __forceinline__ float centre_x(int x, int W) { return mul(__fdiv_rn(MULT, (float)W), (float)(2 * x + 1 - W)); }
-__device__ __forceinline__ float centre_y(int y, int H) { return mul(__fdiv_rn(MULT, (float)H), (float)(H - 2 * y - 1)); }
+// sx = RN(m / W), sy = RN(m / H): the pixel pitches, divided on the host
+__device__ __forceinline__ float centre_x(int x, int W, float sx) { return mul(sx, (float)(2 * x + 1 - W)); }
+__device__ __forceinline__ float centre_y(int y, int H, float sy) { return mul(sy, (float)(H - 2 * y - 1)); }
 
 struct Bary {
     float w0, w1, w2, k3;
@@ -126,7 +189,7 @@ struct TileCtx {
 // Order-preserving compaction of the faces whose expanded bounding box touches the tile.
 // list[] receives face ids in increasing order; posof (optional) maps face -> list position.
 __device__ __forceinline__ int bin_faces(const float4* __restrict__ fg, int F, float x0lo, float x0hi, float y0lo,
-                                         float y0hi, int* list, int* posof, int* warp_cnt) {
+                                         float y0hi, float EXPAND, int* list, int* posof, int* warp_cnt) {
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
     int count = 0;
     for (int base = 0; base < F; base += NT) {
@@ -199,26 +262,61 @@ __device__ __forceinline__ TapWeights tap_weights(float g, const TexTap& tp) {
     return TapWeights{g * wx0 * wy0, g * tp.wx1 * wy0, g * wx0 * tp.wy1, g * tp.wx1 * tp.wy1};
 }
 
-template <bool SHADE>
+// grid_sample with align_corners=False: the unnormalised coordinate ((g + 1) * size - 1) / 2, evaluated as torch's CPU
+// kernel does, (g + 1) * (size / 2) - 0.5, on g = u * 2 - 1 (x) or -(v * 2 - 1) (y, the shader's flip)
+__device__ __forceinline__ float unnorm_x(float u, int Tw) {
+    return __fsub_rn(__fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(u, 2.f), 1.f), 1.f), 0.5f * (float)Tw), 0.5f);
+}
+__device__ __forceinline__ float unnorm_y(float v, int Th) {
+    return __fsub_rn(__fmul_rn(__fadd_rn(-__fsub_rn(__fmul_rn(v, 2.f), 1.f), 1.f), 0.5f * (float)Th), 0.5f);
+}
+
+// grid_sample's cubic convolution weights (A = -0.75) of the taps floor(x) - 1 .. floor(x) + 2 at fraction t, and their
+// derivatives d/dt
+constexpr float CUBIC_A = -0.75f;
+__device__ __forceinline__ float cubic1(float x) { return ((CUBIC_A + 2.f) * x - (CUBIC_A + 3.f)) * x * x + 1.f; }
+__device__ __forceinline__ float cubic2(float x) {
+    return ((CUBIC_A * x - 5.f * CUBIC_A) * x + 8.f * CUBIC_A) * x - 4.f * CUBIC_A;
+}
+__device__ __forceinline__ float dcubic1(float x) { return (3.f * (CUBIC_A + 2.f) * x - 2.f * (CUBIC_A + 3.f)) * x; }
+__device__ __forceinline__ float dcubic2(float x) { return (3.f * CUBIC_A * x - 10.f * CUBIC_A) * x + 8.f * CUBIC_A; }
+__device__ __forceinline__ void cubic_weights(float t, float (&c)[4]) {
+    c[0] = cubic2(t + 1.f);
+    c[1] = cubic1(t);
+    c[2] = cubic1(1.f - t);
+    c[3] = cubic2(2.f - t);
+}
+__device__ __forceinline__ void cubic_dweights(float t, float (&c)[4]) {
+    c[0] = dcubic2(t + 1.f);
+    c[1] = dcubic1(t);
+    c[2] = -dcubic1(1.f - t);
+    c[3] = -dcubic2(2.f - t);
+}
+
+template <int MODE>
 __global__ void __launch_bounds__(NT)
-mesh_raster_fwd_kernel(const float4* __restrict__ fgeo, const float* __restrict__ fuv, const float* __restrict__ tex,
-                       const float* __restrict__ bg, int F, int H, int W, int Th, int Tw,
+mesh_raster_fwd_kernel(const float4* __restrict__ fgeo, const float* __restrict__ fuv, int d, const float* __restrict__ tex,
+                       const float* __restrict__ bg, RASTER_PARAMS, int F, int H, int W, int Th, int Tw,
                        int32_t* __restrict__ imidx, float* __restrict__ imwei, float* __restrict__ imout,
                        float* __restrict__ improb) {
+    constexpr bool SHADE = MODE >= OUT_BILINEAR;
+    RASTER_PARAMS_LOCAL;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float4* stage = reinterpret_cast<float4*>(smem_raw);
     int* list = reinterpret_cast<int*>(stage + CHUNK * 3);
     __shared__ int warp_cnt[NT / 32];
 
+    const float MULT = rp.mult, EXPAND = rp.expand, DELTA = rp.delta;
     const int b = blockIdx.z, tid = threadIdx.x;
     const int tx0 = blockIdx.x * TILE, ty0 = blockIdx.y * TILE;
     const int px = tx0 + (tid & (TILE - 1)), py = ty0 + (tid >> 4);
     const bool valid = px < W && py < H;
-    const float x0 = centre_x(px, W), y0 = centre_y(py, H);
+    const float x0 = centre_x(px, W, rp.sx), y0 = centre_y(py, H, rp.sy);
     const float4* fg = fgeo + (size_t)b * F * 3;
 
-    const int nlist = bin_faces(fg, F, centre_x(tx0, W), centre_x(min(tx0 + TILE - 1, W - 1), W),
-                                centre_y(min(ty0 + TILE - 1, H - 1), H), centre_y(ty0, H), list, nullptr, warp_cnt);
+    const int nlist = bin_faces(fg, F, centre_x(tx0, W, rp.sx), centre_x(min(tx0 + TILE - 1, W - 1), W, rp.sx),
+                                centre_y(min(ty0 + TILE - 1, H - 1), H, rp.sy), centre_y(ty0, H, rp.sy), EXPAND, list,
+                                nullptr, warp_cnt);
 
     // pass A: nearest front-facing face containing the pixel centre
     int best = -1;
@@ -249,7 +347,7 @@ mesh_raster_fwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
         __syncthreads();
     }
 
-    // pass B: soft silhouette of the uncovered pixels (first KNUM faces, in face order, whose expanded
+    // pass B: soft silhouette of the uncovered pixels (first knum faces, in face order, whose expanded
     // bounding box contains the pixel)
     float keep = 1.f;
     if (__syncthreads_or(valid && best < 0)) {
@@ -259,7 +357,7 @@ mesh_raster_fwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
             stage_faces(fg, list, c0, n, stage);
             __syncthreads();
             if (valid && best < 0) {
-                for (int j = 0; j < n && cnt < KNUM; ++j) {
+                for (int j = 0; j < n && cnt < rp.knum; ++j) {
                     const Face f = unpack(stage[3 * j], stage[3 * j + 1], stage[3 * j + 2]);
                     const float xmin = min3(f.ax, f.bx, f.cx), xmax = max3(f.ax, f.bx, f.cx);
                     const float ymin = min3(f.ay, f.by, f.cy), ymax = max3(f.ay, f.by, f.cy);
@@ -270,7 +368,7 @@ mesh_raster_fwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
                     const float d2 = fminf(fminf(seg_dist2(x0, y0, f.ax, f.ay, f.bx, f.by, t, rx, ry),
                                                  seg_dist2(x0, y0, f.bx, f.by, f.cx, f.cy, t, rx, ry)),
                                            seg_dist2(x0, y0, f.cx, f.cy, f.ax, f.ay, t, rx, ry));
-                    keep *= 1.f - expf(-DELTA * d2 / (MULT * MULT));
+                    keep *= 1.f - expf(div_mm(-DELTA * d2, rp));
                     ++cnt;
                 }
             }
@@ -285,20 +383,53 @@ mesh_raster_fwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
     imwei[3 * pix + 1] = bw1;
     imwei[3 * pix + 2] = bw2;
     improb[pix] = best >= 0 ? 1.f : 1.f - keep;
+    if constexpr (MODE == OUT_ATTR) {
+        // imfeat = sum_i w_i attr_i[0..d) on covered pixels, 0 on the background
+        float* o = imout + pix * d;
+        const float* a = fuv + ((size_t)b * F + max(best, 0)) * 3 * d;
+        for (int k = 0; k < d; ++k) o[k] = best >= 0 ? bw0 * a[k] + bw1 * a[d + k] + bw2 * a[2 * d + k] : 0.f;
+        return;
+    }
     float o0 = 0.f, o1 = 0.f, o2 = 0.f;
     if (best >= 0) {
         const ShadePoint sp = shade_point(bw0, bw1, bw2, fuv + ((size_t)b * F + best) * 6);
         const float u = sp.u, v = sp.v, msum = sp.msum;
-        if (SHADE) {
-            const TexTap tp = tex_tap(u, v, Th, Tw);
-            const float wx0 = 1.f - tp.wx1, wy0 = 1.f - tp.wy1;
+        if constexpr (SHADE) {
             float col[3];
+            if constexpr (MODE == OUT_BILINEAR) {
+                const TexTap tp = tex_tap(u, v, Th, Tw);
+                const float wx0 = 1.f - tp.wx1, wy0 = 1.f - tp.wy1;
 #pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const float* t = tex + ((size_t)b * 3 + c) * Th * Tw;
-                col[c] = (tex_at(t, tp.y0, tp.x0, Th, Tw) * wx0 + tex_at(t, tp.y0, tp.x0 + 1, Th, Tw) * tp.wx1) * wy0 +
-                         (tex_at(t, tp.y0 + 1, tp.x0, Th, Tw) * wx0 + tex_at(t, tp.y0 + 1, tp.x0 + 1, Th, Tw) * tp.wx1) *
-                             tp.wy1;
+                for (int c = 0; c < 3; ++c) {
+                    const float* t = tex + ((size_t)b * 3 + c) * Th * Tw;
+                    col[c] = (tex_at(t, tp.y0, tp.x0, Th, Tw) * wx0 + tex_at(t, tp.y0, tp.x0 + 1, Th, Tw) * tp.wx1) * wy0 +
+                             (tex_at(t, tp.y0 + 1, tp.x0, Th, Tw) * wx0 + tex_at(t, tp.y0 + 1, tp.x0 + 1, Th, Tw) * tp.wx1) *
+                                 tp.wy1;
+                }
+            } else if constexpr (MODE == OUT_NEAREST) {
+                const int xi = __float2int_rn(unnorm_x(u, Tw)), yi = __float2int_rn(unnorm_y(v, Th));  // half to even
+#pragma unroll
+                for (int c = 0; c < 3; ++c) col[c] = tex_at(tex + ((size_t)b * 3 + c) * Th * Tw, yi, xi, Th, Tw);
+            } else {
+                const float ix = unnorm_x(u, Tw), iy = unnorm_y(v, Th);
+                const float fx = floorf(ix), fy = floorf(iy);
+                const int xs = (int)fx - 1, ys = (int)fy - 1;
+                float cx[4], cy[4];
+                cubic_weights(ix - fx, cx);
+                cubic_weights(iy - fy, cy);
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    const float* t = tex + ((size_t)b * 3 + c) * Th * Tw;
+                    float acc = 0.f;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        float row = 0.f;
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) row += cx[j] * tex_at(t, ys + i, xs + j, Th, Tw);
+                        acc += cy[i] * row;
+                    }
+                    col[c] = acc;
+                }
             }
             if (bg) {
                 const float* g = bg + 3 * pix;
@@ -325,10 +456,12 @@ mesh_raster_fwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
     imout[3 * pix + 2] = o2;
 }
 
-__device__ __forceinline__ void acc_add(float* acc, int pos, int k, float v, float* gdst) {
+// Per-face adjoints live in shared memory as NSLOT floats per binned face: slots 0-5 the 2-D vertices, the rest the
+// per-vertex uvs (6) or attributes (3d).  Faces past the first `capn` of the tile's list go to global atomics.
+__device__ __forceinline__ void acc_add(float* acc, int pos, int k, float v, float* gdst, int nslot, int capn) {
     if (v == 0.f) return;
-    if (pos < CAPN)
-        atomicAdd(acc + pos * 12 + k, v);
+    if (pos < capn)
+        atomicAdd(acc + pos * nslot + k, v);
     else
         atomicAdd(gdst, v);
 }
@@ -351,19 +484,44 @@ __device__ __forceinline__ void warp_face_acc(float* acc, int fidx, int pos, con
             const float v = b3d::warp_sum(mine ? vals[k] : 0.f);
             if (lane == leader) {
                 const int kk = k0 + k;
-                acc_add(acc, pos, kk, v, kk < 6 ? gdst6a + key * 6 + kk : gdst6b + key * 6 + (kk - 6));
+                acc_add(acc, pos, kk, v, kk < 6 ? gdst6a + key * 6 + kk : gdst6b + key * 6 + (kk - 6), 12, CAPN);
             }
         }
     }
 }
 
-template <bool SHADE>
+// The same for the attribute adjoint w_i * g[k] (i < 3, k < d) of OUT_ATTR: slot 6 + i*d + k, global dattr [F,3d].
+__device__ __forceinline__ void warp_face_acc_attr(float* acc, int fidx, int pos, const float* g, float w0, float w1,
+                                                   float w2, int d, float* gattr, int capn) {
+    const int lane = threadIdx.x & 31, nslot = 6 + 3 * d;
+    unsigned todo = __ballot_sync(0xffffffffu, fidx >= 0);
+    while (todo) {
+        const int leader = __ffs(todo) - 1;
+        const int key = __shfl_sync(0xffffffffu, fidx, leader);
+        const bool mine = fidx == key;
+        todo &= ~__ballot_sync(0xffffffffu, mine);
+        for (int k = 0; k < d; ++k) {
+            const float gk = mine ? g[k] : 0.f;
+            const float v0 = b3d::warp_sum(w0 * gk), v1 = b3d::warp_sum(w1 * gk), v2 = b3d::warp_sum(w2 * gk);
+            if (lane == leader) {
+                float* ga = gattr + (size_t)key * 3 * d + k;
+                acc_add(acc, pos, 6 + k, v0, ga, nslot, capn);
+                acc_add(acc, pos, 6 + d + k, v1, ga + d, nslot, capn);
+                acc_add(acc, pos, 6 + 2 * d + k, v2, ga + 2 * d, nslot, capn);
+            }
+        }
+    }
+}
+
+template <int MODE>
 __global__ void __launch_bounds__(NT)
-mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict__ fuv, const float* __restrict__ tex,
-                       int has_bg, int F, int H, int W, int Th, int Tw, const int32_t* __restrict__ imidx,
-                       const float* __restrict__ imwei, const float* __restrict__ d_imout,
-                       const float* __restrict__ d_improb, float* __restrict__ dfp2d, float* __restrict__ dfuv,
-                       float* __restrict__ dtex) {
+mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict__ fuv, int d, const float* __restrict__ tex,
+                       int has_bg, RASTER_PARAMS, int F, int H, int W, int Th, int Tw,
+                       const int32_t* __restrict__ imidx, const float* __restrict__ imwei,
+                       const float* __restrict__ d_imout, const float* __restrict__ d_improb, float* __restrict__ dfp2d,
+                       float* __restrict__ dfuv, float* __restrict__ dtex) {
+    constexpr bool SHADE = MODE >= OUT_BILINEAR;
+    RASTER_PARAMS_LOCAL;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float4* stage = reinterpret_cast<float4*>(smem_raw);
     float* acc = reinterpret_cast<float*>(stage + CHUNK * 3);
@@ -371,18 +529,23 @@ mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
     int* posof = list + F;
     __shared__ int warp_cnt[NT / 32];
 
+    const float MULT = rp.mult, EXPAND = rp.expand, DELTA = rp.delta;
+    // per-face slots in `acc`: 12 (2-D vertices + uvs), or 6 + 3d with d attributes (fewer faces fit)
+    const int nslot = MODE == OUT_ATTR ? 6 + 3 * d : 12;
+    const int capn = MODE == OUT_ATTR ? CAPN * 12 / nslot : CAPN;
     const int b = blockIdx.z, tid = threadIdx.x;
     const int tx0 = blockIdx.x * TILE, ty0 = blockIdx.y * TILE;
     const int px = tx0 + (tid & (TILE - 1)), py = ty0 + (tid >> 4);
     const bool valid = px < W && py < H;
-    const float x0 = centre_x(px, W), y0 = centre_y(py, H);
+    const float x0 = centre_x(px, W, rp.sx), y0 = centre_y(py, H, rp.sy);
     const float4* fg = fgeo + (size_t)b * F * 3;
     float* gp = dfp2d + (size_t)b * F * 6;
-    float* gu = dfuv + (size_t)b * F * 6;
+    float* gu = dfuv + (size_t)b * F * (MODE == OUT_ATTR ? 3 * d : 6);
 
-    const int nlist = bin_faces(fg, F, centre_x(tx0, W), centre_x(min(tx0 + TILE - 1, W - 1), W),
-                                centre_y(min(ty0 + TILE - 1, H - 1), H), centre_y(ty0, H), list, posof, warp_cnt);
-    const int nacc = min(nlist, CAPN) * 12;
+    const int nlist = bin_faces(fg, F, centre_x(tx0, W, rp.sx), centre_x(min(tx0 + TILE - 1, W - 1), W, rp.sx),
+                                centre_y(min(ty0 + TILE - 1, H - 1), H, rp.sy), centre_y(ty0, H, rp.sy), EXPAND, list,
+                                posof, warp_cnt);
+    const int nacc = min(nlist, capn) * nslot;
     for (int i = tid; i < nacc; i += NT) acc[i] = 0.f;
     __syncthreads();
 
@@ -393,57 +556,138 @@ mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
     float cv[12];
 #pragma unroll
     for (int k = 0; k < 12; ++k) cv[k] = 0.f;
+    bool coord_grad = fidx >= 0;          // nearest filtering: no gradient to the sampling point
     if (fidx >= 0) {
-        const float g0 = d_imout[3 * pix], g1 = d_imout[3 * pix + 1], g2 = d_imout[3 * pix + 2];
         const float w0 = imwei[3 * pix], w1 = imwei[3 * pix + 1], w2 = imwei[3 * pix + 2];
-        const float* a = fuv + ((size_t)b * F + fidx) * 6;
-        float du, dv;
-        if (SHADE) {
-            const ShadePoint sp = shade_point(w0, w1, w2, a);
-            const float msum = sp.msum;
-            const TexTap tp = tex_tap(sp.u, sp.v, Th, Tw);
-            const float wx0 = 1.f - tp.wx1, wy0 = 1.f - tp.wy1;
-            const float g[3] = {g0 * msum, g1 * msum, g2 * msum};      // colour = tex * mask (or lerp)
-            float sx = 0.f, sy = 0.f;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const float* t = tex + ((size_t)b * 3 + c) * Th * Tw;
-                float* dt = dtex + ((size_t)b * 3 + c) * Th * Tw;
-                const float t00 = tex_at(t, tp.y0, tp.x0, Th, Tw), t01 = tex_at(t, tp.y0, tp.x0 + 1, Th, Tw);
-                const float t10 = tex_at(t, tp.y0 + 1, tp.x0, Th, Tw), t11 = tex_at(t, tp.y0 + 1, tp.x0 + 1, Th, Tw);
-                sx += g[c] * ((t01 - t00) * wy0 + (t11 - t10) * tp.wy1);
-                sy += g[c] * ((t10 - t00) * wx0 + (t11 - t01) * tp.wx1);
-                if (g[c] != 0.f) {
-                    const bool xa = tp.x0 >= 0 && tp.x0 < Tw, xb = tp.x0 + 1 >= 0 && tp.x0 + 1 < Tw;
-                    const bool ya = tp.y0 >= 0 && tp.y0 < Th, yb = tp.y0 + 1 >= 0 && tp.y0 + 1 < Th;
-                    // the same products as tap_weights (texel_visibility_kernel marks the taps where they are > 0)
-                    if (ya && xa) atomicAdd(dt + (size_t)tp.y0 * Tw + tp.x0, g[c] * wx0 * wy0);
-                    if (ya && xb) atomicAdd(dt + (size_t)tp.y0 * Tw + tp.x0 + 1, g[c] * tp.wx1 * wy0);
-                    if (yb && xa) atomicAdd(dt + (size_t)(tp.y0 + 1) * Tw + tp.x0, g[c] * wx0 * tp.wy1);
-                    if (yb && xb) atomicAdd(dt + (size_t)(tp.y0 + 1) * Tw + tp.x0 + 1, g[c] * tp.wx1 * tp.wy1);
-                }
+        const float* a = fuv + ((size_t)b * F + fidx) * (MODE == OUT_ATTR ? 3 * d : 6);
+        float du = 0.f, dv = 0.f, dw0, dw1, dw2;
+        if constexpr (MODE == OUT_ATTR) {
+            // d/dw_i of sum_k g_k (sum_i w_i attr_i[k])
+            const float* g = d_imout + pix * d;
+            dw0 = 0.f, dw1 = 0.f, dw2 = 0.f;
+            for (int k = 0; k < d; ++k) {
+                dw0 += g[k] * a[k];
+                dw1 += g[k] * a[d + k];
+                dw2 += g[k] * a[2 * d + k];
             }
-            du = sx * (float)(Tw - 1);
-            dv = -sy * (float)(Th - 1);
         } else {
-            du = g0;
-            dv = g1;
+            const float g0 = d_imout[3 * pix], g1 = d_imout[3 * pix + 1], g2 = d_imout[3 * pix + 2];
+            if constexpr (SHADE) {
+                const ShadePoint sp = shade_point(w0, w1, w2, a);
+                const float msum = sp.msum;
+                const float g[3] = {g0 * msum, g1 * msum, g2 * msum};      // colour = tex * mask (or lerp)
+                if constexpr (MODE == OUT_BILINEAR) {
+                    const TexTap tp = tex_tap(sp.u, sp.v, Th, Tw);
+                    const float wx0 = 1.f - tp.wx1, wy0 = 1.f - tp.wy1;
+                    float sx = 0.f, sy = 0.f;
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) {
+                        const float* t = tex + ((size_t)b * 3 + c) * Th * Tw;
+                        float* dt = dtex + ((size_t)b * 3 + c) * Th * Tw;
+                        const float t00 = tex_at(t, tp.y0, tp.x0, Th, Tw), t01 = tex_at(t, tp.y0, tp.x0 + 1, Th, Tw);
+                        const float t10 = tex_at(t, tp.y0 + 1, tp.x0, Th, Tw), t11 = tex_at(t, tp.y0 + 1, tp.x0 + 1, Th, Tw);
+                        sx += g[c] * ((t01 - t00) * wy0 + (t11 - t10) * tp.wy1);
+                        sy += g[c] * ((t10 - t00) * wx0 + (t11 - t01) * tp.wx1);
+                        if (g[c] != 0.f) {
+                            const bool xa = tp.x0 >= 0 && tp.x0 < Tw, xb = tp.x0 + 1 >= 0 && tp.x0 + 1 < Tw;
+                            const bool ya = tp.y0 >= 0 && tp.y0 < Th, yb = tp.y0 + 1 >= 0 && tp.y0 + 1 < Th;
+                            // the same products as tap_weights (texel_visibility_kernel marks the taps where they are > 0)
+                            if (ya && xa) atomicAdd(dt + (size_t)tp.y0 * Tw + tp.x0, g[c] * wx0 * wy0);
+                            if (ya && xb) atomicAdd(dt + (size_t)tp.y0 * Tw + tp.x0 + 1, g[c] * tp.wx1 * wy0);
+                            if (yb && xa) atomicAdd(dt + (size_t)(tp.y0 + 1) * Tw + tp.x0, g[c] * wx0 * tp.wy1);
+                            if (yb && xb) atomicAdd(dt + (size_t)(tp.y0 + 1) * Tw + tp.x0 + 1, g[c] * tp.wx1 * tp.wy1);
+                        }
+                    }
+                    du = sx * (float)(Tw - 1);
+                    dv = -sy * (float)(Th - 1);
+                } else if constexpr (MODE == OUT_NEAREST) {
+                    const int xi = __float2int_rn(unnorm_x(sp.u, Tw)), yi = __float2int_rn(unnorm_y(sp.v, Th));
+                    if (xi >= 0 && xi < Tw && yi >= 0 && yi < Th) {
+#pragma unroll
+                        for (int c = 0; c < 3; ++c)
+                            if (g[c] != 0.f) atomicAdd(dtex + ((size_t)b * 3 + c) * Th * Tw + (size_t)yi * Tw + xi, g[c]);
+                    }
+                    coord_grad = false;
+                } else {
+                    const float ix = unnorm_x(sp.u, Tw), iy = unnorm_y(sp.v, Th);
+                    const float fx = floorf(ix), fy = floorf(iy);
+                    const int xs = (int)fx - 1, ys = (int)fy - 1;
+                    float cx[4], cy[4], dcx[4], dcy[4];
+                    cubic_weights(ix - fx, cx);
+                    cubic_weights(iy - fy, cy);
+                    cubic_dweights(ix - fx, dcx);
+                    cubic_dweights(iy - fy, dcy);
+                    float sx = 0.f, sy = 0.f;
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) {
+                        const float* t = tex + ((size_t)b * 3 + c) * Th * Tw;
+                        float* dt = dtex + ((size_t)b * 3 + c) * Th * Tw;
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const int y = ys + i;
+                            float rx = 0.f, rdx = 0.f;
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) {
+                                const int x = xs + j;
+                                const float tv = tex_at(t, y, x, Th, Tw);
+                                rx += cx[j] * tv;
+                                rdx += dcx[j] * tv;
+                                if (g[c] != 0.f && x >= 0 && x < Tw && y >= 0 && y < Th)
+                                    atomicAdd(dt + (size_t)y * Tw + x, g[c] * cy[i] * cx[j]);
+                            }
+                            sx += g[c] * cy[i] * rdx;
+                            sy += g[c] * dcy[i] * rx;
+                        }
+                    }
+                    // ix = (u * 2 - 1 + 1) * Tw / 2 - 0.5, iy = (-(v * 2 - 1) + 1) * Th / 2 - 0.5
+                    du = sx * (float)Tw;
+                    dv = -sy * (float)Th;
+                }
+            } else {
+                du = g0;
+                dv = g1;
+            }
+            dw0 = du * a[0] + dv * a[1], dw1 = du * a[2] + dv * a[3], dw2 = du * a[4] + dv * a[5];
+            // d/d(per-vertex uv)
+            cv[6] = w0 * du; cv[7] = w0 * dv; cv[8] = w1 * du; cv[9] = w1 * dv; cv[10] = w2 * du; cv[11] = w2 * dv;
         }
-        // d/d(per-vertex uv)
-        cv[6] = w0 * du; cv[7] = w0 * dv; cv[8] = w1 * du; cv[9] = w1 * dv; cv[10] = w2 * du; cv[11] = w2 * dv;
-        // d/d(2-D vertices) through the barycentrics
-        const float dw0 = du * a[0] + dv * a[1], dw1 = du * a[2] + dv * a[3], dw2 = du * a[4] + dv * a[5];
-        const Face f = unpack(fg[(size_t)fidx * 3], fg[(size_t)fidx * 3 + 1], fg[(size_t)fidx * 3 + 2]);
-        const float m = f.bx - f.ax, p = f.by - f.ay, n = f.cx - f.ax, q = f.cy - f.ay;
-        const float s = x0 - f.ax, t = y0 - f.ay;
-        const float D = (m * q - n * p) + BARY_EPS;
-        const float a1 = (dw1 - dw0) / D, a2 = (dw2 - dw0) / D, a3 = -(a1 * w1 + a2 * w2);
-        const float Gs = a1 * q - a2 * p, Gt = -a1 * n + a2 * m, Gm = a2 * t + a3 * q;
-        const float Gp = -a2 * s - a3 * n, Gn = -a1 * t - a3 * p, Gq = a1 * s + a3 * m;
-        cv[0] = -(Gs + Gm + Gn) * MULT; cv[1] = -(Gt + Gp + Gq) * MULT; cv[2] = Gm * MULT; cv[3] = Gp * MULT;
-        cv[4] = Gn * MULT; cv[5] = Gq * MULT;
+        if (coord_grad) {
+            // d/d(2-D vertices) through the barycentrics
+            const Face f = unpack(fg[(size_t)fidx * 3], fg[(size_t)fidx * 3 + 1], fg[(size_t)fidx * 3 + 2]);
+            const float m = f.bx - f.ax, p = f.by - f.ay, n = f.cx - f.ax, q = f.cy - f.ay;
+            const float s = x0 - f.ax, t = y0 - f.ay;
+            const float D = (m * q - n * p) + BARY_EPS;
+            const float a1 = (dw1 - dw0) / D, a2 = (dw2 - dw0) / D, a3 = -(a1 * w1 + a2 * w2);
+            const float Gs = a1 * q - a2 * p, Gt = -a1 * n + a2 * m, Gm = a2 * t + a3 * q;
+            const float Gp = -a2 * s - a3 * n, Gn = -a1 * t - a3 * p, Gq = a1 * s + a3 * m;
+            cv[0] = -(Gs + Gm + Gn) * MULT; cv[1] = -(Gt + Gp + Gq) * MULT; cv[2] = Gm * MULT; cv[3] = Gp * MULT;
+            cv[4] = Gn * MULT; cv[5] = Gq * MULT;
+        }
     }
-    warp_face_acc<12>(acc, fidx, fidx >= 0 ? posof[fidx] : 0, cv, 0, gp, gu);
+    if constexpr (MODE == OUT_ATTR) {
+        float cp[6];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) cp[k] = cv[k];
+        const int pos = fidx >= 0 ? posof[fidx] : 0;
+        warp_face_acc_attr(acc, fidx, pos, d_imout + pix * d, fidx >= 0 ? imwei[3 * pix] : 0.f,
+                           fidx >= 0 ? imwei[3 * pix + 1] : 0.f, fidx >= 0 ? imwei[3 * pix + 2] : 0.f, d, gu, capn);
+        // 2-D vertex slots of the attribute layout: the same index arithmetic as warp_face_acc's first six
+        const int lane = tid & 31;
+        unsigned todo = __ballot_sync(0xffffffffu, fidx >= 0);
+        while (todo) {
+            const int leader = __ffs(todo) - 1;
+            const int key = __shfl_sync(0xffffffffu, fidx, leader);
+            const bool mine = fidx == key;
+            todo &= ~__ballot_sync(0xffffffffu, mine);
+#pragma unroll
+            for (int k = 0; k < 6; ++k) {
+                const float v = b3d::warp_sum(mine ? cp[k] : 0.f);
+                if (lane == leader) acc_add(acc, pos, k, v, gp + key * 6 + k, nslot, capn);
+            }
+        }
+    } else if constexpr (MODE != OUT_NEAREST) {      // nearest: the colour path adds nothing to the vertices or uvs
+        warp_face_acc<12>(acc, fidx, fidx >= 0 ? posof[fidx] : 0, cv, 0, gp, gu);
+    }
 
     // ---- soft-silhouette path: uncovered pixels ----------------------------------------------------------
     const float gpb = (valid && fidx < 0 && d_improb) ? d_improb[pix] : 0.f;
@@ -461,8 +705,8 @@ mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
                         const Face f = unpack(stage[3 * j], stage[3 * j + 1], stage[3 * j + 2]);
                         const float xmin = min3(f.ax, f.bx, f.cx), xmax = max3(f.ax, f.bx, f.cx);
                         const float ymin = min3(f.ay, f.by, f.cy), ymax = max3(f.ay, f.by, f.cy);
-                        const bool act = soft && cnt < KNUM && !(x0 < sub(xmin, EXPAND) || x0 >= add(xmax, EXPAND) ||
-                                                                 y0 < sub(ymin, EXPAND) || y0 >= add(ymax, EXPAND));
+                        const bool act = soft && cnt < rp.knum && !(x0 < sub(xmin, EXPAND) || x0 >= add(xmax, EXPAND) ||
+                                                                    y0 < sub(ymin, EXPAND) || y0 >= add(ymax, EXPAND));
                         if (!__any_sync(0xffffffffu, act)) continue;
                         float g6[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
                         if (act) {
@@ -474,12 +718,12 @@ mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
                             if (d1 < dm) { dm = d1; e = 1; te = t1; rxe = rx1; rye = ry1; }
                             const float d2 = seg_dist2(x0, y0, f.cx, f.cy, f.ax, f.ay, t1, rx1, ry1);
                             if (d2 < dm) { dm = d2; e = 2; te = t1; rxe = rx1; rye = ry1; }
-                            const float pk = expf(-DELTA * dm / (MULT * MULT));
+                            const float pk = expf(div_mm(-DELTA * dm, rp));
                             if (pass == 0) {
                                 keep *= 1.f - pk;
                             } else if (pk < 1.f - 1e-7f) {
                                 // d improb / d p_k = prod_{j != k}(1 - p_j);  d p_k / d d2 = -delta/m^2 p_k
-                                const float c = gpb * (keep / (1.f - pk)) * (-DELTA / (MULT * MULT)) * pk;
+                                const float c = gpb * (keep / (1.f - pk)) * rp.slope * pk;
                                 const float ga = -2.f * (1.f - te) * c * MULT, gb = -2.f * te * c * MULT;
                                 // edge e joins vertex e and e+1: slots (2e, 2e+1) and (2(e+1)%6, ...)
                                 const float va[2] = {ga * rxe, ga * rye}, vb[2] = {gb * rxe, gb * rye};
@@ -495,7 +739,7 @@ mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
 #pragma unroll
                             for (int k = 0; k < 6; ++k) {
                                 const float v = b3d::warp_sum(g6[k]);
-                                if ((tid & 31) == 0) acc_add(acc, pos, k, v, gp + fi * 6 + k);
+                                if ((tid & 31) == 0) acc_add(acc, pos, k, v, gp + fi * 6 + k, nslot, capn);
                             }
                         }
                     }
@@ -508,8 +752,8 @@ mesh_raster_bwd_kernel(const float4* __restrict__ fgeo, const float* __restrict_
     for (int i = tid; i < nacc; i += NT) {
         const float v = acc[i];
         if (v != 0.f) {
-            const int fi = list[i / 12], k = i % 12;
-            atomicAdd(k < 6 ? gp + fi * 6 + k : gu + fi * 6 + (k - 6), v);
+            const int fi = list[i / nslot], k = i % nslot;
+            atomicAdd(k < 6 ? gp + fi * 6 + k : gu + (size_t)fi * (nslot - 6) + (k - 6), v);
         }
     }
 }
@@ -596,6 +840,164 @@ int b3d_mesh_face_setup(const float* verts, const int32_t* faces, const float* u
     return B3D_OK;
 }
 
+}  // extern "C"
+
+namespace {
+
+// one launch code for every entry point of the rasteriser: `fattr` is fuv [B,F,6] (OUT_UV and the shaded modes) or
+// attr [B,F,3d] (OUT_ATTR)
+// the pixel pitches of an H x W image, rounded as the in-kernel division __fdiv_rn(multiplier, W) would round them
+RasterParams with_pitch(RasterParams rp, int H, int W) {
+    rp.sx = rp.mult / (float)W;
+    rp.sy = rp.mult / (float)H;
+    return rp;
+}
+
+template <int MODE>
+int launch_fwd(const float* fgeo, const float* fattr, int d, const float* tex, const float* bg, RasterParams rp,
+               int B, int F, int H, int W, int Th, int Tw, int32_t* imidx, float* imwei, float* imout, float* improb,
+               cudaStream_t st) {
+    rp = with_pitch(rp, H, W);
+    const size_t smem = fwd_smem(F);
+    B3D_REQUIRE(smem <= 200 * 1024, B3D_EINVAL, "mesh raster: F=%d too large for the tile list", F);
+    dim3 grid(b3d::ceil_div(W, TILE), b3d::ceil_div(H, TILE), B);
+    B3D_CUDA_OK(cudaFuncSetAttribute(mesh_raster_fwd_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    mesh_raster_fwd_kernel<MODE><<<grid, NT, smem, st>>>((const float4*)fgeo, fattr, d, tex, bg, RASTER_PARAMS_ARGS(rp), F, H, W, Th, Tw, imidx,
+                                                         imwei, imout, improb);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+template <int MODE>
+int launch_bwd(const float* fgeo, const float* fattr, int d, const float* tex, int has_bg, RasterParams rp, int B,
+               int F, int H, int W, int Th, int Tw, const int32_t* imidx, const float* imwei, const float* d_imout,
+               const float* d_improb, float* dfp2d, float* dfattr, float* dtex, cudaStream_t st) {
+    rp = with_pitch(rp, H, W);
+    const size_t smem = bwd_smem(F);
+    B3D_REQUIRE(smem <= 200 * 1024, B3D_EINVAL, "mesh raster bwd: F=%d too large for the tile list", F);
+    const size_t nattr = MODE == OUT_ATTR ? 3 * (size_t)d : 6;
+    B3D_CUDA_OK(cudaMemsetAsync(dfp2d, 0, sizeof(float) * 6 * (size_t)B * F, st));
+    B3D_CUDA_OK(cudaMemsetAsync(dfattr, 0, sizeof(float) * nattr * (size_t)B * F, st));
+    if (dtex) B3D_CUDA_OK(cudaMemsetAsync(dtex, 0, sizeof(float) * 3 * (size_t)B * Th * Tw, st));
+    dim3 grid(b3d::ceil_div(W, TILE), b3d::ceil_div(H, TILE), B);
+    B3D_CUDA_OK(cudaFuncSetAttribute(mesh_raster_bwd_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    mesh_raster_bwd_kernel<MODE><<<grid, NT, smem, st>>>((const float4*)fgeo, fattr, d, tex, has_bg, RASTER_PARAMS_ARGS(rp), F, H, W, Th, Tw,
+                                                         imidx, imwei, d_imout, d_improb, dfp2d, dfattr, dtex);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+// B3D_FILTER_* -> shaded output mode
+int filter_mode(int filter) {
+    return filter == B3D_FILTER_BILINEAR ? OUT_BILINEAR
+         : filter == B3D_FILTER_NEAREST  ? OUT_NEAREST
+         : filter == B3D_FILTER_BICUBIC  ? OUT_BICUBIC
+                                         : -1;
+}
+
+int check_params(const char* fn, int d, float expand, int knum, float multiplier, float delta, RasterParams* rp) {
+    B3D_REQUIRE(d >= 1, B3D_EINVAL, "%s: d=%d attributes per vertex, need d >= 1", fn, d);
+    B3D_REQUIRE(knum >= 1, B3D_EINVAL, "%s: knum=%d, need knum >= 1", fn, knum);
+    B3D_REQUIRE(multiplier > 0.f, B3D_EINVAL, "%s: multiplier=%g, need multiplier > 0", fn, multiplier);
+    B3D_REQUIRE(delta > 0.f, B3D_EINVAL, "%s: delta=%g, need delta > 0", fn, delta);
+    B3D_REQUIRE(expand >= 0.f, B3D_EINVAL, "%s: expand=%g, need expand >= 0", fn, expand);
+    // the box margin and the soft-silhouette scale in multiplier units, as kaolin forms them (in double, then fp32)
+    *rp = make_params(multiplier, (float)((double)expand * (double)multiplier), delta, knum);
+    return B3D_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b3d_mesh_face_pack(const float* points3d, const float* points2d, const float* normalz, float multiplier, int B, int F,
+                       float* fgeo, void* stream) {
+    B3D_REQUIRE(B >= 0 && F > 0, B3D_EINVAL, "b3d_mesh_face_pack: bad sizes B=%d F=%d", B, F);
+    B3D_REQUIRE(multiplier > 0.f, B3D_EINVAL, "b3d_mesh_face_pack: multiplier=%g, need multiplier > 0", multiplier);
+    if (B == 0) return B3D_OK;
+    B3D_REQUIRE(points3d && points2d && normalz && fgeo, B3D_EINVAL, "b3d_mesh_face_pack: null pointer");
+    B3D_REQUIRE(B <= 65535, B3D_EINVAL, "b3d_mesh_face_pack: batch too large");
+    B3D_CHECK_ALIGNED(fgeo);
+    mesh_face_pack_kernel<<<dim3(b3d::ceil_div(F, NT), B), NT, 0, (cudaStream_t)stream>>>(points3d, points2d, normalz,
+                                                                                         multiplier, F, (float4*)fgeo);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+int b3d_mesh_raster_attr_fwd(const float* fgeo, const float* attr, int d, int B, int F, int H, int W, float expand,
+                             int knum, float multiplier, float delta, int32_t* imidx, float* imwei, float* imfeat,
+                             float* improb, void* stream) {
+    RasterParams rp;
+    if (int rc = check_params("b3d_mesh_raster_attr_fwd", d, expand, knum, multiplier, delta, &rp)) return rc;
+    B3D_REQUIRE(B >= 0 && F > 0 && H > 0 && W > 0, B3D_EINVAL, "b3d_mesh_raster_attr_fwd: bad sizes");
+    if (B == 0) return B3D_OK;
+    B3D_REQUIRE(fgeo && attr && imidx && imwei && imfeat && improb, B3D_EINVAL, "b3d_mesh_raster_attr_fwd: null pointer");
+    B3D_CHECK_ALIGNED(fgeo);
+    return launch_fwd<OUT_ATTR>(fgeo, attr, d, nullptr, nullptr, rp, B, F, H, W, 0, 0, imidx, imwei, imfeat, improb,
+                                (cudaStream_t)stream);
+}
+
+int b3d_mesh_raster_attr_bwd(const float* fgeo, const float* attr, int d, int B, int F, int H, int W, float expand,
+                             int knum, float multiplier, float delta, const int32_t* imidx, const float* imwei,
+                             const float* d_imfeat, const float* d_improb, float* dp2d, float* dattr, void* stream) {
+    RasterParams rp;
+    if (int rc = check_params("b3d_mesh_raster_attr_bwd", d, expand, knum, multiplier, delta, &rp)) return rc;
+    B3D_REQUIRE(B >= 0 && F > 0 && H > 0 && W > 0, B3D_EINVAL, "b3d_mesh_raster_attr_bwd: bad sizes");
+    if (B == 0) return B3D_OK;
+    B3D_REQUIRE(fgeo && attr && imidx && imwei && d_imfeat && dp2d && dattr, B3D_EINVAL,
+                "b3d_mesh_raster_attr_bwd: null pointer");
+    return launch_bwd<OUT_ATTR>(fgeo, attr, d, nullptr, 0, rp, B, F, H, W, 0, 0, imidx, imwei, d_imfeat, d_improb, dp2d,
+                                dattr, nullptr, (cudaStream_t)stream);
+}
+
+int b3d_mesh_render_filtered_fwd(const float* fgeo, const float* fuv, const float* tex, const float* bg, int B, int F,
+                                 int H, int W, int Th, int Tw, int filter, int32_t* imidx, float* imwei, float* imout,
+                                 float* improb, void* stream) {
+    const int mode = filter_mode(filter);
+    B3D_REQUIRE(mode >= 0, B3D_EINVAL, "b3d_mesh_render_filtered_fwd: unknown filter %d", filter);
+    B3D_REQUIRE(B >= 0 && F > 0 && H > 0 && W > 0, B3D_EINVAL, "b3d_mesh_render_filtered_fwd: bad sizes");
+    if (B == 0) return B3D_OK;
+    B3D_REQUIRE(fgeo && fuv && tex && imidx && imwei && imout && improb, B3D_EINVAL,
+                "b3d_mesh_render_filtered_fwd: null pointer");
+    B3D_REQUIRE(Th > 1 && Tw > 1, B3D_EINVAL, "b3d_mesh_render_filtered_fwd: bad texture size");
+    B3D_CHECK_ALIGNED(fgeo);
+    const RasterParams rp = default_params();
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (mode) {
+        case OUT_NEAREST:
+            return launch_fwd<OUT_NEAREST>(fgeo, fuv, 3, tex, bg, rp, B, F, H, W, Th, Tw, imidx, imwei, imout, improb, st);
+        case OUT_BICUBIC:
+            return launch_fwd<OUT_BICUBIC>(fgeo, fuv, 3, tex, bg, rp, B, F, H, W, Th, Tw, imidx, imwei, imout, improb, st);
+        default:
+            return launch_fwd<OUT_BILINEAR>(fgeo, fuv, 3, tex, bg, rp, B, F, H, W, Th, Tw, imidx, imwei, imout, improb, st);
+    }
+}
+
+int b3d_mesh_render_filtered_bwd(const float* fgeo, const float* fuv, const float* tex, int has_bg, int B, int F, int H,
+                                 int W, int Th, int Tw, int filter, const int32_t* imidx, const float* imwei,
+                                 const float* d_imout, const float* d_improb, float* dfp2d, float* dfuv, float* dtex,
+                                 void* stream) {
+    const int mode = filter_mode(filter);
+    B3D_REQUIRE(mode >= 0, B3D_EINVAL, "b3d_mesh_render_filtered_bwd: unknown filter %d", filter);
+    B3D_REQUIRE(B >= 0 && F > 0 && H > 0 && W > 0, B3D_EINVAL, "b3d_mesh_render_filtered_bwd: bad sizes");
+    if (B == 0) return B3D_OK;
+    B3D_REQUIRE(fgeo && fuv && tex && imidx && imwei && d_imout && dfp2d && dfuv && dtex, B3D_EINVAL,
+                "b3d_mesh_render_filtered_bwd: null pointer");
+    const RasterParams rp = default_params();
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (mode) {
+        case OUT_NEAREST:
+            return launch_bwd<OUT_NEAREST>(fgeo, fuv, 3, tex, has_bg, rp, B, F, H, W, Th, Tw, imidx, imwei, d_imout,
+                                           d_improb, dfp2d, dfuv, dtex, st);
+        case OUT_BICUBIC:
+            return launch_bwd<OUT_BICUBIC>(fgeo, fuv, 3, tex, has_bg, rp, B, F, H, W, Th, Tw, imidx, imwei, d_imout,
+                                           d_improb, dfp2d, dfuv, dtex, st);
+        default:
+            return launch_bwd<OUT_BILINEAR>(fgeo, fuv, 3, tex, has_bg, rp, B, F, H, W, Th, Tw, imidx, imwei, d_imout,
+                                            d_improb, dfp2d, dfuv, dtex, st);
+    }
+}
+
 int b3d_mesh_render_fwd(const float* fgeo, const float* fuv, const float* tex, const float* bg, int B, int F, int H,
                         int W, int Th, int Tw, int32_t* imidx, float* imwei, float* imout, float* improb,
                         void* stream) {
@@ -604,23 +1006,11 @@ int b3d_mesh_render_fwd(const float* fgeo, const float* fuv, const float* tex, c
     B3D_REQUIRE(fgeo && fuv && imidx && imwei && imout && improb, B3D_EINVAL, "b3d_mesh_render_fwd: null pointer");
     B3D_REQUIRE(tex == nullptr || (Th > 1 && Tw > 1), B3D_EINVAL, "b3d_mesh_render_fwd: bad texture size");
     B3D_CHECK_ALIGNED(fgeo);
-    const size_t smem = fwd_smem(F);
-    B3D_REQUIRE(smem <= 200 * 1024, B3D_EINVAL, "b3d_mesh_render_fwd: F=%d too large for the tile list", F);
-    dim3 grid(b3d::ceil_div(W, TILE), b3d::ceil_div(H, TILE), B);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (tex) {
-        B3D_CUDA_OK(cudaFuncSetAttribute(mesh_raster_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem));
-        mesh_raster_fwd_kernel<true><<<grid, NT, smem, st>>>((const float4*)fgeo, fuv, tex, bg, F, H, W, Th, Tw, imidx,
-                                                            imwei, imout, improb);
-    } else {
-        B3D_CUDA_OK(cudaFuncSetAttribute(mesh_raster_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem));
-        mesh_raster_fwd_kernel<false><<<grid, NT, smem, st>>>((const float4*)fgeo, fuv, nullptr, nullptr, F, H, W, 0, 0,
-                                                             imidx, imwei, imout, improb);
-    }
-    B3D_LAUNCH_OK();
-    return B3D_OK;
+    if (tex)
+        return b3d_mesh_render_filtered_fwd(fgeo, fuv, tex, bg, B, F, H, W, Th, Tw, B3D_FILTER_BILINEAR, imidx, imwei,
+                                            imout, improb, stream);
+    return launch_fwd<OUT_UV>(fgeo, fuv, 3, nullptr, nullptr, default_params(), B, F, H, W, 0, 0, imidx, imwei, imout,
+                              improb, (cudaStream_t)stream);
 }
 
 int b3d_mesh_render_bwd(const float* fgeo, const float* fuv, const float* tex, int has_bg, int B, int F, int H, int W,
@@ -631,26 +1021,11 @@ int b3d_mesh_render_bwd(const float* fgeo, const float* fuv, const float* tex, i
     B3D_REQUIRE(fgeo && fuv && imidx && imwei && d_imout && dfp2d && dfuv, B3D_EINVAL,
                 "b3d_mesh_render_bwd: null pointer");
     B3D_REQUIRE((tex == nullptr) == (dtex == nullptr), B3D_EINVAL, "b3d_mesh_render_bwd: tex and dtex go together");
-    const size_t smem = bwd_smem(F);
-    B3D_REQUIRE(smem <= 200 * 1024, B3D_EINVAL, "b3d_mesh_render_bwd: F=%d too large for the tile list", F);
-    cudaStream_t st = (cudaStream_t)stream;
-    B3D_CUDA_OK(cudaMemsetAsync(dfp2d, 0, sizeof(float) * 6 * (size_t)B * F, st));
-    B3D_CUDA_OK(cudaMemsetAsync(dfuv, 0, sizeof(float) * 6 * (size_t)B * F, st));
-    if (dtex) B3D_CUDA_OK(cudaMemsetAsync(dtex, 0, sizeof(float) * 3 * (size_t)B * Th * Tw, st));
-    dim3 grid(b3d::ceil_div(W, TILE), b3d::ceil_div(H, TILE), B);
-    if (tex) {
-        B3D_CUDA_OK(cudaFuncSetAttribute(mesh_raster_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem));
-        mesh_raster_bwd_kernel<true><<<grid, NT, smem, st>>>((const float4*)fgeo, fuv, tex, has_bg, F, H, W, Th, Tw,
-                                                            imidx, imwei, d_imout, d_improb, dfp2d, dfuv, dtex);
-    } else {
-        B3D_CUDA_OK(cudaFuncSetAttribute(mesh_raster_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem));
-        mesh_raster_bwd_kernel<false><<<grid, NT, smem, st>>>((const float4*)fgeo, fuv, nullptr, 0, F, H, W, 0, 0, imidx,
-                                                             imwei, d_imout, d_improb, dfp2d, dfuv, nullptr);
-    }
-    B3D_LAUNCH_OK();
-    return B3D_OK;
+    if (tex)
+        return b3d_mesh_render_filtered_bwd(fgeo, fuv, tex, has_bg, B, F, H, W, Th, Tw, B3D_FILTER_BILINEAR, imidx, imwei,
+                                            d_imout, d_improb, dfp2d, dfuv, dtex, stream);
+    return launch_bwd<OUT_UV>(fgeo, fuv, 3, nullptr, 0, default_params(), B, F, H, W, 0, 0, imidx, imwei, d_imout,
+                              d_improb, dfp2d, dfuv, nullptr, (cudaStream_t)stream);
 }
 
 int b3d_texel_visibility(const int32_t* imidx, const float* imwei, const float* fuv, int B, int F, int H, int W, int Th,

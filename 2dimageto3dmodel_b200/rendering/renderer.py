@@ -26,27 +26,21 @@ def datanormalize(x, axis):
 
 def linear_rasterizer(width, height, points3d_bxfx9, points2d_bxfx6, normalz_bxfx1, vertex_attr_bxfx3d,
                       expand=None, knum=None, multiplier=None, delta=None):
-    """Signature of kaolin.graphics.dib_renderer.rasterizer.linear_rasterizer; only the defaults the
-    reference uses (expand .02, knum 30, multiplier 1000, delta 7000) and d=3 attributes (u,v,1) are built."""
-    for v, dflt in ((expand, 0.02), (knum, 30), (multiplier, 1000), (delta, 7000)):
-        if v is not None and v != dflt:
-            raise _m.B3DError("linear_rasterizer: only kaolin's default expand/knum/multiplier/delta are supported")
-    B, F, _ = points3d_bxfx9.shape
-    # re-pack as an indexed mesh with 3F private vertices so the same kernels apply
-    verts = points3d_bxfx9.reshape(B, 3 * F, 3)
-    faces = torch.arange(3 * F, device=verts.device, dtype=torch.int32).view(F, 3)
-    if vertex_attr_bxfx3d.shape[2] != 9:
-        raise _m.B3DError("linear_rasterizer: expected 3 attributes per vertex (u, v, 1)")
-    uv = vertex_attr_bxfx3d.reshape(B, 3 * F, 3)[:, :, :2].contiguous()
-    imfeat, improb, _, _ = _m.render(verts, faces, uv, None, ft=faces, H=height, W=width)
+    """kaolin.graphics.dib_renderer.rasterizer.linear_rasterizer: -> (imfeat [B,H,W,d], improb [B,H,W,1]).
+
+    points2d and normalz are used as given (any projection, any front-face test), vertex_attr carries any number d of
+    values per face corner, and expand / knum / multiplier / delta default to kaolin's 0.02 / 30 / 1000 / 7000.
+    Differentiable w.r.t. points2d and vertex_attr; points3d (only its depths are read) and normalz get zero gradients,
+    as in kaolin."""
+    imfeat, improb, _, _ = _m.raster_attr(points3d_bxfx9, points2d_bxfx6, normalz_bxfx1, vertex_attr_bxfx3d, height,
+                                          width, expand=expand, knum=knum, multiplier=multiplier, delta=delta)
     return imfeat, improb
 
 
 class Renderer(nn.Module):
     def __init__(self, height, width, filtering='bilinear'):
         super().__init__()
-        if filtering != 'bilinear':
-            raise _m.B3DError("Renderer: only bilinear texture filtering is built (the reference default)")
+        _m.filter_id(filtering)           # 'bilinear' | 'nearest' | 'bicubic', else ValueError (as grid_sample)
         self.height, self.width, self.filtering = height, width, filtering
 
     def forward(self, points, uv_bxpx2, texture_bx3xthxtw, ft_fx3=None, background_image=None,
@@ -56,7 +50,7 @@ class Renderer(nn.Module):
         verts, faces = points
         imrender, improb, imidx, normal1 = _m.render(verts, faces, uv_bxpx2, texture_bx3xthxtw,
                                                      ft=ft_fx3, background=background_image,
-                                                     H=self.height, W=self.width)
+                                                     H=self.height, W=self.width, filtering=self.filtering)
         self.last_face_index = imidx          # face id + 1 per pixel, 0 = background (visibility buffer)
         if return_hardmask:
             improb = (imidx > 0).to(imrender.dtype).unsqueeze(-1)

@@ -176,6 +176,47 @@ B3D_API int b3d_mesh_render_bwd(const float* fgeo, const float* fuv, const float
                                 const float* imwei, const float* d_imout, const float* d_improb,
                                 float* dfp2d, float* dfuv, float* dtex, void* stream);
 
+/* Renderer(height, width, filtering=...)        rendering/renderer.py:33-37,72
+ *   fragmentshader -> texinterpolation          rendering/fragment_shader.py:6-20
+ * The reference's bilinear helper for 'bilinear' (align_corners=True); any other mode goes to
+ * F.grid_sample(texture, grid, mode=filtering) with its defaults align_corners=False, padding_mode='zeros'.  */
+#define B3D_FILTER_BILINEAR 0  /* what b3d_mesh_render_fwd / _bwd shade with */
+#define B3D_FILTER_NEAREST 1   /* the texel at round-half-to-even of ((g + 1) * size - 1) / 2; 0 outside the texture */
+#define B3D_FILTER_BICUBIC 2   /* 4x4 taps, cubic convolution A = -0.75, out-of-range taps read 0 */
+
+/* b3d_mesh_render_fwd / _bwd with a texture and a filter id (B3D_FILTER_*; anything else is B3D_EINVAL).
+ * Same arguments, outputs and raster parameters (kaolin's defaults); tex / dtex must not be NULL.  The hard-mask
+ * multiply, the background lerp and improb are those of the bilinear path.  Backward, nearest: the texture gradient
+ * goes to the one texel read and the 2-D vertices / uvs get no colour-path gradient (as grid_sample); bicubic: texture
+ * gradient to the 16 taps, coordinate gradient through the barycentrics to dfp2d and dfuv.                     */
+B3D_API int b3d_mesh_render_filtered_fwd(const float* fgeo, const float* fuv, const float* tex, const float* bg, int B,
+                                         int F, int H, int W, int Th, int Tw, int filter, int32_t* imidx, float* imwei,
+                                         float* imout, float* improb, void* stream);
+B3D_API int b3d_mesh_render_filtered_bwd(const float* fgeo, const float* fuv, const float* tex, int has_bg, int B, int F,
+                                         int H, int W, int Th, int Tw, int filter, const int32_t* imidx,
+                                         const float* imwei, const float* d_imout, const float* d_improb, float* dfp2d,
+                                         float* dfuv, float* dtex, void* stream);
+
+/* kaolin.graphics.dib_renderer.rasterizer.linear_rasterizer(width, height, points3d_bxfx9, points2d_bxfx6,
+ *   normalz_bxfx1, vertex_attr_bxfx3d, expand=0.02, knum=30, multiplier=1000, delta=7000)   renderer.py:60-67
+ * (restated from SURVEY.md App. B, parity unpinned), with kaolin's inputs as given.
+ * face_pack: points3d [B,F,9] (depths read), points2d [B,F,6], normalz [B,F,1] -> fgeo [B,F,12] as b3d_mesh_face_setup
+ *   lays it out, 2-D coordinates x multiplier.                                                                       */
+B3D_API int b3d_mesh_face_pack(const float* points3d, const float* points2d, const float* normalz, float multiplier,
+                               int B, int F, float* fgeo, void* stream);
+/* attr [B,F,3d] (d values per face corner) -> imfeat [B,H,W,d] = sum_i w_i attr_i on covered pixels, 0 elsewhere;
+ * imidx, imwei, improb as b3d_mesh_render_fwd.  fgeo from b3d_mesh_face_pack with the same multiplier.
+ * d >= 1, knum >= 1, multiplier > 0, delta > 0, expand >= 0, else B3D_EINVAL.
+ * bwd: d_imfeat [B,H,W,d], d_improb [B,H,W] (nullable) -> dp2d [B,F,6] w.r.t. the UNSCALED points2d and dattr [B,F,3d]
+ * (both zeroed by the call).  No gradient to points3d or normalz (kaolin semantics).                             */
+B3D_API int b3d_mesh_raster_attr_fwd(const float* fgeo, const float* attr, int d, int B, int F, int H, int W,
+                                     float expand, int knum, float multiplier, float delta, int32_t* imidx,
+                                     float* imwei, float* imfeat, float* improb, void* stream);
+B3D_API int b3d_mesh_raster_attr_bwd(const float* fgeo, const float* attr, int d, int B, int F, int H, int W,
+                                     float expand, int knum, float multiplier, float delta, const int32_t* imidx,
+                                     const float* imwei, const float* d_imfeat, const float* d_improb, float* dp2d,
+                                     float* dattr, void* stream);
+
 /* Texel visibility of a forward render          run_reconstruction.py:567-572, rendering/inverse_renderer.py texel_visibility
  *   visibility_mask, = torch.autograd.grad(image_pred, pred_tex, torch.ones_like(image_pred))  ->  visibility_mask > 0
  * imidx [B,H,W], imwei [B,H,W,3] of b3d_mesh_render_fwd (tex may be NULL there), fuv [B,F,6] of b3d_mesh_face_setup with the

@@ -74,6 +74,7 @@ _sig("b3d_vertex_pipeline_fwd", _vp, _ll, _ll, _ll, _ll, _i, _i, _vp, _vp, _i, _
 _sig("b3d_vertex_pipeline_bwd", _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp)
 _sig("b3d_bank_forward", _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _sz, _vp, _i, _vp)
 _sig("b3d_bank_backward", _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp)
+_sig("b3d_up2_fold", _vp, _vp, _i, _i, _vp)
 _sig("b3d_pad_x_fwd", _vp, _vp, _ll, _i, _i, _i, _i, _vp)
 _sig("b3d_pad_x_bwd", _vp, _vp, _ll, _i, _i, _i, _i, _vp)
 _sig("b3d_stem_input_fwd", _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp)

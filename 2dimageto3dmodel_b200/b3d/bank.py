@@ -11,6 +11,11 @@ Per layer the bank hands the convolution kernels
   F [T'][Cout][Cin']  tap-major K-major rows (fprop operand; the weight gradient comes back in the same layout),
   D [T'][Cin'][Cout'] its per-tap transpose (input-gradient operand),
 and its backward turns the F-layout gradients into gradients of weight_orig (two launches for the whole network).
+A 3x3 layer whose input is a x2 nearest upsample (`up2`) gets, in place of D, the layouts of the equivalent stride-2
+transposed convolution of the low-resolution input (b3d.conv.conv2d_up2_banked):
+  P  [16][Cout][Cin]  phase weights (fprop operand),
+  D4 [16][Cin][Cout]  P as the taps of a 4x4 stride-2 correlation (input-gradient operand);
+its weight gradient still arrives in the F-layout sink (b3d_up2_fold adds the adjoint of P there).
 """
 import struct
 
@@ -29,19 +34,20 @@ def _r64(v):
 
 class LayerWeights:
     """What one convolution needs from the bank for one forward/backward: wf (autograd output), wd, df (gradient sink)."""
-    __slots__ = ("wf", "wd", "df", "Cout", "Cin", "kh", "kw", "fold", "Cinp", "Coutp", "Tp", "bias")
+    __slots__ = ("wf", "wd", "wp", "df", "Cout", "Cin", "kh", "kw", "fold", "Cinp", "Coutp", "Tp", "bias")
 
     def __init__(self, spec):
         for k in ("Cout", "Cin", "kh", "kw", "fold", "Cinp", "Coutp", "Tp"):
             setattr(self, k, spec[k])
-        self.wf = self.wd = self.df = self.bias = None
+        self.wf = self.wd = self.wp = self.df = self.bias = None
 
 
 class WeightBank:
-    def __init__(self, convs, fold=(), no_dgrad=(), round_tf32=True):
+    def __init__(self, convs, fold=(), no_dgrad=(), round_tf32=True, up2=()):
         """convs: ordered {name: conv module} (spectral-normalised modules expose weight_orig / weight_u / weight_v, plain
         ones weight).  fold: names whose kh vertical taps are folded into the channel dimension (thin stems).
-        no_dgrad: names that never need an input gradient (no D layout is written)."""
+        no_dgrad: names that never need an input gradient (no D layout is written).
+        up2: 3x3 layers whose input is a x2 nearest upsample (P and D4 are written in place of D)."""
         self.names = list(convs)
         self.mods = [convs[n] for n in self.names]
         # emitted weights rounded to the nearest tf32 value (the tensor cores would otherwise truncate the fp32 words)
@@ -55,8 +61,11 @@ class WeightBank:
             fd = n in fold
             Cinp = _r32(kh * Cin if fd else Cin)
             Tp = kw if fd else kh * kw
+            u2 = n in up2
+            if u2 and (fd or (kh, kw) != (3, 3) or Cin % 32 or Cout % 32):
+                raise B3DError(f"bank: {n}: up2 needs an unfolded 3x3 layer with Cin, Cout multiples of 32")
             sp = dict(name=n, sn=sn, Cout=Cout, Cin=Cin, kh=kh, kw=kw, fold=int(fd), Cinp=Cinp, Coutp=_r32(Cout), Tp=Tp,
-                      K=Cin * kh * kw, need_d=n not in no_dgrad)
+                      K=Cin * kh * kw, need_d=n not in no_dgrad or u2, up2=int(u2))
             sp["wf_off"] = off_out
             off_out += _r64(Tp * Cout * Cinp)
             self.specs.append(sp)
@@ -65,7 +74,7 @@ class WeightBank:
             sp["wd_off"] = -1
             if sp["need_d"]:
                 sp["wd_off"] = off_out
-                off_out += _r64(sp["Tp"] * sp["Cinp"] * sp["Coutp"])
+                off_out += _r64((32 if sp["up2"] else sp["Tp"]) * sp["Cinp"] * sp["Coutp"])
         for sp in self.specs:
             sp["u_off"], sp["v_off"], sp["scal_off"] = off_out, off_out + _r64(sp["Cout"]), off_out + _r64(sp["Cout"]) + _r64(sp["K"])
             off_out = sp["scal_off"] + 64
@@ -97,7 +106,7 @@ class WeightBank:
             rec.append(struct.pack("<3Q9q12i", ptrs[-1][0], ptrs[-1][1], ptrs[-1][2], sp["t_off"], sp["s_off"], sp["wf_off"],
                                    sp["wd_off"], sp["u_off"], sp["v_off"], sp["scal_off"], sp["wf_off"], sp["dw_off"],
                                    sp["Cout"], sp["Cin"], sp["kh"], sp["kw"], sp["fold"], sp["Cinp"], sp["Coutp"], sp["Tp"],
-                                   int(sp["sn"]), 0, 0, 0))
+                                   int(sp["sn"]), sp["up2"], 0, 0))
             if sp["sn"]:
                 wtu += [(i, a, b, 0) for a in range(-(-sp["K"] // 256)) for b in range(-(-sp["Cout"] // 64))]
                 wv += [(i, a, 0, 0) for a in range(-(-sp["Cout"] // 8))]
@@ -141,6 +150,8 @@ class WeightBank:
             lw = LayerWeights(sp)
             lw.wf = outs[i]
             lw.wd = outs[n + i] if sp["need_d"] else None
+            if sp["up2"]:
+                lw.wp, lw.wd = lw.wd[:16], lw.wd[16:].reshape(16, sp["Cin"], sp["Cout"])
             if need_grad:
                 sz = sp["Tp"] * sp["Cout"] * sp["Cinp"]
                 lw.df = df_flat[sp["wf_off"]: sp["wf_off"] + sz].view(sp["Tp"], sp["Cout"], sp["Cinp"])
@@ -161,7 +172,9 @@ class _BankFn(torch.autograd.Function):
         wfs, wds = [], []
         for sp in bank.specs:
             wfs.append(out[sp["wf_off"]: sp["wf_off"] + sp["Tp"] * sp["Cout"] * sp["Cinp"]].view(sp["Tp"], sp["Cout"], sp["Cinp"]))
-            if sp["need_d"]:
+            if sp["up2"]:       # P [16][Cout][Cin] then D4 [16][Cin][Cout], split by LayerWeights
+                wds.append(out[sp["wd_off"]: sp["wd_off"] + 32 * sp["Cin"] * sp["Cout"]].view(32, sp["Cout"], sp["Cin"]))
+            elif sp["need_d"]:
                 wds.append(out[sp["wd_off"]: sp["wd_off"] + sp["Tp"] * sp["Cinp"] * sp["Coutp"]].view(sp["Tp"], sp["Cinp"], sp["Coutp"]))
             else:
                 wds.append(out.new_empty(0))

@@ -194,6 +194,136 @@ def _wgrad(gy, x, kh, kw, pad_y=0, stride=1, x_crop=0, sink=None, g_pitch=0, fol
     return dw if tap_major else dw[:Cout, :Cin]
 
 
+# ------------------------------------------------------------------------------------------------------------------
+# a 3x3 convolution of a x2 nearest-upsampled input (and the 1x1 shortcut beside it) on the low-resolution map
+# ------------------------------------------------------------------------------------------------------------------
+# conv3x3(pad_x(up2(X), 1), W, padding=(1, 0)) is the stride-2 transposed convolution of Xp = pad_x(X, 1) (replicate or
+# circular alike: the pad columns of the upsampled map are the upsampled pad columns of X):
+#   Y[2i + py, 2j + px] = sum_{a, b in {0, 1}} P[q] Xp[i + py + a - 1 (zero outside 0 .. H-1), j + px + b],
+#   q = ((py*2 + px)*2 + a)*2 + b,  P[q] = sum_k sum_l A_py[a][k] A_px[b][l] W[k][l],  A_0 = [[1,0,0],[0,1,1]], A_1 = [[1,1,0],[0,0,1]]
+# (the bank writes P and its 4x4 transposed layout D4, csrc/sn_kernels.cu): 4 taps per output pixel instead of 9, and the
+# upsampled map is never written.  A 1x1 shortcut commutes with the upsample and runs on the low-resolution pixels.
+def up2_fprop_taps():
+    """(dy, dx, wtap, classes) of the forward's one launch: four parity classes (py, px), output stride 2, class c at output
+    offset classes[c], taps (a, b) of class c reading Xp at (i + dy, j + dx) with P[wtap]."""
+    cls = [(py, px) for py in range(2) for px in range(2)]
+    q = [(py, px, a, b) for py, px in cls for a in range(2) for b in range(2)]
+    return ([py + a - 1 for py, px, a, b in q], [px + b for py, px, a, b in q], [((py * 2 + px) * 2 + a) * 2 + b for py, px, a, b in q],
+            cls)
+
+
+def up2_dgrad_taps():
+    """(dy, dx) of the input gradient, a 4x4 stride-2 correlation of dY [N,2H,2W,Cout] on D4:
+    dXp[i, j'] = sum_{r,s} D4[4r + s] dY[2i + r - 1, 2j' + s - 3] (zero outside dY), for the W + 2 columns j' of Xp.
+    Tap (r, s) carries P[q]^T with (r, s) = (3 - py - 2a, 3 - px - 2b)."""
+    return [r - 1 for r in range(4) for _ in range(4)], [s - 3 for _ in range(4) for s in range(4)]
+
+
+def up2_wgrad_columns(W):
+    """(first Xp column, columns, x offset) of the three weight-gradient launches that give dP^T [16][Cin][Cout] =
+    sum Xp[i, j'] (x) dY[2i + r - 1, 2j' + s - 3] with Xp as the M operand: the interior columns, then each pad column alone
+    (of whose taps only s = 3, resp. s = 0 land inside dY), so that no 32-pixel K slice is spent on two pad columns."""
+    return [(1, W, -1), (0, 1, -3), (W + 1, 1, 2 * W - 1)]
+
+
+def _up_fprop(xp, wp, wsc=None, stats=None):
+    """xp [N,H,W+2,Cin] (the x-padded low-resolution input), wp = P [16][Cout][Cin] -> y [N,2H,2W,Cout], the 3x3
+    convolution of the upsampled map; stats: zeroed fp64 [2*Cout] the epilogue accumulates y's per-channel sum / sum of
+    squares into (the four classes tile y).  wsc: the 1x1 shortcut's F [1][Csc][Cin] -> its output [N,H,W,Csc] on the
+    interior of xp, else None."""
+    N, H, Wp, Cin = xp.shape
+    W, Cout = Wp - 2, wp.shape[1]
+    st = stream_ptr(xp)
+    y = torch.empty(N, 2 * H, 2 * W, Cout, device=xp.device, dtype=torch.float32)
+    dy, dx, wtap, cls = up2_fprop_taps()
+    opts = _ConvOpts(None, 1.0, 0, 0, 4)
+    for i, (py, px) in enumerate(cls):
+        opts.class_ooy[i], opts.class_oox[i] = py, px
+    check(_conv_call(lib.b3d_conv2d_tf32, ptr(xp), ptr(wp), None, ptr(y), N, H, Wp, Cin, H, W, Cout, 16, _ints(dy), _ints(dx), 1, 1,
+                     2 * H, 2 * W, Cout, 2, 2, 0, 0, 1.0, _ints(wtap), 16, ptr(stats), 0, 0,
+                     ctypes.cast(ctypes.pointer(opts), ctypes.c_void_p), st))
+    sc = None
+    if wsc is not None:
+        Csc = wsc.shape[1]
+        sc = torch.empty(N, H, W, Csc, device=xp.device, dtype=torch.float32)
+        check(_conv_call(lib.b3d_conv2d_tf32, ptr(xp), ptr(wsc), None, ptr(sc), N, H, Wp, Cin, H, W, Csc, 1, _ints([0]), _ints([1]), 1,
+                         1, H, W, Csc, 1, 1, 0, 0, 1.0, None, 0, None, 0, 0, None, st))
+    return y, sc
+
+
+def _up_dgrad(gy, wd4, gsc=None, wdsc=None):
+    """Gradient w.r.t. xp [N,H,W+2,Cin] from gy [N,2H,2W,Cout] on D4 = wd4 [16][Cin][Cout], plus the shortcut's from gsc
+    [N,H,W,Csc] on its D = wdsc [1][Cin][Csc] when given."""
+    N, H2, W2, Cout = gy.shape
+    H, Wp, Cin = H2 // 2, W2 // 2 + 2, wd4.shape[1]
+    st = stream_ptr(gy)
+    gx = torch.empty(N, H, Wp, Cin, device=gy.device, dtype=torch.float32)
+    dy, dx = up2_dgrad_taps()
+    check(_conv_call(lib.b3d_conv2d_tf32, ptr(gy), ptr(wd4), None, ptr(gx), N, H2, W2, Cout, H, Wp, Cin, 16, _ints(dy), _ints(dx), 2, 2,
+                     H, Wp, Cin, 1, 1, 0, 0, 1.0, None, 0, None, 0, 0, None, st))
+    if gsc is not None:
+        gs = torch.empty_like(gx)
+        check(_conv_call(lib.b3d_conv2d_tf32, ptr(gsc), ptr(wdsc), None, ptr(gs), N, H, Wp - 2, gsc.shape[3], H, Wp, Cin, 1, _ints([0]),
+                         _ints([-1]), 1, 1, H, Wp, Cin, 1, 1, 0, 0, 1.0, None, 0, None, 0, 0, None, st))
+        gx += gs
+    return gx
+
+
+def _up_wgrad(gy, xp, df, gsc=None, dfsc=None):
+    """Weight gradients from gy [N,2H,2W,Cout] and xp [N,H,W+2,Cin]: dP^T [16][Cin][Cout] from the 4x4 stride-2 weight
+    gradient with the roles swapped (Xp as the M operand, so that Cin, not Cout, fills the wgmma tile), folded into the
+    F-layout sink df [9][Cout][Cin] by b3d_up2_fold; the shortcut's from gsc [N,H,W,Csc] into its sink dfsc."""
+    N, H, Wp, Cin = xp.shape
+    _, H2, W2, Cout = gy.shape
+    st = stream_ptr(gy)
+    dpt = torch.zeros(16, Cin, Cout, device=gy.device, dtype=torch.float32)
+    for j0, w, x_off in up2_wgrad_columns(Wp - 2):
+        check(_conv_call(lib.b3d_conv2d_wgrad_tf32, ctypes.c_void_p(xp.data_ptr() + 4 * Cin * j0), ptr(gy), ptr(dpt), N, H2, W2, Cout,
+                         H, w, Cin, 4, 4, 1, 2, x_off, 1, 0, Wp, st))
+    check(lib.b3d_up2_fold(ptr(dpt), ptr(df), Cout, Cin, st))
+    if gsc is not None:
+        check(_conv_call(lib.b3d_conv2d_wgrad_tf32, ptr(gsc), ptr(xp), ptr(dfsc), N, H, Wp, Cin, H, Wp - 2, gsc.shape[3], 1, 1, 0, 1,
+                         1, 1, 0, 0, st))
+
+
+class _UpConv(torch.autograd.Function):
+    """conv1 of an upsampling block (and its 1x1 shortcut when lwsc is given) on the low-resolution padded input xp; wf / wfsc
+    are the bank outputs autograd differentiates, whose gradients go to the bank's F-layout sinks."""
+
+    @staticmethod
+    def forward(ctx, xp, wf, wfsc, lw, lwsc, stats):
+        xp = dev(xp.detach(), "x")
+        if xp.shape[3] != lw.Cin or lw.wp is None:
+            raise B3DError(f"conv2d_up2: input has {xp.shape[3]} channels (layer: {lw.Cin}), or the layer is not an up2 layer")
+        y, sc = _up_fprop(xp, dev(lw.wp.detach(), "weight"), dev(lwsc.wf.detach(), "weight") if lwsc is not None else None, stats)
+        ctx.save_for_backward(xp)
+        ctx.lw, ctx.lwsc = lw, lwsc
+        return (y, sc) if sc is not None else y
+
+    @staticmethod
+    def backward(ctx, gy, gsc=None):
+        xp, = ctx.saved_tensors
+        lw, lwsc = ctx.lw, ctx.lwsc
+        gy = dev(gy, "grad_output")
+        gsc = dev(gsc, "grad_output") if gsc is not None else None
+        gx = _up_dgrad(gy, lw.wd, gsc, lwsc.wd if gsc is not None else None) if ctx.needs_input_grad[0] else None
+        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            if lw.df is None or (gsc is not None and lwsc.df is None):
+                raise B3DError("conv2d_up2: weight gradients need the bank's gradient sinks")
+            _up_wgrad(gy, xp, lw.df, gsc, lwsc.df if gsc is not None else None)
+        return (gx, lw.df if ctx.needs_input_grad[1] else None, lwsc.df if ctx.needs_input_grad[2] else None, None, None, None)
+
+
+def conv2d_up2_banked(xp_nchw, lw, lw_sc=None, stats=None):
+    """conv2d_banked(pad_x(up2(x), 1), lw, pad_y=1, stats=stats) from xp = pad_x(x, 1) alone (lw: a layer the bank registered
+    with up2), and the block's 1x1 shortcut conv2d_banked(up2(x), lw_sc) at low resolution, i.e. before its upsample.
+    Returns (y, shortcut output or None), logically NCHW."""
+    x = xp_nchw.permute(0, 2, 3, 1)
+    out = _UpConv.apply(x, lw.wf, lw_sc.wf if lw_sc is not None else None, lw, lw_sc, stats)
+    y, sc = out if lw_sc is not None else (out, None)
+    return y.permute(0, 3, 1, 2), sc.permute(0, 3, 1, 2) if sc is not None else None
+
+
 def conv2d_nhwc(x, weight, bias=None, pad_y=0, stride=1, leaky=1.0, wt=None, pad_out=0, pad_mode=1, x_crop=0):
     """x [N,H,W,Cin] (Cin % 32 == 0), weight [Cout,Cin,kh,kw] -> [N,Hout,Wout,Cout]; zero pad along y only.
     pad_out > 0: the result is written into the interior of a [N,Hout,Wout + 2*pad_out,Cout] buffer whose pad columns
@@ -250,6 +380,8 @@ class _Conv(torch.autograd.Function):
         fold_fwd: the forward alone runs on a folded copy of x (b3d.ew.fold_rows), freed when it returns; the backward still
         reads the raw input."""
         x = dev(x.detach(), "x")
+        if lw.wp is not None:               # its wd is D4, not D: only conv2d_up2_banked runs such a layer
+            raise B3DError("conv2d: a layer registered with up2 runs through conv2d_up2_banked")
         Cx = x.shape[3]
         fold_pad = 0
         if fold_raw:

@@ -206,7 +206,8 @@ class _CBNActPad(torch.autograd.Function):
     or CIRCULAR x padding of the output (wrapped in upsampled coordinates)."""
 
     @staticmethod
-    def forward(ctx, y, gb, cb, key, bn, skip, skip_off, up, pad, post_leaky, sums_in=None, slope=0.2, pad_mode=REPLICATE):
+    def forward(ctx, y, gb, cb, key, bn, skip, skip_off, up, pad, post_leaky, sums_in=None, slope=0.2, pad_mode=REPLICATE,
+                skip_half=False):
         y = dev(y.detach(), "y")
         N, H, W, C = y.shape
         gbd = dev(gb.detach(), "gamma/beta")
@@ -262,14 +263,14 @@ class _CBNActPad(torch.autograd.Function):
                                       ptr(bn.num_batches_tracked) if track else None,
                                       ptr(mean), ptr(invstd), ptr(scale), ptr(shift), ptr(gt), N, C, st))
         sk = dev(skip.detach(), "skip") if skip is not None else None
-        pitch = sk.shape[2] if sk is not None else 0
+        pitch = (-sk.shape[2] if skip_half else sk.shape[2]) if sk is not None else 0       # < 0: half-resolution skip
         out = torch.empty(N, up * H, up * W + 2 * pad, C, device=y.device, dtype=torch.float32)
         check(lib.b3d_cbn_act_fwd(ptr(y), ptr(scale), ptr(shift), ptr(sk), pitch, skip_off, ptr(out), N, H, W, C, up, pad,
                                   int(pad_mode), float(slope), int(post_leaky), st))
         ctx.save_for_backward(y, gt, scale, shift, mean, invstd, sk if sk is not None else torch.empty(0))
         ctx.cb, ctx.key = cb, key
         ctx.cfg = (skip_off, up, pad, post_leaky, mode, sync, count, sk is not None, skip.shape if skip is not None else None,
-                   P, goff, boff, float(slope), int(pad_mode))
+                   P, goff, boff, float(slope), int(pad_mode), pitch)
         ctx.peers = peers
         # mode 2's inv_std of a clamped channel, as the kernels round it: (float)(1 / sqrt((double)eps))
         ctx.clamp_lim = _f32(1.0 / math.sqrt(_f32(bn.eps))) if sync else None
@@ -278,7 +279,7 @@ class _CBNActPad(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gout):
         y, gt, scale, shift, mean, invstd, sk = ctx.saved_tensors
-        skip_off, up, pad, post_leaky, mode, sync, count, has_skip, skip_shape, P, goff, boff, slope, pad_mode = ctx.cfg
+        skip_off, up, pad, post_leaky, mode, sync, count, has_skip, skip_shape, P, goff, boff, slope, pad_mode, pitch = ctx.cfg
         cb = ctx.cb
         N, H, W, C = y.shape
         gout = dev(gout, "grad")
@@ -286,16 +287,17 @@ class _CBNActPad(torch.autograd.Function):
         ga = torch.empty_like(y)
         gskip, gpitch = None, 0
         if has_skip and ctx.needs_input_grad[5]:
-            gpitch = skip_shape[2]
-            gskip = torch.zeros(skip_shape, device=y.device) if gpitch != W else torch.empty(skip_shape, device=y.device)
+            gpitch = pitch                                  # < 0: one value per 2 x 2 footprint, at half resolution
+            covered = abs(gpitch) == (W // 2 if gpitch < 0 else W)        # else the pad columns stay zero
+            gskip = torch.empty(skip_shape, device=y.device) if covered else torch.zeros(skip_shape, device=y.device)
         want_gb = ctx.needs_input_grad[1]
         sink = cb.grad_sink(N) if want_gb else torch.empty(N, P, device=y.device)
         s1 = ctypes.c_void_p(sink.data_ptr() + 4 * boff)        # d beta  = sum ga
         s2 = ctypes.c_void_p(sink.data_ptr() + 4 * goff)        # d gamma = sum ga * xhat
         stat_pitch = C if mode >= 3 else 0                 # per-sample mean / inv_std rows (instance / no normalisation)
-        check(lib.b3d_cbn_act_bwd1(ptr(gout), ptr(y), ptr(scale), ptr(shift), ptr(sk) if has_skip else None,
-                                   sk.shape[2] if has_skip else 0, skip_off, ptr(mean), ptr(invstd), stat_pitch, ptr(ga), ptr(gskip),
-                                   gpitch, skip_off, s1, s2, P, N, H, W, C, up, pad, pad_mode, slope, int(post_leaky), st))
+        check(lib.b3d_cbn_act_bwd1(ptr(gout), ptr(y), ptr(scale), ptr(shift), ptr(sk) if has_skip else None, pitch, skip_off,
+                                   ptr(mean), ptr(invstd), stat_pitch, ptr(ga), ptr(gskip), gpitch, skip_off, s1, s2, P, N, H, W, C,
+                                   up, pad, pad_mode, slope, int(post_leaky), st))
         inv_m = 0.0
         if mode >= 3:
             # per-sample coupling terms inv_m * gamma_t * (S1, S2) read straight from the d(gamma, beta) rows
@@ -329,7 +331,7 @@ class _CBNActPad(torch.autograd.Function):
                 if cb.done != cb.n_layers:
                     raise RuntimeError(f"CBNBatch: {cb.done} of {cb.n_layers} layers ran their backward before the first layer's")
                 ggb = sink.sum(dim=0, keepdim=True) if cb.shared else sink
-        return ga, ggb, None, None, None, gskip, None, None, None, None, None, None, None
+        return ga, ggb, None, None, None, gskip, None, None, None, None, None, None, None, None
 
 
 def bn_act_pad(y_nchw, bn, skip_nchw=None, skip_off=0, up=1, pad=1, post_relu=False, slope=0.0):
@@ -346,8 +348,9 @@ def bn_act_pad(y_nchw, bn, skip_nchw=None, skip_off=0, up=1, pad=1, post_relu=Fa
 
 
 def cbn_act_pad(y_nchw, cbn, z, skip_nchw=None, skip_off=0, up=1, pad=1, post_leaky=False, cb=None, sums=None,
-                pad_mode=REPLICATE):
+                pad_mode=REPLICATE, skip_half=False):
     """ConditionalBatchNorm2d(y, z) -> LeakyReLU(0.2) [-> + skip] [-> LeakyReLU] [-> x2 upsample] -> x pad, fused.
+    skip_half: the skip has half y's resolution and is added as its x2 nearest upsample (pixel (y/2, x/2)).
     `cbn` is a models.gan.ConditionalBatchNorm2d whose .norm is a (Synchronized)BatchNorm2d without affine (statistics and
     running buffers follow F.batch_norm in a single process, the reference's SyncBN formulas under torch.distributed), an
     InstanceNorm2d without affine or running buffers (per-sample statistics), or identity_norm (no normalisation).
@@ -361,7 +364,7 @@ def cbn_act_pad(y_nchw, cbn, z, skip_nchw=None, skip_off=0, up=1, pad=1, post_le
     y = y_nchw.permute(0, 2, 3, 1)
     skip = skip_nchw.permute(0, 2, 3, 1) if skip_nchw is not None else None
     out = _CBNActPad.apply(y, cb.gb, cb, id(cbn), cbn.norm, skip, int(skip_off), int(up), int(pad), bool(post_leaky), sums, 0.2,
-                           int(pad_mode))
+                           int(pad_mode), bool(skip_half))
     return out.permute(0, 3, 1, 2)
 
 

@@ -712,6 +712,7 @@ struct CbnGeom {
     int N, H, W, C4;             // input y [N,H,W,4*C4]
     int up, pad;                 // output [N, up*H, up*W + 2*pad, C]
     int skip_pitch, skip_off;    // skip pixel (y,x) lives at row (y*skip_pitch + x + skip_off); pitch 0 = no skip
+    int skip_sh;                 // 1: the skip has half y's resolution, pixel (y,x) of y adds skip pixel (y/2, x/2)
     float slope;                 // LeakyReLU slope of the first activation
     int post_leaky;              // apply LeakyReLU again after the residual add (blk6 / mesh head)
 };
@@ -741,7 +742,8 @@ cbn_act_fwd_kernel(const float4* __restrict__ y, const float4* __restrict__ scal
         float4 o = make_float4(lk(fmaf(v.x, sc.x, sh.x), g.slope), lk(fmaf(v.y, sc.y, sh.y), g.slope),
                                lk(fmaf(v.z, sc.z, sh.z), g.slope), lk(fmaf(v.w, sc.w, sh.w), g.slope));
         if (g.skip_pitch) {
-            const float4 k = __ldg(skip + (((long long)n * g.H + ys) * g.skip_pitch + xs + g.skip_off) * g.C4 + c);
+            const float4 k = __ldg(skip + (((long long)n * (g.H >> g.skip_sh) + (ys >> g.skip_sh)) * g.skip_pitch + (xs >> g.skip_sh) +
+                                           g.skip_off) * g.C4 + c);
             o.x += k.x; o.y += k.y; o.z += k.z; o.w += k.w;
         }
         if (g.post_leaky) o = make_float4(lk(o.x, g.slope), lk(o.y, g.slope), lk(o.z, g.slope), lk(o.w, g.slope));
@@ -763,7 +765,8 @@ cbn_act_fwd_rows_kernel(const float4* __restrict__ y, const float4* __restrict__
         const int ys = yo / g.up;
         const float4 sc = __ldg(scale + (long long)n * g.C4 + c), sh = __ldg(shift + (long long)n * g.C4 + c);
         const float4* yrow = y + (((long long)n * g.H + ys) * g.W) * g.C4 + c;
-        const float4* srow = g.skip_pitch ? skip + (((long long)n * g.H + ys) * g.skip_pitch + g.skip_off) * g.C4 + c : nullptr;
+        const float4* srow = g.skip_pitch ? skip + (((long long)n * (g.H >> g.skip_sh) + (ys >> g.skip_sh)) * g.skip_pitch + g.skip_off) * g.C4 + c
+                                          : nullptr;
         float4* orow = out + (long long)row * Wo * g.C4 + c;
         constexpr int U = 4;                                 // independent pixels in flight per thread
         for (int xb = px0; xb < Wo; xb += U * PPB) {
@@ -775,7 +778,7 @@ cbn_act_fwd_rows_kernel(const float4* __restrict__ y, const float4* __restrict__
                 int xs = src_col(xo, g.pad, Wu, PM);
                 xs = g.up == 2 ? xs >> 1 : xs;
                 v[u] = __ldg(yrow + (long long)xs * g.C4);
-                if (srow) k[u] = __ldg(srow + (long long)xs * g.C4);
+                if (srow) k[u] = __ldg(srow + (long long)(xs >> g.skip_sh) * g.C4);
             }
 #pragma unroll
             for (int u = 0; u < U; ++u) {
@@ -796,7 +799,8 @@ cbn_act_fwd_rows_kernel(const float4* __restrict__ y, const float4* __restrict__
 // with xhat = (y - mean) * inv_std.  One CTA walks `rows_per_cta` image rows of one sample, threads own channel quads.
 // PM: the forward's pad mode; with circular padding (1) every pad column is folded back onto the upsampled column it wraps
 // from (the order interior, right pad, left pad of b3d_pad_x_bwd).  PS: mean / inv_std are per-sample rows [N, C].
-template <int PM, bool PS>
+// HS: 1 = the skip has half the resolution (g.skip_sh), 0 = the same as y.
+template <int PM, bool PS, int HS>
 __global__ void __launch_bounds__(NT)
 cbn_act_bwd1_kernel(const float4* __restrict__ gout, const float4* __restrict__ y, const float4* __restrict__ scale,
                     const float4* __restrict__ shift, const float4* __restrict__ skip, const float4* __restrict__ mean,
@@ -810,52 +814,61 @@ cbn_act_bwd1_kernel(const float4* __restrict__ gout, const float4* __restrict__ 
         const long long so = PS ? (long long)n * g.C4 + c : c;
         const float4 mu = __ldg(mean + so), is = __ldg(invstd + so);
         float4 a1 = make_float4(0.f, 0.f, 0.f, 0.f), a2 = a1;
-        for (int p = y0 * g.W + lane_px; p < y1 * g.W; p += px_step) {
-            const int ys = p / g.W, xs = p % g.W;
-            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-            for (int i = 0; i < g.up; ++i) {
-                const float4* row = gout + (((long long)n * g.up * g.H + g.up * ys + i) * Wo) * g.C4 + c;
-                if (PM == 0) {
-                    int lo = g.up * xs + g.pad, hi = lo + g.up;      // children columns [lo, hi)
-                    if (xs == 0) lo = 0;                              // left pad columns replicate column 0
-                    if (xs == g.W - 1) hi = Wo;                       // right pad columns replicate the last column
-                    for (int xo = lo; xo < hi; ++xo) {
-                        const float4 v = __ldg(row + (long long)xo * g.C4);
-                        s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-                    }
-                } else {
-                    for (int u = g.up * xs; u < g.up * xs + g.up; ++u) {   // upsampled column u: interior + its copies
-                        float4 v = __ldg(row + (long long)(u + g.pad) * g.C4);
-                        s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-                        if (u < g.pad) {                              // right pad column Wu + pad + u
-                            v = __ldg(row + (long long)(u + g.pad + Wu) * g.C4);
+        // a half-resolution skip (skip_sh): one thread walks the 2 x 2 footprint of each skip pixel, so that its gradient is
+        // summed in a fixed order; otherwise one pixel per step
+        const int Wq = g.W >> HS;
+        for (int p = (y0 >> HS) * Wq + lane_px; p < (y1 >> HS) * Wq; p += px_step) {
+            float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+            for (int e = 0; e < (1 << (2 * HS)); ++e) {
+                const int ys = ((p / Wq) << HS) + (e >> 1), xs = ((p % Wq) << HS) + (e & 1);
+                float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+                for (int i = 0; i < g.up; ++i) {
+                    const float4* row = gout + (((long long)n * g.up * g.H + g.up * ys + i) * Wo) * g.C4 + c;
+                    if (PM == 0) {
+                        int lo = g.up * xs + g.pad, hi = lo + g.up;      // children columns [lo, hi)
+                        if (xs == 0) lo = 0;                              // left pad columns replicate column 0
+                        if (xs == g.W - 1) hi = Wo;                       // right pad columns replicate the last column
+                        for (int xo = lo; xo < hi; ++xo) {
+                            const float4 v = __ldg(row + (long long)xo * g.C4);
                             s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
                         }
-                        if (u >= Wu - g.pad) {                        // left pad column u + pad - Wu
-                            v = __ldg(row + (long long)(u + g.pad - Wu) * g.C4);
+                    } else {
+                        for (int u = g.up * xs; u < g.up * xs + g.up; ++u) {   // upsampled column u: interior + its copies
+                            float4 v = __ldg(row + (long long)(u + g.pad) * g.C4);
                             s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+                            if (u < g.pad) {                              // right pad column Wu + pad + u
+                                v = __ldg(row + (long long)(u + g.pad + Wu) * g.C4);
+                                s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+                            }
+                            if (u >= Wu - g.pad) {                        // left pad column u + pad - Wu
+                                v = __ldg(row + (long long)(u + g.pad - Wu) * g.C4);
+                                s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+                            }
                         }
                     }
                 }
+                const long long idx = (((long long)n * g.H + ys) * g.W + xs) * g.C4 + c;
+                const float4 v = __ldg(y + idx);
+                const float4 pre = make_float4(fmaf(v.x, sc.x, sh.x), fmaf(v.y, sc.y, sh.y), fmaf(v.z, sc.z, sh.z), fmaf(v.w, sc.w, sh.w));
+                if (g.post_leaky) {                                       // sign of (leaky(pre) + skip)
+                    float4 k = make_float4(0.f, 0.f, 0.f, 0.f);
+                    if (g.skip_pitch)
+                        k = __ldg(skip + (((long long)n * (g.H >> HS) + (ys >> HS)) * g.skip_pitch + (xs >> HS) + g.skip_off) * g.C4 + c);
+                    s.x = (lk(pre.x, g.slope) + k.x) >= 0.f ? s.x : s.x * g.slope;
+                    s.y = (lk(pre.y, g.slope) + k.y) >= 0.f ? s.y : s.y * g.slope;
+                    s.z = (lk(pre.z, g.slope) + k.z) >= 0.f ? s.z : s.z * g.slope;
+                    s.w = (lk(pre.w, g.slope) + k.w) >= 0.f ? s.w : s.w * g.slope;
+                }
+                t.x += s.x; t.y += s.y; t.z += s.z; t.w += s.w;
+                const float4 a = make_float4(pre.x >= 0.f ? s.x : s.x * g.slope, pre.y >= 0.f ? s.y : s.y * g.slope,
+                                             pre.z >= 0.f ? s.z : s.z * g.slope, pre.w >= 0.f ? s.w : s.w * g.slope);
+                ga[idx] = a;
+                a1.x += a.x; a1.y += a.y; a1.z += a.z; a1.w += a.w;
+                a2.x = fmaf(a.x, (v.x - mu.x) * is.x, a2.x); a2.y = fmaf(a.y, (v.y - mu.y) * is.y, a2.y);
+                a2.z = fmaf(a.z, (v.z - mu.z) * is.z, a2.z); a2.w = fmaf(a.w, (v.w - mu.w) * is.w, a2.w);
             }
-            const long long idx = (((long long)n * g.H + ys) * g.W + xs) * g.C4 + c;
-            const float4 v = __ldg(y + idx);
-            const float4 pre = make_float4(fmaf(v.x, sc.x, sh.x), fmaf(v.y, sc.y, sh.y), fmaf(v.z, sc.z, sh.z), fmaf(v.w, sc.w, sh.w));
-            if (g.post_leaky) {                                       // sign of (leaky(pre) + skip)
-                float4 k = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (g.skip_pitch) k = __ldg(skip + (((long long)n * g.H + ys) * g.skip_pitch + xs + g.skip_off) * g.C4 + c);
-                s.x = (lk(pre.x, g.slope) + k.x) >= 0.f ? s.x : s.x * g.slope;
-                s.y = (lk(pre.y, g.slope) + k.y) >= 0.f ? s.y : s.y * g.slope;
-                s.z = (lk(pre.z, g.slope) + k.z) >= 0.f ? s.z : s.z * g.slope;
-                s.w = (lk(pre.w, g.slope) + k.w) >= 0.f ? s.w : s.w * g.slope;
-            }
-            if (gskip) gskip[(((long long)n * g.H + ys) * gskip_pitch + xs + gskip_off) * g.C4 + c] = s;
-            const float4 a = make_float4(pre.x >= 0.f ? s.x : s.x * g.slope, pre.y >= 0.f ? s.y : s.y * g.slope,
-                                         pre.z >= 0.f ? s.z : s.z * g.slope, pre.w >= 0.f ? s.w : s.w * g.slope);
-            ga[idx] = a;
-            a1.x += a.x; a1.y += a.y; a1.z += a.z; a1.w += a.w;
-            a2.x = fmaf(a.x, (v.x - mu.x) * is.x, a2.x); a2.y = fmaf(a.y, (v.y - mu.y) * is.y, a2.y);
-            a2.z = fmaf(a.z, (v.z - mu.z) * is.z, a2.z); a2.w = fmaf(a.w, (v.w - mu.w) * is.w, a2.w);
+            if (gskip) gskip[(((long long)n * (g.H >> HS) + p / Wq) * gskip_pitch + p % Wq + gskip_off) * g.C4 + c] = t;
         }
         float* s1 = S1 + (long long)n * s_pitch + c * 4;
         float* s2 = S2 + (long long)n * s_pitch + c * 4;
@@ -900,9 +913,12 @@ int b3d_cbn_act_fwd(const float* y, const float* scale, const float* shift, cons
                 "b3d_cbn_act_fwd: bad arguments");
     B3D_REQUIRE(pad_mode == 0 || (pad_mode == 1 && pad <= up * W), B3D_EINVAL, "b3d_cbn_act_fwd: pad mode %d with pad %d > %d columns",
                 pad_mode, pad, up * W);
+    const int skip_sh = skip_pitch < 0;
+    skip_pitch = skip_sh ? -skip_pitch : skip_pitch;
+    B3D_REQUIRE(!skip_sh || (H % 2 == 0 && W % 2 == 0), B3D_EINVAL, "b3d_cbn_act_fwd: a half-resolution skip needs even H, W");
     if (N == 0) return B3D_OK;
     B3D_REQUIRE(y && scale && shift && out && (skip != nullptr) == (skip_pitch != 0), B3D_EINVAL, "b3d_cbn_act_fwd: null pointer");
-    CbnGeom g{N, H, W, C / 4, up, pad, skip_pitch, skip_off, slope, post_leaky};
+    CbnGeom g{N, H, W, C / 4, up, pad, skip_pitch, skip_off, skip_sh, slope, post_leaky};
     const long long total = (long long)N * up * H * (up * W + 2 * pad) * (C / 4);
     cudaStream_t st = (cudaStream_t)stream;
     if (g.C4 <= NT && NT % g.C4 == 0 && (up == 1 || up == 2)) {
@@ -925,7 +941,8 @@ int b3d_cbn_act_fwd(const float* y, const float* scale, const float* shift, cons
 }
 
 // S1, S2 [N,C] are zeroed by the call; gskip (nullable) is written at pixel offset gskip_off with row pitch gskip_pitch
-// (its pad columns are NOT touched: the caller zeroes the buffer when gskip_pitch != W).  stat_pitch: row pitch of mean /
+// (its pad columns are NOT touched: the caller zeroes the buffer when gskip_pitch != W).  skip_pitch, gskip_pitch < 0: the
+// skip has half the resolution (see b3d_cbn_act_fwd) and gskip receives the sum over each 2 x 2 footprint.  stat_pitch: row pitch of mean /
 // inv_std, 0 = one row for all samples (batch statistics), C = per-sample rows (instance / no normalisation).
 int b3d_cbn_act_bwd1(const float* gout, const float* y, const float* scale, const float* shift, const float* skip, int skip_pitch,
                      int skip_off, const float* mean, const float* invstd, int stat_pitch, float* ga, float* gskip, int gskip_pitch,
@@ -936,19 +953,27 @@ int b3d_cbn_act_bwd1(const float* gout, const float* y, const float* scale, cons
     B3D_REQUIRE(stat_pitch == 0 || stat_pitch == C, B3D_EINVAL, "b3d_cbn_act_bwd1: statistics pitch %d must be 0 or C=%d", stat_pitch, C);
     B3D_REQUIRE(pad >= 0 && (pad_mode == 0 || (pad_mode == 1 && pad <= up * W)), B3D_EINVAL,
                 "b3d_cbn_act_bwd1: pad mode %d with pad %d > %d columns", pad_mode, pad, up * W);
+    const int skip_sh = skip_pitch < 0;
+    skip_pitch = skip_sh ? -skip_pitch : skip_pitch;
+    B3D_REQUIRE(skip_sh == (gskip_pitch < 0) || !gskip, B3D_EINVAL, "b3d_cbn_act_bwd1: skip and its gradient differ in resolution");
+    gskip_pitch = gskip_pitch < 0 ? -gskip_pitch : gskip_pitch;
+    B3D_REQUIRE(!skip_sh || (H % 2 == 0 && W % 2 == 0), B3D_EINVAL, "b3d_cbn_act_bwd1: a half-resolution skip needs even H, W");
     if (N == 0) return B3D_OK;
     B3D_REQUIRE(gout && y && scale && shift && mean && invstd && ga && S1 && S2, B3D_EINVAL, "b3d_cbn_act_bwd1: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
     B3D_REQUIRE(s_pitch >= C && s_pitch % 4 == 0, B3D_EINVAL, "b3d_cbn_act_bwd1: S pitch %d must be >= C and a multiple of 4", s_pitch);
     B3D_CUDA_OK(cudaMemset2DAsync(S1, sizeof(float) * (size_t)s_pitch, 0, sizeof(float) * (size_t)C, (size_t)N, st));
     B3D_CUDA_OK(cudaMemset2DAsync(S2, sizeof(float) * (size_t)s_pitch, 0, sizeof(float) * (size_t)C, (size_t)N, st));
-    CbnGeom g{N, H, W, C / 4, up, pad, skip_pitch, skip_off, slope, post_leaky};
+    CbnGeom g{N, H, W, C / 4, up, pad, skip_pitch, skip_off, skip_sh, slope, post_leaky};
     // enough CTAs to fill the GPU a few times, each with >= 1 row
     int rows = (int)(((long long)N * H + 132 * 8 - 1) / (132 * 8));
     rows = rows < 1 ? 1 : rows;
+    rows += skip_sh && rows % 2;                          // a CTA owns whole 2 x 2 footprints of a half-resolution skip
     dim3 grid(b3d::ceil_div(H, rows), N);
-    auto kernel = pad_mode == 0 ? (stat_pitch ? cbn_act_bwd1_kernel<0, true> : cbn_act_bwd1_kernel<0, false>)
-                                : (stat_pitch ? cbn_act_bwd1_kernel<1, true> : cbn_act_bwd1_kernel<1, false>);
+    auto kernel = skip_sh ? (pad_mode == 0 ? (stat_pitch ? cbn_act_bwd1_kernel<0, true, 1> : cbn_act_bwd1_kernel<0, false, 1>)
+                                           : (stat_pitch ? cbn_act_bwd1_kernel<1, true, 1> : cbn_act_bwd1_kernel<1, false, 1>))
+                          : (pad_mode == 0 ? (stat_pitch ? cbn_act_bwd1_kernel<0, true, 0> : cbn_act_bwd1_kernel<0, false, 0>)
+                                           : (stat_pitch ? cbn_act_bwd1_kernel<1, true, 0> : cbn_act_bwd1_kernel<1, false, 0>));
     kernel<<<grid, NT, 0, st>>>((const float4*)gout, (const float4*)y, (const float4*)scale, (const float4*)shift, (const float4*)skip,
                                 (const float4*)mean, (const float4*)invstd, (float4*)ga, (float4*)gskip, gskip_pitch, gskip_off, S1, S2,
                                 s_pitch, g, rows);

@@ -12,6 +12,13 @@
 // Layouts written for the convolution kernels (csrc/tc_conv.cu, thin_kernels.cu):
 //   F [T'][Cout][Cin']   tap-major, K-major rows: fprop B operand, wgrad output layout
 //   D [T'][Cin'][Cout']  per-tap transpose (Cout' = Cout rounded up to 32, zero filled): dgrad B operand
+// 3x3 layers whose input is a x2 nearest upsample (up2 = 1; Cin, Cout multiples of 32) get, in place of D, the layouts
+// of the equivalent stride-2 transposed convolution of the low-resolution input (b3d/conv.py:_up_fprop):
+//   P  [16][Cout][Cin]   phase weights, tap q = ((py*2 + px)*2 + a)*2 + b:
+//                        P[q] = sum_k sum_l A_py[a][k] A_px[b][l] W[k][l],  A_0 = [[1,0,0],[0,1,1]], A_1 = [[1,1,0],[0,0,1]]
+//                        (summed in fp32 from W / sigma, rounded to tf32 once)
+//   D4 [16][Cin][Cout]   P transposed as the taps (r, s) = (3 - py - 2a, 3 - px - 2b) of a 4x4 stride-2 correlation
+//                        (the input gradient)
 // plain (fold = 0): T' = kh*kw, Cin' = Cin rounded up to 32 (zero filled);
 // folded stems (fold = 1, discriminator conv1 with 8 / 11 input channels): the kh vertical taps live in the channel
 // dimension, T' = kw, Cin' = kh*Cin rounded up to 32, F[s][co][r*Cin + c] = W[co][c][r][s] (b3d/conv.py:fold_kh_weight).
@@ -43,7 +50,7 @@ struct alignas(16) BankLayer {
     long long dw_off;    // backward out: gradient in weight_orig layout
     int Cout, Cin, kh, kw;
     int fold, Cinp, Coutp, Tp;
-    int sn, pad0, pad1, pad2;
+    int sn, up2, pad1, pad2;
 };
 
 struct Item { int layer, a, b, c; };
@@ -131,7 +138,20 @@ __device__ __forceinline__ float layer_sigma(const BankLayer& L, const float* sv
     return p / nrm;
 }
 
-// Emit F (and D) for a (32 co) x (32 ci') chunk of all taps; chunk (0,0) also stores u, v, sigma.
+// Row a of A_p (see the layouts above) covers filter rows k = up2_lo(p, a) .. up2_hi(p, a)
+__device__ __forceinline__ int up2_lo(int p, int a) { return p ? 2 * a : a; }
+__device__ __forceinline__ int up2_hi(int p, int a) { return p ? 1 + a : 2 * a; }
+
+// P[q] of one (co, ci) from its nine normalised taps w (row-major k, l)
+__device__ __forceinline__ float up2_phase(const float (&w)[9], int q) {
+    const int py = q >> 3, px = (q >> 2) & 1, a = (q >> 1) & 1, b = q & 1;
+    float v = 0.f;
+    for (int k = up2_lo(py, a); k <= up2_hi(py, a); ++k)
+        for (int l = up2_lo(px, b); l <= up2_hi(px, b); ++l) v += w[k * 3 + l];
+    return v;
+}
+
+// Emit F (and D, or P and D4) for a (32 co) x (32 ci') chunk of all taps; chunk (0,0) also stores u, v, sigma.
 // item: (layer, co chunk, ci' chunk)
 __global__ void __launch_bounds__(NT)
 bank_emit_kernel(const BankLayer* __restrict__ layers, const Item* __restrict__ items, const float* __restrict__ scratch,
@@ -184,6 +204,27 @@ bank_emit_kernel(const BankLayer* __restrict__ layers, const Item* __restrict__ 
         }
     }
     if (L.wd_off < 0) return;
+    if (L.up2) {
+        // P: lanes along ci, D4: lanes along co (coalesced stores); Cin and Cout are multiples of 32
+        float* P = outb + L.wd_off;
+        float* D4 = P + (size_t)16 * L.Cout * L.Cin;
+        for (int pass = 0; pass < 2; ++pass)
+            for (int e = threadIdx.x; e < 32 * 32; e += NT) {
+                const int ci = ci0 + (pass ? e >> 5 : e & 31), co = co0 + (pass ? e & 31 : e >> 5);
+                if (co >= L.Cout || ci >= L.Cin) continue;
+                float w[9];
+#pragma unroll
+                for (int t = 0; t < 9; ++t) w[t] = __ldg(L.w + (co * L.Cin + ci) * 9 + t) * rs;
+                for (int q = 0; q < 16; ++q) {
+                    const float val = tf32_rna(up2_phase(w, q), round_tf32);
+                    const int py = q >> 3, px = (q >> 2) & 1, a = (q >> 1) & 1, b = q & 1;
+                    const int t4 = (3 - py - 2 * a) * 4 + 3 - px - 2 * b;
+                    if (pass) D4[((size_t)t4 * L.Cin + ci) * L.Cout + co] = val;
+                    else P[((size_t)q * L.Cout + co) * L.Cin + ci] = val;
+                }
+            }
+        return;
+    }
     // D: lanes along co' (coalesced stores); rows co >= Cout are zero
     const int cop0 = it.a * 32;
     for (int e = threadIdx.x; e < 32 * 32; e += NT) {
@@ -254,9 +295,46 @@ bank_bwd_emit_kernel(const BankLayer* __restrict__ layers, const Item* __restric
     }
 }
 
+// Adjoint of P for one 32 x 32 (ci, co) tile: dF[k*3 + l][co][ci] += sum over the taps q with A_py[a][k] A_px[b][l] = 1 of
+// dPt[t4(q)][ci][co], where dPt [16][Cin][Cout] is the weight gradient of the 4x4 stride-2 correlation that computes the
+// input gradient (taps t4 as in D4).  Read along co, transposed through shared memory, added along ci.
+__global__ void __launch_bounds__(NT)
+up2_fold_kernel(const float* __restrict__ dpt, float* __restrict__ df, int Cout, int Cin) {
+    __shared__ float tile[9][32][33];
+    const int co0 = blockIdx.x * 32, ci0 = blockIdx.y * 32;
+    for (int e = threadIdx.x; e < 32 * 32; e += NT) {
+        const int co = e & 31, ci = e >> 5;
+        float acc[9] = {};
+        for (int q = 0; q < 16; ++q) {
+            const int py = q >> 3, px = (q >> 2) & 1, a = (q >> 1) & 1, b = q & 1;
+            const int t4 = (3 - py - 2 * a) * 4 + 3 - px - 2 * b;
+            const float g = __ldg(dpt + ((size_t)t4 * Cin + ci0 + ci) * Cout + co0 + co);
+            for (int k = up2_lo(py, a); k <= up2_hi(py, a); ++k)
+                for (int l = up2_lo(px, b); l <= up2_hi(px, b); ++l) acc[k * 3 + l] += g;
+        }
+#pragma unroll
+        for (int t = 0; t < 9; ++t) tile[t][co][ci] = acc[t];
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < 32 * 32; e += NT) {
+        const int ci = e & 31, co = e >> 5;
+#pragma unroll
+        for (int t = 0; t < 9; ++t) df[((size_t)t * Cout + co0 + co) * Cin + ci0 + ci] += tile[t][co][ci];
+    }
+}
+
 }  // namespace
 
 extern "C" {
+
+// dpt [16][Cin][Cout] -> accumulated into df [9][Cout][Cin] (the F-layout gradient sink of a 3x3 layer with up2 = 1)
+int b3d_up2_fold(const float* dpt, float* df, int Cout, int Cin, void* stream) {
+    B3D_REQUIRE(dpt && df && Cout > 0 && Cin > 0 && Cout % 32 == 0 && Cin % 32 == 0, B3D_EINVAL,
+                "b3d_up2_fold: bad arguments (Cout=%d, Cin=%d must be multiples of 32)", Cout, Cin);
+    up2_fold_kernel<<<dim3(Cout / 32, Cin / 32), NT, 0, (cudaStream_t)stream>>>(dpt, df, Cout, Cin);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
 
 int b3d_bank_layer_bytes(void) { return (int)sizeof(BankLayer); }
 

@@ -219,6 +219,14 @@ inline EncodeTiledFn encode_fn() {
 inline int make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_b,
                          const uint32_t* box, const uint32_t* elem_strides = nullptr,
                          CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+    // The encoder needs a current context, and a host thread that has made no runtime call yet has none (autograd's
+    // worker threads, when a convolution's backward is the first thing they run): cudaSetDevice makes the device's primary
+    // context current, once per thread (allowed during stream capture).
+    thread_local bool ctx_bound = false;
+    if (!ctx_bound) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) == cudaSuccess && cudaSetDevice(dev) == cudaSuccess) ctx_bound = true;
+    }
     EncodeTiledFn fn = encode_fn();
     if (!fn) {
         b3d::set_error("cuTensorMapEncodeTiled is not available from the driver");

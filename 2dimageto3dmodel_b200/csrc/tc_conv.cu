@@ -891,7 +891,16 @@ int b3d_conv2d_tf32(const float* x, const float* wt, const float* bias, float* o
         B3D_REQUIRE(fold_kh <= 8 && Cin == 32 * ((8 * fold_kh + 31) / 32) && sy == 1 && sx == 1 && !wtap && Wout % BM == 0,
                     B3D_EINVAL, "b3d_conv2d_tf32: on-the-fly fold needs 8 input channels, stride 1 and Wout %% 128 == 0 (Wout=%d)", Wout);
     }
-    B3D_REQUIRE(!stats || mask || (osy == 1 && osx == 1), B3D_EINVAL, "b3d_conv2d_tf32: statistics need a dense output");
+    // statistics are taken over the pixels the launch writes: the whole output when it is dense, or when four parity classes
+    // at output stride 2 tile it (the forward of a 3x3 convolution of a x2-upsampled input, b3d/conv.py:_up_fprop)
+    bool tiles = ncls == 4 && osy == 2 && osx == 2 && OH == 2 * Hout && OW == 2 * Wout;
+    for (int c = 0, seen = 0; tiles && c < 4; ++c) {
+        const int bit = 1 << (2 * cooy[c] + coox[c]);
+        tiles = cooy[c] >= 0 && cooy[c] <= 1 && coox[c] >= 0 && coox[c] <= 1 && !(seen & bit);
+        seen |= bit;
+    }
+    B3D_REQUIRE(!stats || mask || (osy == 1 && osx == 1) || tiles, B3D_EINVAL,
+                "b3d_conv2d_tf32: statistics need a dense output, or four parity classes that tile it");
     // 256-wide output-channel tiles halve the input-tile bytes per FLOP through the L2 -> SM path when there are >= 256
     // output channels and enough work items to give every SM one.  Every launch of cfg3, cfg4 and cfg5 this rule gives
     // 256-wide tiles, timed against the same kernels forced to 128 (tools/time_conv128.py, H100 SXM, 700 W): 256 wins on
@@ -1019,7 +1028,8 @@ int b3d_conv2d_wgrad_tf32(const float* dy, const float* x, float* dw, int N, int
                           void* stream) {
     B3D_REQUIRE(N > 0 && Cin > 0 && Cout > 0 && H > 0 && W > 0 && Hout > 0 && Wout > 0, B3D_EINVAL,
                 "b3d_conv2d_wgrad_tf32: bad sizes");
-    B3D_REQUIRE(kh * kw <= MAX_TAPS && (stride == 1 || stride == 2) && x_off >= 0, B3D_EINVAL, "b3d_conv2d_wgrad_tf32: bad kernel/stride");
+    // x_off < 0: the first taps of a row read left of x; TMA fills those columns with zeros
+    B3D_REQUIRE(kh * kw <= MAX_TAPS && (stride == 1 || stride == 2) && x_off > -kw, B3D_EINVAL, "b3d_conv2d_wgrad_tf32: bad kernel/stride");
     B3D_REQUIRE(dy && x && dw, B3D_EINVAL, "b3d_conv2d_wgrad_tf32: null pointer");
     B3D_REQUIRE(Cin % 32 == 0 && Cout % 32 == 0, B3D_EINVAL,
                 "b3d_conv2d_wgrad_tf32: Cin=%d and Cout=%d must be multiples of 32 (pad the channels with zeros)", Cin, Cout);

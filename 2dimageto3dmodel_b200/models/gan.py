@@ -19,7 +19,7 @@ import torch.nn.functional as F
 from b3d import B3DError
 from b3d.bank import WeightBank
 from b3d.conv import conv2d as _tc_conv2d
-from b3d.conv import ActLink, conv2d_banked
+from b3d.conv import ActLink, conv2d_banked, conv2d_up2_banked
 from b3d.ew import CIRCULAR, REPLICATE, CBNBatch, cbn_act_pad, identity_norm, in_act_pad, norm_kind, pad_x, stem_input
 from rendering.utils import adjust_poles, symmetrize_texture
 
@@ -367,6 +367,20 @@ class ResBlockUp(nn.Module):
         return cbn_act_pad(y2, self.norm2, z, skip_nchw=skip, skip_off=off, up=up, pad=pad_next, post_leaky=post_leaky, cb=cb,
                            sums=s2, pad_mode=pad_mode)
 
+    def forward_fused_up(self, xp, z, pad_next, W, prefix, cb, post_leaky=False, pad_mode=REPLICATE):
+        """forward_fused(pad(up(x), 1), z, up=1, ...) from the LOW-resolution xp = pad(x, 1) alone: conv1 runs as a stride-2
+        transposed convolution of xp and the 1x1 shortcut before the upsample (b3d.conv.conv2d_up2_banked, conv1 registered
+        with up2 in the bank W), and the second glue pass adds the residual from (y/2, x/2).  The upsampled map is never
+        written, in the forward or the backward."""
+        s1, s2 = cb.stats_slot(self.norm1), cb.stats_slot(self.norm2)
+        has_sc = isinstance(self.shortcut, nn.Module)
+        y1, skip = conv2d_up2_banked(xp, W[prefix + ".conv1"], W[prefix + ".shortcut"] if has_sc else None, stats=s1)
+        a = cbn_act_pad(y1, self.norm1, z, up=1, pad=1, cb=cb, sums=s1, pad_mode=pad_mode)
+        y2 = conv2d_banked(a, W[prefix + ".conv2"], pad_y=1, stats=s2)
+        skip, off = (skip, 0) if has_sc else (xp, 1)                 # identity: the interior of the padded input
+        return cbn_act_pad(y2, self.norm2, z, skip_nchw=skip, skip_off=off, skip_half=True, up=1, pad=pad_next,
+                           post_leaky=post_leaky, cb=cb, sums=s2, pad_mode=pad_mode)
+
 
 class Generator(nn.Module):
     def __init__(self, args, emb_dim, symmetric=True, mesh_head=True):
@@ -456,6 +470,9 @@ class Generator(nn.Module):
                 attention_map = symmetrize_texture(attention_map)
         return (x_tex, x_mesh, attention_map) if return_attention else (x_tex, x_mesh)
 
+    # blocks whose input is the previous block's x2 upsampled output (their conv1 runs on the low-resolution map)
+    UP_BLOCKS = ('blk2', 'blk3a', 'blk3b', 'blk3c', 'blk4', 'blk5', 'blk6', 'blk3_mesh')
+
     def _weights(self):
         """Spectral norm + kernel layouts of every convolution of the generator in one WeightBank pass (b3d/bank.py)."""
         if getattr(self, 'disable_bank', False):
@@ -473,7 +490,7 @@ class Generator(nn.Module):
             convs["conv_final"] = self.conv_final
             if self.mesh_head:
                 convs["conv_mesh"] = self.conv_mesh
-            bank = self.__dict__['_bank'] = WeightBank(convs)
+            bank = self.__dict__['_bank'] = WeightBank(convs, up2=[n + ".conv1" for n in self.UP_BLOCKS])
         return bank.forward(self.training)
 
     def _forward_fused(self, x, z, return_attention):
@@ -487,7 +504,13 @@ class Generator(nn.Module):
             names.append('blk3_mesh')
         # gamma / beta of all conditional batch norms from one GEMM (blk1.norm1 first: it closes the gradient sink)
         cb = CBNBatch([m for n in names for m in (getattr(self, n).norm1, getattr(self, n).norm2)], z)
-        blk = lambda name, inp, **kw: getattr(self, name).forward_fused(inp, z, W=W, prefix=name, cb=cb, pad_mode=pm, **kw)
+
+        def blk(name, inp, up=2, pad_next=1, post_leaky=False):
+            b = getattr(self, name)
+            if W is not None and name in self.UP_BLOCKS:       # low-resolution maps between the blocks
+                return b.forward_fused_up(inp, z, pad_next, W, name, cb, post_leaky=post_leaky, pad_mode=pm)
+            return b.forward_fused(inp, z, up=1 if W is not None else up, pad_next=pad_next, post_leaky=post_leaky, W=W, prefix=name,
+                                   cb=cb, pad_mode=pm)
         head = (lambda conv, name, inp: conv(inp)) if W is None else (lambda conv, name, inp: conv2d_banked(inp, W[name], pad_y=2))
         sym = symmetrize_texture if self.symmetric else (lambda t: t)
         p = pad_x(x, 1, pm)

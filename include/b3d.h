@@ -386,6 +386,10 @@ B3D_API int b3d_bank_forward(const void* layers, const void* items_wtu, int n_wt
                              int training, void* stream);
 B3D_API int b3d_bank_backward(const void* layers, const void* items_dot, int n_dot, const void* items_emit, int n_emit,
                               float* out, const float* df, float* dw, void* stream);
+/* Layers with up2 = 1 (a 3x3 convolution of a x2 nearest-upsampled input) get the phase weights P [16][Cout][Cin] and
+ * their 4x4 transposed layout D4 [16][Cin][Cout] in place of D (csrc/sn_kernels.cu).  b3d_up2_fold accumulates the
+ * adjoint of P, from the gradient dpt [16][Cin][Cout] in D4's tap order, into the layer's F-layout sink df [9][Cout][Cin]. */
+B3D_API int b3d_up2_fold(const float* dpt, float* df, int Cout, int Cin, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * One-pass NHWC helpers between the GAN's convolutions.
@@ -429,6 +433,9 @@ B3D_API int b3d_leaky_bwd(const float* gy, const float* y, float* out, long long
  *   out[n, yo, xo, :] = post( leaky(y[n,ys,xs,:] * scale[n,:] + shift[n,:]) + skip[n,ys,xs,:] ),
  *   (ys, xs) = (yo / up, clamp(xo - pad, 0, up*W-1) / up);  out [N, up*H, up*W + 2*pad, C];  scale = inv_std*(1+gamma),
  *   shift = beta - mean*scale ([N,C]); skip (nullable) is read at row pitch skip_pitch, pixel offset skip_off.
+ *   skip_pitch < 0: the skip has half y's resolution (H, W even) and row pitch -skip_pitch; pixel (ys, xs) adds skip
+ *   pixel (ys/2, xs/2), i.e. a x2 nearest upsample of it.  bwd1 then takes gskip_pitch < 0 too and writes the sum over
+ *   each 2 x 2 footprint into gskip (one thread per footprint: a fixed summation order).
  *   pad_mode 0 = replicate (the clamp above), 1 = circular for the asymmetric generator and the discriminators (pad <= up*W;
  *   the column wraps in upsampled coordinates, bwd1 folds every pad column back onto the column it copies).
  * bwd1: gout -> ga = d/d(pre-activation) [N,H,W,C], gskip (nullable), S1[n,c] = sum ga, S2[n,c] = sum ga*xhat: rows of

@@ -125,6 +125,7 @@ _sig("b3d_mesh_raster_attr_bwd", _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _f, _f, _
 _sig("b3d_texel_visibility", _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp)
 _sig("b3d_pseudogt_pack", _vp, _i, _i, _vp, _vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp, _vp, _vp)
 _sig("b3d_sample_pack", _vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp)
+_sig("b3d_recon_texture_pack", _vp, _i, _i, _vp, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp)
 
 
 def mode_id(mode):

@@ -4,7 +4,8 @@ mirroring).  The stores may sit in device memory or in pinned host memory (read 
 b3d_image_batch: one launch that builds a reconstruction batch (crop, cv2-style resize, mirror, poses) from packed photo
 windows in device memory.
 b3d_pseudogt_pack: one launch that masks, transposes and rounds a batch of pseudo-ground-truth records to fp16.
-b3d_sample_pack: one launch that turns a batch of sample renders and textures into the bytes of their PNGs."""
+b3d_sample_pack: one launch that turns a batch of sample renders and textures into the bytes of their PNGs.
+b3d_recon_texture_pack: one launch that builds the texture bytes of a batch of exported reconstructions."""
 import ctypes
 
 import torch
@@ -172,3 +173,36 @@ def sample_pack(image, imidx, tex, tiles_out, tex8_out):
                            "fallback")
     check(lib.b3d_sample_pack(ptr(image), ptr(imidx), B, H, W, ptr(tex), T, ptr(tiles_out), ptr(tex8_out),
                               stream_ptr(image)))
+
+
+def recon_texture_pack(vis, proj, alpha, pred, symmetric, tex8_out, src8_out):
+    """b3d_recon_texture_pack: one launch builds the textures of a batch of exported reconstructions.
+    vis uint8 [B,Th,Tw] (texel visibility), proj fp32 [B,R,R,3] and alpha fp32 [B,R,R,1] (the photo projected into UV
+    space and its hard mask), pred fp32 [B,3,T,T] (the network's texture) -> tex8_out uint8 [B,R,R,3], src8_out uint8
+    [B,R,R]: the projection where the pseudo-ground-truth mask keeps it (source 1), with a symmetric template its mirror
+    image where only that is kept (source 2), pred bilinearly resampled to R elsewhere (source 0); bytes as sample_pack's
+    tex8.  R even; all tensors contiguous on the device.  Shapes are checked before the device."""
+    def need(t, dtype, name, dim):
+        if not (isinstance(t, torch.Tensor) and t.dtype == dtype and t.dim() == dim and t.is_contiguous()):
+            raise B3DError(f"recon_texture_pack: {name} must be a contiguous {dtype} tensor with {dim} dimensions")
+    need(vis, torch.uint8, 'vis', 3)
+    need(proj, torch.float32, 'proj', 4)
+    need(alpha, torch.float32, 'alpha', 4)
+    need(pred, torch.float32, 'pred', 4)
+    need(tex8_out, torch.uint8, 'tex8_out', 4)
+    need(src8_out, torch.uint8, 'src8_out', 3)
+    B, Th, Tw = vis.shape
+    R, T = proj.shape[1], pred.shape[2]
+    if R % 2:
+        raise B3DError(f"recon_texture_pack: R {R} is odd; the mirrored column map needs an even resolution")
+    for name, t, shape in (('proj', proj, (B, R, R, 3)), ('alpha', alpha, (B, R, R, 1)), ('pred', pred, (B, 3, T, T)),
+                           ('tex8_out', tex8_out, (B, R, R, 3)), ('src8_out', src8_out, (B, R, R))):
+        if tuple(t.shape) != shape:
+            raise B3DError(f"recon_texture_pack: {name} has shape {tuple(t.shape)}; expected {list(shape)}")
+    for name, t in (('vis', vis), ('proj', proj), ('alpha', alpha), ('pred', pred), ('tex8_out', tex8_out),
+                    ('src8_out', src8_out)):
+        if not t.is_cuda:
+            raise B3DError(f"recon_texture_pack: {name} is on {t.device}; libb3d runs on CUDA tensors only, there is no "
+                           "CPU fallback")
+    check(lib.b3d_recon_texture_pack(ptr(vis), Th, Tw, ptr(proj), ptr(alpha), B, R, ptr(pred), T, int(bool(symmetric)),
+                                     ptr(tex8_out), ptr(src8_out), stream_ptr(proj)))

@@ -32,6 +32,6 @@ void count_launch(int n) { g_launches.fetch_add((uint64_t)n, std::memory_order_r
 extern "C" {
 const char* b3d_last_error(void) { return b3d::g_err; }
 const char* b3d_last_variant(void) { return b3d::g_variant; }
-int b3d_version(void) { return 430; }   // 4.3: x2-upsampled 3x3 convolutions as stride-2 transposed convolutions of the low-resolution map
+int b3d_version(void) { return 440; }   // 4.4: b3d_recon_texture_pack, the reconstruction export's texture
 uint64_t b3d_launch_count(void) { return b3d::g_launches.load(std::memory_order_relaxed); }
 }

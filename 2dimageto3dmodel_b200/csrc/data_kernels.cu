@@ -395,6 +395,85 @@ __global__ void __launch_bounds__(PACK_NT) sample_pack_kernel(const __grid_const
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Reconstruction export: the final texture of one exported mesh.  Each texel takes the photo projected into UV space
+// where the pseudo-ground-truth mask would keep it, its mirror image across the template's symmetry plane where only that
+// one is kept, and the network's texture resampled to R elsewhere; quantised as the sample export quantises.
+
+struct ReconPackArgs {
+    const uint8_t* vis;      // [B, Th, Tw] 0 / 1
+    int Th, Tw;
+    float sy, sx;            // Th / R, Tw / R
+    const float* proj;       // [B, R, R, 3]
+    const float* alpha;      // [B, R, R, 1]
+    int R;
+    const float* pred;       // [B, 3, T, T]
+    int T;
+    float st;                // T / R
+    int symmetric;
+    long long total;         // B R R
+    uint8_t* tex8;           // [B, R, R, 3]
+    uint8_t* src8;           // [B, R, R]
+};
+
+// b3d_pseudogt_pack's mask pixel (y, x) of sample b, and the projection's hard mask there
+__device__ __forceinline__ bool recon_valid(const ReconPackArgs& a, long long b, int y, int x) {
+    const long long t = (b * a.R + y) * a.R + x;
+    if (!(a.alpha[t] > 0.f)) return false;
+    int y0, y1, x0, x1;
+    bool uy, ux;
+    mask_taps(y, a.Th, a.sy, y0, y1, uy);
+    mask_taps(x, a.Tw, a.sx, x0, x1, ux);
+    const uint8_t* v = a.vis + b * a.Th * a.Tw;
+    return v[y0 * a.Tw + x0] || (ux && v[y0 * a.Tw + x1]) || (uy && (v[y1 * a.Tw + x0] || (ux && v[y1 * a.Tw + x1])));
+}
+
+// upsample_bilinear2d's taps (align_corners=False) as mask_taps computes them, with the weight of the second tap
+__device__ __forceinline__ void bilinear_taps(int d, int in, float scale, int& i0, int& i1, float& l1) {
+    float src = __fmaf_rn(scale, (float)d + 0.5f, -0.5f);
+    if (src < 0.f) src = 0.f;
+    i0 = (int)src;
+    i1 = i0 + (i0 < in - 1 ? 1 : 0);
+    l1 = __fsub_rn(src, (float)i0);
+}
+
+__global__ void __launch_bounds__(PACK_NT) recon_texture_pack_kernel(const __grid_constant__ ReconPackArgs a) {
+    const long long t = (long long)blockIdx.x * PACK_NT + threadIdx.x;
+    if (t >= a.total) return;
+    const long long plane = (long long)a.R * a.R;
+    const long long b = t / plane;
+    const int pos = (int)(t - b * plane), y = pos / a.R, x = pos - y * a.R;
+    int src = 0;
+    long long from = t;
+    if (recon_valid(a, b, y, x)) {
+        src = 1;
+    } else if (a.symmetric) {
+        const int mx = a.R - 1 - (x + a.R / 2) % a.R;        // data.pseudo_gt.mirror_tex's column map
+        if (recon_valid(a, b, y, mx)) {
+            src = 2;
+            from = t - x + mx;
+        }
+    }
+    if (src) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) a.tex8[t * 3 + c] = to_byte(to_unit(a.proj[from * 3 + c]));
+    } else {
+        int y0, y1, x0, x1;
+        float ly, lx;
+        bilinear_taps(y, a.T, a.st, y0, y1, ly);
+        bilinear_taps(x, a.T, a.st, x0, x1, lx);
+        const float hy = __fsub_rn(1.f, ly), hx = __fsub_rn(1.f, lx);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const float* p = a.pred + (b * 3 + c) * a.T * a.T;
+            const float top = __fadd_rn(__fmul_rn(hx, p[y0 * a.T + x0]), __fmul_rn(lx, p[y0 * a.T + x1]));
+            const float bot = __fadd_rn(__fmul_rn(hx, p[y1 * a.T + x0]), __fmul_rn(lx, p[y1 * a.T + x1]));
+            a.tex8[t * 3 + c] = to_byte(to_unit(__fadd_rn(__fmul_rn(hy, top), __fmul_rn(ly, bot))));
+        }
+    }
+    a.src8[t] = (uint8_t)src;
+}
+
 int check_device_ptr(const void* p, const char* what, const char* fn = "b3d_image_batch") {
     cudaPointerAttributes at;
     B3D_CUDA_OK(cudaPointerGetAttributes(&at, p));
@@ -550,6 +629,34 @@ int b3d_sample_pack(const float* image, const int32_t* imidx, int B, int H, int 
         if (rc != B3D_OK) return rc;
     }
     sample_pack_kernel<<<(unsigned)blocks, PACK_NT, 0, (cudaStream_t)stream>>>(a);
+    B3D_LAUNCH_OK();
+    return B3D_OK;
+}
+
+int b3d_recon_texture_pack(const uint8_t* vis, int Th, int Tw, const float* proj, const float* alpha, int B, int R,
+                           const float* pred, int T, int symmetric, uint8_t* tex8, uint8_t* src8, void* stream) {
+    B3D_REQUIRE(B >= 0 && Th >= 1 && Tw >= 1 && R >= 2 && T >= 1, B3D_EINVAL,
+                "b3d_recon_texture_pack: bad sizes (B %d, visibility %d x %d, R %d, texture %d)", B, Th, Tw, R, T);
+    B3D_REQUIRE(R % 2 == 0, B3D_EINVAL,
+                "b3d_recon_texture_pack: R %d is odd; the mirrored column map needs an even resolution", R);
+    if (B == 0) return B3D_OK;
+    ReconPackArgs a = {};
+    a.vis = vis, a.Th = Th, a.Tw = Tw;
+    a.sy = (float)Th / (float)R, a.sx = (float)Tw / (float)R;
+    a.proj = proj, a.alpha = alpha, a.R = R, a.pred = pred, a.T = T, a.st = (float)T / (float)R;
+    a.symmetric = symmetric ? 1 : 0;
+    a.total = (long long)B * R * R;
+    a.tex8 = tex8, a.src8 = src8;
+    const long long blocks = (a.total + PACK_NT - 1) / PACK_NT;
+    B3D_REQUIRE(blocks < (1LL << 31), B3D_EINVAL, "b3d_recon_texture_pack: batch too large");
+    const void* ptrs[] = {vis, proj, alpha, pred, tex8, src8};
+    const char* names[] = {"vis", "proj", "alpha", "pred", "tex8", "src8"};
+    for (int i = 0; i < 6; ++i) {
+        B3D_REQUIRE(ptrs[i], B3D_EINVAL, "b3d_recon_texture_pack: null %s", names[i]);
+        const int rc = check_device_ptr(ptrs[i], names[i], "b3d_recon_texture_pack");
+        if (rc != B3D_OK) return rc;
+    }
+    recon_texture_pack_kernel<<<(unsigned)blocks, PACK_NT, 0, (cudaStream_t)stream>>>(a);
     B3D_LAUNCH_OK();
     return B3D_OK;
 }

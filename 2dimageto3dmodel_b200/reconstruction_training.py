@@ -31,6 +31,31 @@ from rendering.utils import qmul, qrot
 from utils.losses import loss_flat
 
 
+TURNTABLE_ANGLES = (0, 45, 90, 135, 180, 225, 270, 315)
+
+
+def turntable_rotations(device):
+    """The quaternions of run_reconstruction.py's eight turntable views (:188-221), fp32 [8,4]: a fixed tilt, then each
+    angle of TURNTABLE_ANGLES, scaled by 0.8, about the vertical axis."""
+    rad = -90 / 180 * np.pi
+    q0 = torch.tensor([np.cos(-rad / 2), 0, 0, np.sin(-rad / 2)], dtype=torch.float32, device=device)
+    rad = 110 / 180 * np.pi
+    q1 = torch.tensor([np.cos(-rad / 2), 0, np.sin(-rad / 2), 0], dtype=torch.float32, device=device)
+    q0 = qmul(q0, q1)
+    rot = []
+    for angle in TURNTABLE_ANGLES:
+        rad = angle / 180 * np.pi * 0.8
+        rot.append(qmul(q0, torch.tensor([np.cos(-rad / 2), 0, 0, np.sin(-rad / 2)], dtype=torch.float32, device=device)))
+    return torch.stack(rot, dim=0)
+
+
+def turntable_vertices(rot, raw):
+    """Camera-space vertices of object-space vertices raw [N,V,3] seen from the views rot [N,4] (:209-211)."""
+    vtx = qrot(rot, raw) * 0.9
+    vtx[:, :, 1:] *= -1
+    return vtx
+
+
 def default_args(**kw):
     """run_reconstruction.py's argparse defaults (:37-65) for the fields the step and the epoch loop read."""
     a = dict(symmetric=True, texture_resolution=128, mesh_resolution=32, image_resolution=256, loss='mse',
@@ -224,22 +249,10 @@ class ReconTrainer:
     def render_multiview(self, raw_vtx, pred_tex, idx=0):
         """Sample `idx` (object-space vertices raw_vtx [B,V,3], texture pred_tex [B,3,T,T]) rendered from the reference's
         eight turntable views (:188-221) in one batch-8 render -> numpy [2R, 4R, 3] tile (rows of four views) in [0, 1]."""
-        d = raw_vtx.device
-        rad = -90 / 180 * np.pi
-        q0 = torch.tensor([np.cos(-rad / 2), 0, 0, np.sin(-rad / 2)], dtype=torch.float32, device=d)
-        rad = 110 / 180 * np.pi
-        q1 = torch.tensor([np.cos(-rad / 2), 0, np.sin(-rad / 2), 0], dtype=torch.float32, device=d)
-        q0 = qmul(q0, q1)
-        rot = []
-        for angle in (0, 45, 90, 135, 180, 225, 270, 315):
-            rad = angle / 180 * np.pi * 0.8
-            rot.append(qmul(q0, torch.tensor([np.cos(-rad / 2), 0, 0, np.sin(-rad / 2)], dtype=torch.float32, device=d)))
-        rot = torch.stack(rot, dim=0)
+        rot = turntable_rotations(raw_vtx.device)
         raw = raw_vtx[idx:idx + 1].expand(len(rot), -1, -1).contiguous()
         tex = pred_tex[idx:idx + 1].expand(len(rot), -1, -1, -1).contiguous()
-        vtx = qrot(rot, raw) * 0.9
-        vtx[:, :, 1:] *= -1
-        view, _ = self.tpl.forward_renderer(self.renderer, vtx, tex)
+        view, _ = self.tpl.forward_renderer(self.renderer, turntable_vertices(rot, raw), tex)
         R = view.shape[1]
         tile = view.view(2, 4, R, view.shape[2], 3).permute(0, 2, 1, 3, 4).reshape(2 * R, 4 * view.shape[2], 3)
         return (tile.cpu().numpy() + 1) / 2

@@ -17,6 +17,8 @@ SCRIPT = 'run_reconstruction.py'
 DEBUG_IDS = {'p3d': [6, 9, 16, 23, 34, 39, 40, 54, 60, 61, 64, 66, 67, 75, 77, 84],
              'cub': [0, 1, 12, 18, 20, 42, 72, 100, 101, 115, 123, 125, 142, 158, 188, 203]}
 INCEPTION_RES = 299
+# --mesh_path autodetect (run_reconstruction.py:70-76)
+MESH_PATHS = {'p3d': 'mesh_templates/uvsphere_31rings.obj', 'cub': 'mesh_templates/uvsphere_16rings.obj'}
 
 
 def build_parser():
@@ -58,7 +60,7 @@ def derive_settings(args):
     if args.mesh_path == 'autodetect':
         if args.dataset not in ('cub', 'p3d'):
             raise ValueError('Invalid dataset')
-        args.mesh_path = {'p3d': 'mesh_templates/uvsphere_31rings.obj', 'cub': 'mesh_templates/uvsphere_16rings.obj'}[args.dataset]
+        args.mesh_path = MESH_PATHS[args.dataset]
         print('Using autodetected mesh', args.mesh_path)
     if args.generate_pseudogt:
         renderer_res = max(1024, 2 * args.pseudogt_resolution)

@@ -589,6 +589,23 @@ B3D_API int b3d_pseudogt_pack(const uint8_t* vis, int Th, int Tw, const float* t
 B3D_API int b3d_sample_pack(const float* image, const int32_t* imidx, int B, int H, int W, const float* tex, int T,
                             uint8_t* tiles, uint8_t* tex8, void* stream);
 
+/* ---- Reconstruction export: the texture of one exported mesh --------------------------------------------------------
+ * b3d_recon_texture_pack  vis [B,Th,Tw] uint8 (b3d_texel_visibility), proj [B,R,R,3] and alpha [B,R,R,1] fp32 (the photo
+ *                  projected into UV space and its hard mask, InverseRenderer), pred [B,3,T,T] fp32 in [-1, 1] (the
+ *                  network's texture) -> tex8 [B,R,R,3] uint8 and src8 [B,R,R] uint8, the source of each texel:
+ *                    valid(y, x) = b3d_pseudogt_pack's mask pixel (y, x) && alpha(y, x) > 0
+ *                    valid(y, x)                                  -> proj(y, x),  source 1
+ *                    symmetric && valid(y, mx)                    -> proj(y, mx), source 2, mx = R-1-((x + R/2) mod R)
+ *                                                                    (data.pseudo_gt.mirror_tex's column map)
+ *                    otherwise                                    -> pred at (y, x), source 0: upsample_bilinear2d to R
+ *                                                                    (align_corners=False), taps as b3d_pseudogt_pack's,
+ *                                                                    h0 (w0 a + w1 b) + h1 (w0 c + w1 d), no fused
+ *                                                                    multiply-add
+ *                  Bytes as b3d_sample_pack's tex8: x / 2 + 0.5, * 255, clamp to [0, 255], truncation.  R must be even
+ *                  and every pointer device memory (B3D_EINVAL otherwise).                                              */
+B3D_API int b3d_recon_texture_pack(const uint8_t* vis, int Th, int Tw, const float* proj, const float* alpha, int B, int R,
+                                   const float* pred, int T, int symmetric, uint8_t* tex8, uint8_t* src8, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -281,14 +281,20 @@ def _window(lo, hi, n, size, flip):
     return i0, max(i0, i1)
 
 
-def rasterize(p3d, p2d, normalz, attr, H, W, expand=EXPAND, knum=KNUM, multiplier=MULTIPLIER, delta=DELTA):
+def rasterize(p3d, p2d, normalz, attr, H, W, expand=EXPAND, knum=KNUM, multiplier=MULTIPLIER, delta=DELTA,
+              record=None):
     """kaolin linear_rasterizer restated from SURVEY.md App. B (PARITY UNPINNED).
 
     p3d [B,F,9], p2d [B,F,6], normalz [B,F,1], attr [B,F,3d] ->
       imfeat [B,H,W,d], improb [B,H,W,1], imidx [B,H,W] int32 (face+1, 0 = background), imwei [B,H,W,3].
     Differentiable w.r.t. p2d and attr (not p3d / normalz), like kaolin's backward.
     The loops run face by face in face order, like kaolin's per-pixel loops; per face only the pixel
-    window that can pass its (expanded) bounding-box test is touched (an exact restriction)."""
+    window that can pass its (expanded) bounding-box test is touched (an exact restriction).
+
+    record: an optional dict that receives every discrete decision behind each pixel (see `_Record`); the outputs
+    are the same with or without it."""
+    rec = _Record(B=p2d.shape[0], H=H, W=W, dev=p2d.device, multiplier=multiplier, knum=knum) \
+        if record is not None else None
     assert multiplier == MULTIPLIER
     B, Fn, _ = p2d.shape
     d = attr.shape[2] // 3
@@ -361,6 +367,10 @@ def rasterize(p3d, p2d, normalz, attr, H, W, expand=EXPAND, knum=KNUM, multiplie
             near = (xs >= xmin[b, f] - e) & (xs < xmax[b, f] + e) & (ys >= ymin[b, f] - e) & (ys < ymax[b, f] + e)
             cnt = count[b, r0:r1, c0:c1]
             use = near & (~covered[b, r0:r1, c0:c1]) & (cnt < knum)
+            if rec is not None:
+                bounds = (xmin[b, f] - e, xmax[b, f] + e, ymin[b, f] - e, ymax[b, f] + e)
+                rec.face(b, f, r0, r1, c0, c1, xs, ys, Pm[b, f].detach(), bounds, near, use,
+                         (~covered[b, r0:r1, c0:c1]) & (cnt < knum), covered[b, r0:r1, c0:c1], delta)
             if not bool(use.any()):
                 continue
             a = Pm[b, f]
@@ -373,6 +383,8 @@ def rasterize(p3d, p2d, normalz, attr, H, W, expand=EXPAND, knum=KNUM, multiplie
             count[b, r0:r1, c0:c1] = cnt + use.to(torch.int32)
     log_keep = _SumWindows.apply((B, H, W), [p[:5] for p in pieces], x0, *[p[5] for p in pieces])
     improb = torch.where(covered, torch.ones_like(log_keep), 1 - torch.exp(log_keep))
+    if rec is not None:
+        record.update(rec.finish(imidx, count))
     return imfeat, improb.unsqueeze(-1), imidx, imwei
 
 
@@ -390,6 +402,183 @@ class _SumWindows(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         return (None, None, None) + tuple(g[b, r0:r1, c0:c1] for (b, r0, r1, c0, c1) in ctx.wins)
+
+
+# ---------------------------------------------------------------------------------------------
+# the rasteriser's discrete decisions (rasterize(record=...)) and the pixels where they are stable
+# ---------------------------------------------------------------------------------------------
+# An fp32 kernel and the fp64 oracle agree to rounding only where both take the same discrete decisions.  stable_pixels
+# keeps the pixels where the fp32 and fp64 oracle runs take identical decisions AND every decision is further from its
+# switch point than the margins below, so that the kernel (whose soft-path and shading arithmetic is not rounding-exact)
+# takes them too.  The face-index buffer is left out of the margins: the kernel reproduces the fp32 oracle's bit for bit.
+#   EDGE_TIE_REL  closest edge: the next edge with a different closest point is further by more than this factor of
+#                 d^2 + EDGE_TIE_SCALE * multiplier * d.  rx, ry are differences of coordinates up to ~multiplier,
+#                 rounded to ~1e-7 multiplier in fp32, so d^2 carries ~2.4e-7 * multiplier * d: the second term keeps
+#                 the margin ~8x that rounding for pixels close to the edge, the first is 1e-4 relative far from it.
+#                 Two edges that both clamp to their shared vertex have the same closest point and the same adjoint,
+#                 so that tie is not a decision.
+#   T_MARGIN      segment clamp: the arg-min edge's unclamped foot parameter t is this far from 0 and from 1.
+#   TEXEL_MARGIN  texel floor (bilinear, bicubic) or round (nearest): the fractional texel coordinate is this far from
+#                 0 and 1, or from 0.5; u, v carry ~1 ulp and textures here are < 300 texels, i.e. < 2e-5 texel.
+#   BOX_MARGIN    expanded-box tests, in multiplier units: pixel centres and box bounds (|x| <~ 1) round to ~1e-7.
+#   PK_MAX        the soft-silhouette clamp p_k < 1 - 1e-7: p_k stays below this; 1 - p_k then keeps >= 3 significant
+#                 digits in fp32.
+EDGE_TIE_REL = 1e-4
+EDGE_TIE_SCALE = 0.02
+T_MARGIN = 1e-4
+TEXEL_MARGIN = 1e-4
+BOX_MARGIN = 1e-6
+PK_MAX = 1 - 1e-4
+_SIG_MOD, _SIG_MUL = 2147483647, 1000003
+
+
+class _Record:
+    """Per-pixel decisions of one rasterize call.  Filled face by face by the soft-silhouette loop; `finish` returns:
+      imidx      [B,H,W] the coverage / depth winner (face + 1)
+      soft_n     [B,H,W] faces that shaped the soft silhouette (<= knum), cand [B,H,W] faces whose expanded box holds
+                 the uncovered pixel (cand > soft_n: knum cut the list)
+      soft_sig   [B,H,W] hash of the ordered (face, closest point) list
+      edge_gap   [B,H,W] min over those faces of (d2 of the next edge with another closest point - d2)
+                 / (d2 + EDGE_TIE_SCALE * multiplier * d)
+      t_gap      [B,H,W] min over those faces of the arg-min edge's distance of unclamped t from {0, 1}
+      box_gap    [B,H,W] min over the faces tested before the knum cap of the distance (multiplier units) of the
+                 expanded-box decision from its switch point
+      pk_max     [B,H,W] max p_k over those faces
+      soft       list of (b, f, r0, c0, use [h,w], edge [h,w], gap [h,w], t [h,w]) per face window, in face order
+      tiles      {(b, ty, tx): [faces whose expanded box holds a pixel of the 16x16 tile, in face order]}"""
+
+    def __init__(self, B, H, W, dev, multiplier, knum):
+        z = dict(device=dev)
+        self.m, self.knum = float(multiplier), knum
+        inf = float("inf")
+        self.cand = torch.zeros(B, H, W, dtype=torch.int32, **z)
+        self.sig = torch.zeros(B, H, W, dtype=torch.int64, **z)
+        self.edge_gap = torch.full((B, H, W), inf, dtype=torch.float64, **z)
+        self.t_gap = torch.full((B, H, W), inf, dtype=torch.float64, **z)
+        self.box_gap = torch.full((B, H, W), inf, dtype=torch.float64, **z)
+        self.pk_max = torch.zeros(B, H, W, dtype=torch.float64, **z)
+        self.soft, self.tiles = [], {}
+
+    def face(self, b, f, r0, r1, c0, c1, xs, ys, a, bounds, near, use, consider, covered, delta):
+        shape = (r1 - r0, c1 - c0)
+        xs, ys = xs.expand(shape), ys.expand(shape)
+        win = (b, slice(r0, r1), slice(c0, c1))
+        rc = near.nonzero()
+        for ty, tx in torch.unique(torch.stack([(rc[:, 0] + r0) // 16, (rc[:, 1] + c0) // 16], 1), dim=0).tolist():
+            self.tiles.setdefault((b, ty, tx), []).append(f)
+        self.cand[win] += (near & ~covered).to(torch.int32)
+        # expanded box: all four tests pass -> the nearest bound decides; else all failing tests must flip
+        lo_x, hi_x, lo_y, hi_y = bounds
+        s = torch.stack([(xs - lo_x).abs(), (hi_x - xs).abs(), (ys - lo_y).abs(), (hi_y - ys).abs()]).double()
+        ok = torch.stack([xs >= lo_x, xs < hi_x, ys >= lo_y, ys < hi_y])
+        gap = torch.where(near, s.min(0).values, torch.where(ok, torch.zeros_like(s), s).max(0).values) / self.m
+        self.box_gap[win] = torch.minimum(self.box_gap[win], torch.where(consider, gap, torch.full_like(gap, math.inf)))
+        if not bool(use.any()):
+            return
+        d2s, ts, feats = [], [], []
+        for k in range(3):
+            k1 = (k + 1) % 3
+            ax, ay, bx, by = a[2 * k], a[2 * k + 1], a[2 * k1], a[2 * k1 + 1]
+            ex, ey = bx - ax, by - ay
+            traw = ((xs - ax) * ex + (ys - ay) * ey) / (ex * ex + ey * ey + SEG_EPS)
+            tc = traw.clamp(0, 1)
+            d2s.append(_seg_dist2(xs, ys, ax, ay, bx, by))
+            ts.append(traw)
+            # closest point: interior of edge k (k), or vertex k / k+1 (3 + vertex) where t clamps
+            feats.append(torch.where(tc <= 0, 3 + k, torch.where(tc >= 1, 3 + k1, k)))
+        d2, t, feat = torch.stack(d2s), torch.stack(ts), torch.stack(feats)
+        e = torch.zeros(shape, dtype=torch.long, device=xs.device)
+        dm = d2[0]
+        for k in (1, 2):                               # the kernel's arg-min: strict <, first edge wins ties
+            less = d2[k] < dm
+            e, dm = torch.where(less, k, e), torch.where(less, d2[k], dm)
+        fe = feat.gather(0, e.unsqueeze(0))[0]
+        second = torch.where(feat != fe, d2, torch.full_like(d2, math.inf)).min(0).values
+        dmd = dm.double()
+        scale = dmd + EDGE_TIE_SCALE * self.m * dmd.sqrt()
+        egap = torch.where(dmd > 0, (second.double() - dmd) / scale.clamp_min(1e-300), torch.zeros_like(dmd))
+        te = t.gather(0, e.unsqueeze(0))[0].double()
+        tgap = torch.minimum(te.abs(), (te - 1).abs())
+        pk = torch.exp(-delta * dmd / (self.m * self.m))
+        inf = torch.full_like(egap, math.inf)
+        self.edge_gap[win] = torch.minimum(self.edge_gap[win], torch.where(use, egap, inf))
+        self.t_gap[win] = torch.minimum(self.t_gap[win], torch.where(use, tgap, inf))
+        self.pk_max[win] = torch.maximum(self.pk_max[win], torch.where(use, pk, torch.zeros_like(pk)))
+        code = f * 8 + fe + 1
+        self.sig[win] = torch.where(use, (self.sig[win] * _SIG_MUL + code) % _SIG_MOD, self.sig[win])
+        self.soft.append((b, f, r0, c0, use, e, egap, te))
+
+    def finish(self, imidx, count):
+        return dict(imidx=imidx.clone(), soft_n=count.clone(), cand=self.cand, soft_sig=self.sig,
+                    edge_gap=self.edge_gap, t_gap=self.t_gap, box_gap=self.box_gap, pk_max=self.pk_max,
+                    soft=self.soft, tiles=self.tiles, multiplier=self.m, knum=self.knum)
+
+
+def pixel_faces(rec, b, y, x):
+    """The ordered soft-silhouette list of one pixel: [(face, arg-min edge, edge gap, unclamped t)]."""
+    out = []
+    for bb, f, r0, c0, use, e, gap, t in rec["soft"]:
+        r, c = y - r0, x - c0
+        if bb == b and 0 <= r < use.shape[0] and 0 <= c < use.shape[1] and bool(use[r, c]):
+            out.append((f, int(e[r, c]), float(gap[r, c]), float(t[r, c])))
+    return out
+
+
+def texel_coords(uv, Th, Tw, filtering):
+    """Unnormalised texel coordinates (ix, iy) at which the shader samples (u, v): grid_sample's with the shader's
+    (u * 2 - 1, -(v * 2 - 1)) grid, align_corners=True for bilinear, False for nearest / bicubic."""
+    gx, gy = uv[..., 0] * 2 - 1, -(uv[..., 1] * 2 - 1)
+    if filtering == "bilinear":
+        return (gx + 1) / 2 * (Tw - 1), (gy + 1) / 2 * (Th - 1)
+    return (gx + 1) * (Tw / 2) - 0.5, (gy + 1) * (Th / 2) - 0.5
+
+
+def stable_pixels(rec32, rec64, uv32=None, uv64=None, tex_hw=None, filtering="bilinear"):
+    """[B,H,W] bool: pixels whose every decision is identical in the fp32 and fp64 records and further than the
+    margins above from its switch point.  uv32 / uv64 [B,H,W,2] (the interpolated texture coordinates of each run) and
+    tex_hw = (Th, Tw) add the texel decisions of `filtering` on covered pixels."""
+    ok = (rec32["imidx"] == rec64["imidx"]) & (rec32["soft_n"] == rec64["soft_n"]) & \
+         (rec32["soft_sig"] == rec64["soft_sig"])
+    for r in (rec32, rec64):
+        ok &= (r["edge_gap"] > EDGE_TIE_REL) & (r["t_gap"] > T_MARGIN) & (r["box_gap"] > BOX_MARGIN) & \
+              (r["pk_max"] < PK_MAX)
+    if uv32 is not None:
+        Th, Tw = tex_hw
+        cov = rec32["imidx"] > 0
+        fl = []
+        for uv in (uv32, uv64):                     # each run's coordinates in its own precision
+            for c in texel_coords(uv.detach(), Th, Tw, filtering):
+                fr = (c - c.floor()).double()
+                near = (fr - 0.5).abs() < TEXEL_MARGIN if filtering == "nearest" else \
+                    (fr < TEXEL_MARGIN) | (fr > 1 - TEXEL_MARGIN)
+                ok &= ~(cov & near)
+                fl.append(c.floor().double())
+        ok &= ~cov | ((fl[0] == fl[2]) & (fl[1] == fl[3]))
+    return ok
+
+
+def bin_faces(p2d, H, W, expand=EXPAND, multiplier=MULTIPLIER, tile=16):
+    """The CUDA rasteriser's per-tile face lists restated in fp32: -> pos [B, ceil(H/tile), ceil(W/tile), F] int64, the
+    face's position in the tile's list (faces in face order whose expanded bounding box reaches the tile's pixel
+    centres), -1 where the face is not listed."""
+    f32 = torch.float32
+    P = p2d.detach().to(f32) * float(multiplier)
+    E = torch.tensor(float(expand) * float(multiplier), dtype=f32)
+    X, Y = P[..., 0::2], P[..., 1::2]
+    lo_x, hi_x = X.min(-1).values - E, X.max(-1).values + E
+    lo_y, hi_y = Y.min(-1).values - E, Y.max(-1).values + E
+    sx = torch.tensor(float(multiplier), dtype=f32) / torch.tensor(float(W), dtype=f32)
+    sy = torch.tensor(float(multiplier), dtype=f32) / torch.tensor(float(H), dtype=f32)
+    tx0 = torch.arange(0, W, tile)
+    ty0 = torch.arange(0, H, tile)
+    cx = lambda x: sx * (2 * x + 1 - W).to(f32)
+    cy = lambda y: sy * (H - 2 * y - 1).to(f32)
+    x_lo, x_hi = cx(tx0), cx((tx0 + tile - 1).clamp(max=W - 1))
+    y_lo, y_hi = cy((ty0 + tile - 1).clamp(max=H - 1)), cy(ty0)
+    flag = (lo_x[:, None, None, :] <= x_hi[None, None, :, None]) & (x_lo[None, None, :, None] < hi_x[:, None, None, :]) \
+        & (lo_y[:, None, None, :] <= y_hi[None, :, None, None]) & (y_lo[None, :, None, None] < hi_y[:, None, None, :])
+    pos = flag.long().cumsum(-1) - 1
+    return torch.where(flag, pos, torch.full_like(pos, -1))
 
 
 def texinterpolation(uv, texture):
